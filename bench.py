@@ -1,20 +1,21 @@
 #!/usr/bin/env python
-"""bench.py — top-k queries/sec of the brute-force scan on B200 (BASELINE.json metric).
+"""bench.py — top-k queries/sec of the brute-force scan on H100 (BASELINE.json metric).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config c2|c4]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Default workload (BASELINE.json configs[1], "c2"): vector_quantize_scan, int8 quantized from a synthetic N(0,1) f32
 10M x 384 corpus with the reference's S8 rule, L2 (the default metric), k=20, batch=1.  A "step" is one query scanned against
-the whole resident corpus (3.84 GB >> 126 MB L2, so every step streams from HBM).  The K steps are repeated until the timed
-region lasts >= --min-ms (default 50 ms: at 8 GPUs 20 steps would be a 2 ms sample); `steps_timed` says how many ran.
+the whole resident corpus (3.84 GB >> 50 MB L2, so every step streams from HBM).  Exactly --steps steps are timed, after
+--warmup untimed ones; `--dump-outputs DIR` writes what the last timed step returned (top-k rowids and distances) as .npy files.
 
 Our arm prints `value` (queries already in HBM; launch -> candidates -> exact top-k on the host, per query), `e2e` (HOST query
 in, host top-k out through the C ABI call the SQLite plugin makes, vsb_scan_topk, one at a time; the pipelined
 submit/collect figure beside it; sharded runs: the peer-memory exchange fed with host queries), the batch=1024 half of the
 metric (`batched`, tensor-core path, with its own roofline and parity sample), a f32 single-query roofline, the same
 statements through SQL for both extensions (`sql_e2e`) and the reference's CPU scan beside it (`cpu_baseline`).
-`--config c4` runs BASELINE configs[3] (uint8 cosine dim 1536 n=50M k=100 batch=256, row-sharded over the ranks).
+`--config c4` runs BASELINE configs[3] (uint8 cosine dim 1536 k=100 batch=256, row-sharded over the ranks; 25M rows by default,
+38 GB, so that one 80 GB H100 holds the column).
 `--impl reference` times the reference's own CPU scan (oracle/_ref built from the unmodified sources with -mavx2 -mfma;
 falls back to the oracle port) on all host cores.  One JSON line on stdout (rank 0).
 """
@@ -222,17 +223,20 @@ def emit(obj):
 
 
 def peaks():
+    """the denominators of the rooflines (HBM GB/s, dense bf16 TFLOP/s): MEASURED_PEAKS.json beside this file when the machine
+    provides one, else NVIDIA's data-sheet figures for the H100 SXM at 700 W.  A card set to a lower power limit reaches less;
+    `clocks` in the output says what this one ran at."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm": float(d["hbm_gbs"]), "bf16": float(d["bf16_tflops"]), "bf16_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm": 6650.0, "bf16": 1590.0, "bf16_sustained": 1590.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm": 3350.0, "bf16": 989.0, "bf16_sustained": 989.0, "source": "H100 SXM data sheet (700 W; dense bf16), not measured"}
 
 
 def measure_int8_peak(torch, device):
     """dense int8 tensor throughput of this GPU through the library GEMM (torch._int_mm -> cuBLASLt), 8192^3, best of 5:
-    the denominator of the int8 batched roofline (MEASURED_PEAKS.json has no int8 figure)"""
+    the denominator of the int8 batched roofline"""
     try:
         n = 8192
         a = torch.randint(-8, 8, (n, n), device=device, dtype=torch.int8)
@@ -253,16 +257,11 @@ def measure_int8_peak(torch, device):
         return None, f"unavailable ({ex})"
 
 
-def ncu_fact(pattern: str, key: str):
-    """a figure from the newest committed ncu summary that has it (profiles/*<pattern>*.json)"""
-    for p in sorted(glob.glob(os.path.join(ROOT, "profiles", f"*{pattern}*.json")), reverse=True):
-        try:
-            d = json.load(open(p))
-        except (OSError, ValueError):
-            continue
-        if isinstance(d, dict) and d.get(key) is not None:
-            return d[key], os.path.relpath(p, ROOT)
-    return None, None
+def dump_outputs(out_dir: str, **arrays):
+    """the result arrays of the last timed step as DIR/<name>.npy, float64 (rowids < 2^53 stay exact)"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(arr, dtype=np.float64))
 
 
 # ------------------------------------------------------------------ main
@@ -270,14 +269,17 @@ def main():
     claim_stdout()
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=400)
+    ap.add_argument("--steps", type=int, default=400,
+                    help="timed steps of the GPU arms (exactly this many); --impl reference stops early when its 150 s budget is spent "
+                         "and says so in `clamp`")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="c2", choices=["c2", "c4"], help="c2: BASELINE configs[1] (the metric's config); c4: configs[3]")
     ap.add_argument("--n", "--rows", dest="n", type=int, default=0, help="corpus rows (--rows: torchrun's own parser rejects a bare --n as ambiguous)")
     ap.add_argument("--dim", type=int, default=0)
     ap.add_argument("--k", type=int, default=0)
-    ap.add_argument("--min-ms", type=float, default=50.0, help="repeat the K steps until the timed region lasts at least this long")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the top-k rowids and distances of the last timed step to DIR/<name>.npy (float64)")
     ap.add_argument("--cpu-threads", type=int, default=0, help="threads of the CPU reference leg (0 = all cores)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-batched", action="store_true", help="skip the batch=1024 tensor-core legs")
@@ -300,7 +302,7 @@ def main():
     if a.config == "c4":
         if a.impl == "reference":
             if rank == 0:
-                emit({"impl": "reference", "unavailable": "config c4 has no CPU arm: one batch is ~1.7 h of the reference's AVX2 scan (BASELINE.md section 2)"})
+                emit({"impl": "reference", "unavailable": "config c4 has no CPU arm: one batch is ~0.85 h of the reference's AVX2 scan at 25M rows (BASELINE.md section 2)"})
             return 0
         return run_c4(torch, a, rank, local_rank, world)
 
@@ -421,18 +423,6 @@ def main():
         run_single(0, max(W, 1))
     else:
         run_sharded(0, max(W, 1), True)
-    # how many times the K steps must repeat for the timed region to last >= min_ms (same decision on every rank)
-    barrier()
-    t_probe = time.perf_counter()
-    (run_single if world == 1 else (lambda f, c: run_sharded(f, c, True)))(0, min(K, 4 * G if world > 1 else 16))
-    barrier()
-    est_ms = (time.perf_counter() - t_probe) * 1e3 / min(K, 4 * G if world > 1 else 16)
-    reps = max(1, int(np.ceil(a.min_ms / max(est_ms * K, 1e-6))))
-    if world > 1:
-        t = torch.tensor([reps], device=device)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        reps = int(t.item())
-    KT = K * reps
     if sampler:
         sampler.wait_first(2.0)
     barrier()
@@ -442,12 +432,14 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     t_wall0 = time.perf_counter()
     e0.record(st)
-    last, last_qi = run_single(W, KT) if world == 1 else run_sharded(W, KT, True)
+    last, last_qi = run_single(W, K) if world == 1 else run_sharded(W, K, True)
     e1.record(st)
     barrier()
     t_wall = time.perf_counter() - t_wall0
     ms_dev = e0.elapsed_time(e1)
     launches = eng.kernel_launches() - l0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, topk_rowids=last[0], topk_distances=last[1])
     # the step time is the slower of the device-event span and the wall clock around the same region
     ms_total = max(ms_dev, t_wall * 1e3) if world > 1 else ms_dev
     if world > 1:
@@ -493,26 +485,26 @@ def main():
         # (a) THE call the SQLite plugin makes from xFilter (vsb_scan_topk), one query at a time: pinned H2D of the query + scan +
         #     filter + D2H of the candidate head + host slot replay, nothing overlapped across queries.  This is e2e.value.
         t0 = time.perf_counter()
-        for i in range(KT):
+        for i in range(K):
             last_e2e = ix.scan_topk(api.L2, q_host[W + (i % (NQ - W - 1))], k)[0]
         e2e_s = time.perf_counter() - t0
-        e2e_qi = W + ((KT - 1) % (NQ - W - 1))
+        e2e_qi = W + ((K - 1) % (NQ - W - 1))
         # (b) the asynchronous pair vsb_scan_submit(host query) / vsb_collect, two queries in flight (what a batching caller gets)
         t0 = time.perf_counter()
         pending = None
-        for i in range(KT):
+        for i in range(K):
             slot = ix.scan_submit(api.L2, q_host[W + (i % (NQ - W - 1))], k, on_device=False, fetch=True)
             if pending is not None:
                 ix.collect(pending, k)
             pending = slot
         ix.collect(pending, k)
-        pipelined_qps = KT / (time.perf_counter() - t0)
+        pipelined_qps = K / (time.perf_counter() - t0)
         avg_surv = (ix.stat("survivors") - surv0) / max(ix.stat("queries") - q0, 1)
     else:
         run_sharded(0, max(W, 1), False)
         barrier()
         t0 = time.perf_counter()
-        last_e2e, e2e_qi = run_sharded(W, KT, False)
+        last_e2e, e2e_qi = run_sharded(W, K, False)
         barrier()
         e2e_s = time.perf_counter() - t0
         t = torch.tensor([e2e_s], device=device)
@@ -560,9 +552,9 @@ def main():
                 batched_sharded = {"workload": f"vector_quantize_scan int8 dim={dim} n={n} k={k} batch={B} L2, {world} row shards",
                                    "queries_per_s": B / dtb, "ms_per_batch": dtb * 1e3, "batch": B,
                                    "end_to_end_tflops": 2.0 * dim * B * n / dtb / 1e12,
-                                   "path": ("per shard: tcgen05 scoring + exact refine + slot replay with entry logs; the log blocks are pushed into every peer's log area over NVLink "
+                                   "path": ("per shard: wgmma scoring + exact refine + slot replay with entry logs; the log blocks are pushed into every peer's log area over NVLink "
                                             "(push_logs_kernel), device-side flag wait, GPU merge replay; two batches in flight, one host wait per batch" if use_peer else
-                                            "per shard: tcgen05 scoring + exact refine + slot replay with entry logs; NCCL all-gather of the logs; GPU merge replay"),
+                                            "per shard: wgmma scoring + exact refine + slot replay with entry logs; NCCL all-gather of the logs; GPU merge replay"),
                                    "_result": rb}
         except Exception as ex:  # never lose the headline line
             batched_sharded = {"error": str(ex)}
@@ -605,7 +597,7 @@ def main():
                                 "queries_per_s": world * B / dtb, "ms_per_global_batch": dtb * 1e3, "batch_per_gpu": B, "global_batch": world * B,
                                 "queries_per_s_results_on_every_rank": world * B / dtg,
                                 "scaling": "weak in queries (each GPU answers its own 1024 of the global batch over the whole column)",
-                                "path": "shard.query_sharded_batch_topk: vsb_scan_topk (tcgen05 batch path) on this rank's query slice, host queries in, host top-k out; "
+                                "path": "shard.query_sharded_batch_topk: vsb_scan_topk (wgmma batch path) on this rank's query slice, host queries in, host top-k out; "
                                         "no exchange on the data path; queries_per_s_results_on_every_rank adds one NCCL all-gather of the results",
                                 "_result": (rid, rdd, rcn, q_glob[qlo:qhi])}
         except Exception as ex:  # never lose the headline line
@@ -618,39 +610,37 @@ def main():
     # ---- roofline of the dominant kernel (scan_kernel): algorithmic bytes = rows * dim * 1 B per launch
     pk = peaks()
     shard_bytes = (hi - lo) * dim
-    step_ms = ms_total / KT
+    step_ms = ms_total / K
     achieved = shard_bytes / (step_ms * 1e-3) / 1e9
-    traffic, traffic_src = (ncu_fact("scan_kernel_traffic", "dram_bytes_per_launch") if (world == 1 and n == 10_000_000 and dim == 384) else (None, None))
 
     out = {
-        "metric": METRIC_NAME, "value": KT / (ms_total * 1e-3), "unit": "queries/s", "n_gpus": world, "steps": K, "warmup": W,
-        "steps_timed": KT, "ms_per_step": step_ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "int8",
+        "metric": METRIC_NAME, "value": K / (ms_total * 1e-3), "unit": "queries/s", "n_gpus": world, "steps": K, "warmup": W,
+        "steps_timed": K, "ms_per_step": step_ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "int8",
         "data": "synthetic N(0,1) f32 (seed 1234) quantized to int8 with the reference S8 rule; queries seed 4321",
         "config": {"workload": workload, "metric": "L2", "k": k, "batch": 1, "rows": n, "dim": dim, "shards": world,
-                   "l2_flush": "none needed: each step streams the whole shard (%.2f GB) which exceeds the 126 MB L2" % (shard_bytes / 1e9),
+                   "l2_flush": "none needed: each step streams the whole shard (%.2f GB) which exceeds the 50 MB L2" % (shard_bytes / 1e9),
                    "result_mode": "exact reference slot replay (bit-exact rowids/order/distances vs distance-cpu.c)",
-                   "timed_region": f"the {K} steps repeated {reps}x back to back so that the region lasts >= {a.min_ms:.0f} ms",
+                   "timed_region": f"{K} steps back to back",
                    "in_flight": 2 if world == 1 else depth * G,
                    "exchange": None if world == 1 else (
                        f"groups of {G} independent queries, {depth} groups in flight; every filter kernel stores its result head into every peer's gather buffer over NVLink "
                        "(cudaIpc peer memory) and raises a flag; the receiver waits on the flags on its own stream, one D2H per group, host slot replay (no collective library on the data path)"
                        if a.exchange == "peer" else f"groups of {G} queries: one NCCL all-gather of the shards' result heads + one D2H per group")},
-        "e2e": {"value": KT / e2e_s, "unit": "queries/s", "h2d_bytes_per_step": int(pitch),
+        "e2e": {"value": K / e2e_s, "unit": "queries/s", "h2d_bytes_per_step": int(pitch),
                 "d2h_bytes_per_step": d2h_bytes, "avg_candidates_per_query": avg_surv, "pipelined_value": pipelined_qps,
                 "note": ("value = the synchronous vsb_scan_topk call the SQLite plugin makes from xFilter, one query at a time (pinned H2D of the query, scan + filter kernels, "
                          "one D2H of the candidate head, host slot replay); pipelined_value = vsb_scan_submit(host query)/vsb_collect with two queries in flight"
                          if world == 1 else
                          "vsb_exchange_submit with HOST queries (pinned H2D per query) + scan/filter kernels on every rank + peer-memory push of the heads + D2H + host slot replay, same grouping as value")},
         "gpu_launches": int(launches),
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": pk["hbm"], "unit": "GB/s", "frac": achieved / pk["hbm"], "traffic": traffic,
-                     "traffic_source": traffic_src, "kernel": "vsb::scan_kernel<int8,L2>", "avg_launch_ms": step_ms, "launches_timed": KT,
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": pk["hbm"], "unit": "GB/s", "frac": achieved / pk["hbm"], "kernel": "vsb::scan_kernel<int8,L2>", "avg_launch_ms": step_ms, "launches_timed": K,
                      "kernel_alone_ms": alone_ms, "kernel_alone_gbs": (shard_bytes / (alone_ms * 1e-3) / 1e9) if alone_ms else None,
                      "filter_kernel_alone_ms": filter_ms, "peak_source": pk["source"] + " hbm_gbs",
                      "algorithmic_bytes_per_launch": int(shard_bytes),
                      "note": "consecutive scan launches alternate between two streams and overlap at CTA granularity (an SM starts the next query's CTA when its CTA of the "
                              "current one exits), so per-launch events would double count: avg_launch_ms is the device-timed span of the timed region / launches, i.e. achieved is "
-                             "the WHOLE-STEP rate (filter, copies and host replay included); kernel_alone_* is one launch at a time on one stream. peak is the measured COPY bandwidth "
-                             "(reads + writes); this kernel only reads, so frac can exceed 1.0"},
+                             "the WHOLE-STEP rate (filter, copies and host replay included); kernel_alone_* is one launch at a time on one stream. peak_source says whether peak is "
+                             "measured or the H100 SXM data sheet"},
         "clocks": clocks,
         "wall_s_timed_region": t_wall,
         "single_query_latency_ms": lat_ms,
@@ -728,14 +718,12 @@ def main():
 
 
 def batched_legs(torch, vs, api, eng, ix, q_host, buf, n, dim, k, device, pk):
-    """batch=1024 through vsb_scan_topk (host queries in, host top-k out): tcgen05 scoring + exact refinement.  First-class
+    """batch=1024 through vsb_scan_topk (host queries in, host top-k out): wgmma scoring + exact refinement.  First-class
     half of the BASELINE metric: each leg carries its own tensor roofline (tc_scan_kernel device time from the engine's CUDA
     events, peak measured) and a parity sample against the reference / oracle on the same data."""
     from oracle import pyoracle as po
     res = {}
     int8_peak, int8_note = measure_int8_peak(torch, device)
-    pct_i8, src_i8 = ncu_fact("ncu_summary", "tc_int8_tensor_pipe_pct")
-    pct_bf, src_bf = ncu_fact("ncu_summary", "tc_bf16_tensor_pipe_pct")
 
     def run(name, index, queries, metric, flop_per_pair, peak, peak_note, parity):
         B = queries.shape[0]
@@ -767,8 +755,6 @@ def batched_legs(torch, vs, api, eng, ix, q_host, buf, n, dim, k, device, pk):
         return {"queries_checked": [0, 257, 1023], "gpu_result_matches_reference": all(ok), "checked_against": how, "rule": "bit-exact rowids, order, distances"}
 
     run("int8_L2_dim%d_n%d_b1024" % (dim, n), ix, q_host[:1024], api.L2, 2.0 * dim, int8_peak, int8_note, parity_int8)
-    res["int8_L2_dim%d_n%d_b1024" % (dim, n)]["roofline"]["tensor_pipe_pct_ncu"] = pct_i8
-    res["int8_L2_dim%d_n%d_b1024" % (dim, n)]["roofline"]["tensor_pipe_pct_source"] = src_i8
 
     # BASELINE configs[2]: vector_full_scan dot bf16 dim=768 n=10M k=20 batch=1024
     n3, d3 = 10_000_000, 768
@@ -814,11 +800,9 @@ def batched_legs(torch, vs, api, eng, ix, q_host, buf, n, dim, k, device, pk):
                 "rule": "distances within 1e-5 relative, rowids equal except oracle near-ties (tests/fpcheck.py)", "max_rel_err": worst,
                 "queries_equal_to_single_query_path": f"{same}/64"}
 
-    run("bf16_DOT_dim768_n10M_b1024", ix3, q3, api.DOT, 2.0 * d3, pk["bf16"], "measured cuBLAS bf16 burst peak (MEASURED_PEAKS.json bf16_tflops)", parity_bf16)
+    run("bf16_DOT_dim768_n10M_b1024", ix3, q3, api.DOT, 2.0 * d3, pk["bf16"], pk["source"], parity_bf16)
     res["bf16_DOT_dim768_n10M_b1024"]["roofline"]["frac_of_sustained_peak"] = (
         res["bf16_DOT_dim768_n10M_b1024"]["roofline"]["achieved"] / pk["bf16_sustained"] if res["bf16_DOT_dim768_n10M_b1024"]["roofline"]["achieved"] else None)
-    res["bf16_DOT_dim768_n10M_b1024"]["roofline"]["tensor_pipe_pct_ncu"] = pct_bf
-    res["bf16_DOT_dim768_n10M_b1024"]["roofline"]["tensor_pipe_pct_source"] = src_bf
     ix3.close()
     return res
 
@@ -878,14 +862,14 @@ def sql_e2e_leg(n=200_000, queries=30):
 
 # ------------------------------------------------------------------ BASELINE configs[3]
 def run_c4(torch, a, rank, local_rank, world):
-    """vector_quantize_scan cosine uint8 dim=1536 n=50M k=100 batch=256, row-sharded over the ranks (8 x B200 in BASELINE.json;
-    the whole column also fits ONE B200).  A step is one batch of 256 queries; value = queries/s."""
+    """vector_quantize_scan cosine uint8 dim=1536 n=25M k=100 batch=256, row-sharded over the ranks (the 38 GB column fits one
+    80 GB H100 with the batch workspace beside it).  A step is one batch of 256 queries; value = queries/s."""
     import torch.distributed as dist
 
     import sqlite_vector_b200 as vs
     from sqlite_vector_b200 import api, shard
-    n, dim, k, B = a.n or 50_000_000, a.dim or 1536, a.k or 100, 256
-    K, W = max(min(a.steps, 20), 1), max(a.warmup, 1)
+    n, dim, k, B = a.n or 25_000_000, a.dim or 1536, a.k or 100, 256
+    K, W = max(a.steps, 1), max(a.warmup, 1)
     torch.cuda.set_device(local_rank)
     device = torch.device("cuda", local_rank)
     if world > 1:
@@ -958,6 +942,8 @@ def run_c4(torch, a, rank, local_rank, world):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         dt = float(t.item())
     launches = eng.kernel_launches() - l0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, topk_rowids=rb[0], topk_distances=rb[1], topk_counts=rb[2])
     tc_s = (ix.stat("tc_us") - us0) / K * 1e-6
     tc_rows = (ix.stat("tc_rows") - rows0) / K
     clocks = sampler.stop() if sampler else None
@@ -981,12 +967,12 @@ def run_c4(torch, a, rank, local_rank, world):
     pk = peaks()
     int8_peak, int8_note = measure_int8_peak(torch, device)
     ops = 2.0 * B * tc_rows * dim
-    out = {"metric": "top-k queries/sec, vector_quantize_scan cosine uint8 dim=1536 n=50M k=100 batch=256 (BASELINE configs[3])",
+    out = {"metric": f"top-k queries/sec, vector_quantize_scan cosine uint8 dim={dim} n={n} k={k} batch={B} (BASELINE configs[3])",
            "value": B * K / dt, "unit": "queries/s", "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": dt / K * 1e3,
            "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "u8", "data": "synthetic |N(0,1)|*48 rounded to uint8 (seed 1234); queries seed 4321",
            "config": {"workload": f"vector_quantize_scan cosine uint8 dim={dim} n={n} k={k} batch={B}", "shards": world, "rows_per_shard": hi - lo,
                       "l2_flush": "none needed: every batch streams the whole shard (%.1f GB)" % ((hi - lo) * dim / 1e9),
-                      "path": "per shard: tcgen05 (kind::i8) scoring + exact refine + slot replay" + ("" if world == 1 else (" with entry logs; logs pushed over NVLink peer memory, device-side wait, GPU merge replay; two batches in flight" if exch is not None else " with entry logs; NCCL all-gather of the logs; GPU merge replay"))},
+                      "path": "per shard: wgmma (s8/u8) scoring + exact refine + slot replay" + ("" if world == 1 else (" with entry logs; logs pushed over NVLink peer memory, device-side wait, GPU merge replay; two batches in flight" if exch is not None else " with entry logs; NCCL all-gather of the logs; GPU merge replay"))},
            "e2e": {"value": B * K / dt, "unit": "queries/s", "h2d_bytes_per_step": int(q.nbytes), "d2h_bytes_per_step": int(B * 128 * 8),
                    "note": "host queries in, host top-k out: the timed call IS the public C-ABI call (vsb_scan_topk / vsb_batch_shard_scan + vsb_batch_merge)"},
            "gpu_launches": int(launches),

@@ -1,5 +1,5 @@
 /*
- * vsb200.h — C ABI of the B200 scan engine (libvsb200.so / vector.so).
+ * vsb200.h — C ABI of the H100 scan engine (libvsb200.so / vector.so).
  *
  * This is the drop-in boundary for sqlite-vector's brute-force scan path.  Every entry point
  * names the reference interface it replaces (file:line relative to sqliteai/sqlite-vector 0.9.23).
@@ -94,7 +94,7 @@ VSB_API void vsb_index_free(vsb_index *ix);
  * max_index (in/out, may be NULL, nq == 1 only): the cursor's slot index quirk (:1808-1813 never resets it).
  * nq > 1 has no counterpart in the reference (one vector per xFilter); each query then behaves like a fresh cursor.
  * For nq >= 16 on f16/bf16/int8/uint8 columns with L2/SQUARED_L2/COSINE/DOT the scores are computed on the tensor
- * cores (tcgen05) and refined exactly; results are the same as nq single calls. */
+ * cores (wgmma) and refined exactly; results are the same as nq single calls. */
 VSB_API int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k, int64_t *out_rowids,
                           double *out_dist, int *out_counts, int *max_index);
 

@@ -1,28 +1,30 @@
-// batch_kernels.cuh — batched-query path: tcgen05 tensor-core scoring + exact candidate refinement.
+// batch_kernels.cuh — batched-query path: wgmma tensor-core scoring + exact candidate refinement.
 //
 // For B queries against the resident shard the scores  S[row][q] = <row, query_q>  are a dense GEMM
 // (rows x dim) x (dim x B): this is the one place where the scan IS tensor-core work (north_star).
-// tc_scan_kernel computes S tile by tile with tcgen05.mma (A = 128 corpus rows, B = up to 256 queries, both K-major
-// in 128B-swizzled shared memory filled by TMA, accumulators in TMEM) and NEVER materialises S: the epilogue reads
-// the accumulators back with tcgen05.ld and only tests each score against a per-query bound, appending the rare
-// hits (row, query) to a candidate log.  The bound is conservative (it absorbs the tensor-core rounding), so the log
+// tc_scan_kernel computes S tile by tile with Hopper warpgroup MMAs (A = 128 corpus rows, B = up to 256 queries, both K-major
+// in 128B-swizzled shared memory filled by TMA, accumulators in registers) and NEVER materialises S: each consumer warpgroup
+// tests its 64 x N accumulators against a per-query bound straight from registers, appending the rare hits (row, query) to a
+// candidate log.  The bound is conservative (it absorbs the tensor-core rounding), so the log
 // is a superset of the rows whose EXACT reference distance beats the query's running k-th distance; the refinement
 // kernels below recompute those distances with exactly the arithmetic of the single-query kernel (accum16/finalize)
 // and replay the reference's slot algorithm (src/sqlite-vector.c:2022-2069, 2145-2152) per query, level by level.
 #pragma once
 #include <cuda.h>
 
+#include <type_traits>
+
 #include "scan_kernels.cuh"
+#include "wgmma.cuh"
 
 namespace vsb {
 
 enum { TK_BF16 = 0, TK_F16 = 1, TK_I8 = 2, TK_U8 = 3 };
-// warp 0: TMA, warp 1: MMA, warp 2: TMEM alloc, warps 4.. : epilogue.  EPI = 1: warps 4-7 (one per TMEM lane quadrant)
-// drain all N accumulator columns; EPI = 2: warps 4-7 take columns [0, N/2), warps 8-11 columns [N/2, N) — two epilogue
-// warps per SM sub-partition, which is what small-K tiles need (the tile is drain-bound, not MMA-bound).
-__host__ __device__ constexpr int tc_threads(int epi) { return 128 + 128 * epi; }
+// warps 0-7: two consumer warpgroups (rows 0-63 and 64-127 of the corpus tile), warp 8: TMA producer
+constexpr int kTcConsumers = 2;
+constexpr int kTcThreads = kTcConsumers * 128 + 32;
 constexpr int kTcMaxStages = 8;
-constexpr int kTcM = 128;           // corpus rows per MMA tile
+constexpr int kTcM = 128;           // corpus rows per tile
 constexpr int kTcKBytes = 128;      // one swizzle atom of K per stage
 
 struct TcParams {
@@ -34,6 +36,7 @@ struct TcParams {
     int KB;                 // 128-byte K blocks per row
     int nstages;            // ring depth (2..kTcMaxStages)
     int mc;                 // MC_L2 / MC_COS / MC_DOT
+    int chunk_test;         // integer kinds: test 32-column chunks before single scores (see tc_scan_kernel)
     float eps;              // fp kinds: relative slack of the tensor-core score, see tc_fp_eps
     const float *qc;        // [NG*N] per-query constant (float, or int bit pattern for the integer kinds)
     const void *norms;      // [n] float (fp kinds) or int (integer kinds): sum of squares of each row
@@ -42,7 +45,7 @@ struct TcParams {
     unsigned cand_cap;
 };
 
-// ------------------------------------------------------------------ PTX wrappers (tcgen05 / TMA)
+// ------------------------------------------------------------------ PTX wrappers (TMA / wgmma)
 __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
                      smem_u32(dst)),
@@ -52,72 +55,24 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, i
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// wait with back-off: the epilogue warps of an MMA-bound tile (long K) spend most of their time here, and 8 - 16 warps polling
-// an mbarrier in shared memory compete with the tensor core's operand reads and with the producer / MMA warps' issue slots
-// (config 4, dim 1536: 16 polling epilogue warps cost 40 % of the batch time, profiles/r02k)
-__device__ __forceinline__ void mbar_wait_backoff(uint64_t *bar, uint32_t parity) {
-    uint32_t done;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    while (!done) {
-        __nanosleep(128);
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    }
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-template <bool INT8>
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (INT8) {
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-                     "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-                     : "memory");
-    } else {
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-                     "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-                     : "memory");
-    }
-}
-// 32 lanes x 32 columns of 32-bit accumulators -> 32 registers per thread (lane = TMEM lane, i.e. corpus row)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
 
 // K-major operand tile in 128B-swizzled shared memory (rows of 128 bytes, 8-row groups 1024 B apart):
-// start address >> 4 | LBO = 1 | SBO = 1024 >> 4 | version 1 (Blackwell) | layout SWIZZLE_128B (2)   [cute/arch/mma_sm100_desc.hpp]
-__device__ __forceinline__ uint64_t umma_desc_sw128(const void *smem) {
+// start address >> 4 | LBO = 1 (unused with this swizzle) | SBO = 1024 >> 4 | layout SWIZZLE_128B (1 << 62)
+__device__ __forceinline__ uint64_t gmma_desc_sw128(const void *smem) {
     const uint64_t addr = (uint64_t)((smem_u32(smem) & 0x3FFFFu) >> 4);
-    return addr | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 46) | (uint64_t(2) << 61);
+    return addr | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
 }
-// instruction descriptor: D format bits [4,6), A/B formats [7,10)/[10,13), K-major both, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ inline uint32_t umma_idesc(int kind, int N) {
-    uint32_t cfmt, abfmt;
-    switch (kind) {
-    case TK_BF16: cfmt = 1; abfmt = 1; break;   // F32 accumulate, BF16 inputs
-    case TK_F16: cfmt = 1; abfmt = 0; break;    // F32 accumulate, F16 inputs
-    case TK_I8: cfmt = 2; abfmt = 1; break;     // S32 accumulate, signed 8-bit
-    default: cfmt = 2; abfmt = 0; break;        // S32 accumulate, unsigned 8-bit
-    }
-    return (cfmt << 4) | (abfmt << 7) | (abfmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(kTcM >> 4) << 24);
+
+template <int KIND, int N, class Acc>
+__device__ __forceinline__ void tc_mma(Acc (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+    if constexpr (KIND == TK_BF16) Wgmma<N>::bf16(d, a, b, scale_d);
+    else if constexpr (KIND == TK_F16) Wgmma<N>::f16(d, a, b, scale_d);
+    else if constexpr (KIND == TK_I8) Wgmma<N>::s8(d, a, b, scale_d);
+    else Wgmma<N>::u8(d, a, b, scale_d);
 }
 
 // the per-element candidate test.  fp kinds use negated comparisons so that NaN scores count as hits.
@@ -136,32 +91,7 @@ __device__ __forceinline__ bool tc_hit(uint32_t sbits, uint32_t qcbits, float ro
     }
 }
 
-// issue a 32-column TMEM load without waiting (pair with tmem_wait_ld)
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t *v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t *v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// one lane of the calling (converged) warp; the same lane every time, so that the thread that issues the tcgen05.mma's also
-// issues their tcgen05.commit's.  Keeping the producer / MMA warps in warp-uniform control flow and electing only around the
-// asynchronous instructions lets the compiler hold descriptors, coordinates and barrier addresses in uniform registers: inside
-// an `if (lane == 0)` region it has to assume divergence and wraps every UTMALDG / UTCIMMA in an ELECT + R2UR.BROADCAST loop,
-// which made the single issuing thread — not the tensor pipe — the pace setter of short (K = 384 B) tiles (profiles/r02c).
+// one lane of the calling (converged) warp; keeps the producer warp in warp-uniform control flow around the TMA issue
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xFFFFFFFF;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -169,8 +99,8 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 // Tile order: tile t = corpus-tile * NG + query-group, t = blockIdx.x, + gridDim.x, ...  (both operands streamed through the
-// stage ring; the 4 query groups of one corpus tile run on different CTAs at about the same time, so the corpus tile is read
-// from HBM once and from L2 three times).  Walked incrementally: no division per tile.
+// stage ring; the query groups of one corpus tile run on different CTAs at about the same time, so the corpus tile is read
+// from HBM once and from L2 by the others).  Walked incrementally: no division per tile.
 struct TileWalk {
     long long mt0;        // first corpus tile of the level
     uint32_t count;       // tiles this CTA processes
@@ -193,48 +123,40 @@ struct TileWalk {
     }
 };
 
-// CH: accumulator columns per epilogue step (64 = two 32-column TMEM loads in flight per buffer, 32 = one)
-// TEST: 0 = every score is compared with its query's bound (two dependent ALU ops per score);
-//       2 = chunk test (integer kinds, CH = 32; the default): the hit condition is monotone in the score, so a 32-column chunk
-//           can only contain a hit if  max_j s_ij  passes against the chunk's WEAKEST bound  min_j qc_j  (precomputed per chunk
-//           in shared memory).  The maximum costs 16 three-input VIMNMX per 32 scores instead of 64 dependent IADD3/ISETP, no
-//           per-column constants are loaded, and only chunks that pass (a few in 10^4 for queries of similar norm) run the
-//           per-column test that builds the exact hit masks.  The log is the same set of (row, query) pairs either way.
-template <int KIND, int MC, int EPI, int CH, int TEST = 0>
-__global__ void __launch_bounds__(tc_threads(EPI), 1) tc_scan_kernel(const __grid_constant__ CUtensorMap tmA,
+// Accumulator layout of one consumer warpgroup (m64nN, PTX ISA "wgmma register fragments"): thread t of the warpgroup holds
+// rows  ra = 16 * (t / 32) + (t % 32) / 4  and  ra + 8  of its 64 rows; d[4j + 0/1] are row ra, columns 8j + 2 (t % 4) + 0/1,
+// d[4j + 2/3] row ra + 8, the same columns.
+// chunk_test (integer kinds): the hit condition is monotone in the score, so the 8 scores a thread holds of one row in a
+// 32-column chunk can only contain a hit if their maximum passes against the chunk's WEAKEST bound (min over its 32 columns,
+// precomputed in shared memory).  Only chunks that pass run the per-column test; the log is the same set of (row, query)
+// pairs either way.
+template <int KIND, int MC, int N>
+__global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                 const __grid_constant__ CUtensorMap tmB, const TcParams prm) {
-    constexpr int NACC = 2;                                                    // accumulator buffers in TMEM (2 x N <= 512 columns)
     constexpr bool INT8 = (KIND == TK_I8 || KIND == TK_U8);
+    using Acc = typename std::conditional<INT8, uint32_t, float>::type;
     extern __shared__ __align__(1024) uint8_t tsm[];
-    const int N = prm.N, NS = prm.nstages;
-    const uint32_t a_bytes = kTcM * kTcKBytes, b_bytes = (uint32_t)N * kTcKBytes;
-    const uint32_t stage_bytes = a_bytes + b_bytes;
+    const int NS = prm.nstages;
+    constexpr uint32_t a_bytes = kTcM * kTcKBytes, b_bytes = (uint32_t)N * kTcKBytes;
+    constexpr uint32_t stage_bytes = a_bytes + b_bytes;
     uint8_t *stages = tsm;                                                     // [NS][A | B], 1024-aligned
     uint8_t *tail = tsm + (size_t)NS * stage_bytes;
     uint64_t *full = reinterpret_cast<uint64_t *>(tail);
     uint64_t *empty = full + kTcMaxStages;
-    uint64_t *tfull = empty + kTcMaxStages;                                    // [NACC] accumulator ready
-    uint64_t *tempty = tfull + NACC;                                           // [NACC] accumulator drained
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tempty + NACC + 2);
-    uint32_t *qc_s = tmem_slot + 4;                                            // [NG*N]
-    uint32_t *qcm_s = qc_s + prm.NG * prm.N;                                   // [NG*N/32] weakest bound of each 32-column chunk (TEST = 2)
+    uint32_t *qc_s = reinterpret_cast<uint32_t *>(empty + kTcMaxStages);      // [NG*N]
+    uint32_t *qcm_s = qc_s + prm.NG * N;                                       // [NG*N/32] weakest bound of each 32-column chunk
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t tmem_cols = (NACC * N <= 32) ? 32 : (NACC * N <= 64 ? 64 : (NACC * N <= 128 ? 128 : (NACC * N <= 256 ? 256 : 512)));
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < kTcMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < NACC; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4 * EPI); }
+        for (int i = 0; i < kTcMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kTcConsumers); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, tmem_cols);
-    constexpr bool kChunkTest = (TEST == 2) && INT8 && CH == 32;
-    for (int i = threadIdx.x; i < prm.NG * N; i += tc_threads(EPI)) qc_s[i] = __float_as_uint(prm.qc[i]);
-    tc_fence_before();
+    for (int i = threadIdx.x; i < prm.NG * N; i += kTcThreads) qc_s[i] = __float_as_uint(prm.qc[i]);
     __syncthreads();
-    tc_fence_after();
-    if constexpr (kChunkTest) {
-        for (int c = threadIdx.x; c < prm.NG * N / 32; c += tc_threads(EPI)) {
+    const bool chunk = INT8 && prm.chunk_test;
+    if (chunk) {
+        for (int c = threadIdx.x; c < prm.NG * N / 32; c += kTcThreads) {
             if constexpr (MC == MC_COS) {
                 float m = __uint_as_float(qc_s[c * 32]);
                 for (int j = 1; j < 32; ++j) m = fminf(m, __uint_as_float(qc_s[c * 32 + j]));
@@ -247,13 +169,12 @@ __global__ void __launch_bounds__(tc_threads(EPI), 1) tc_scan_kernel(const __gri
         }
         __syncthreads();
     }
-    const uint32_t tmem_base = *tmem_slot;
 
     TileWalk tw;
     tw.init(prm);
     const int KB = prm.KB;
 
-    if (warp == 0) {                                                           // ===== TMA producer: the whole warp walks, one lane issues
+    if (warp == kTcConsumers * 4) {                                            // ===== TMA producer: the whole warp walks, one lane issues
         int s = 0;
         uint32_t ph = 1;                                                       // parity to wait for on empty[s]: the first pass is free
         for (uint32_t tl = 0; tl < tw.count; ++tl, tw.next()) {
@@ -270,188 +191,124 @@ __global__ void __launch_bounds__(tc_threads(EPI), 1) tc_scan_kernel(const __gri
                 if (++s == NS) { s = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == 1) {                                                    // ===== MMA issuer: the whole warp walks, one lane issues
-        const uint32_t idesc = umma_idesc(KIND, N);
-        int s = 0;
-        uint32_t ph = 0;                                                       // parity to wait for on full[s]
-        uint32_t as = 0, aph = 1;                                              // accumulator buffer, parity to wait for on tempty[as]
-        for (uint32_t tl = 0; tl < tw.count; ++tl) {
-            mbar_wait(&tempty[as], aph);
-            tc_fence_after();
-            const uint32_t dcol = tmem_base + as * (uint32_t)N;
-            for (int kb = 0; kb < KB; ++kb) {
-                mbar_wait(&full[s], ph);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint8_t *st = stages + (size_t)s * stage_bytes;
-                    const uint64_t ad = umma_desc_sw128(st), bd = umma_desc_sw128(st + a_bytes);
-#pragma unroll
-                    for (int k4 = 0; k4 < kTcKBytes / 32; ++k4)                // UMMA_K = 32 bytes: advance the start address by 2 (x16 B)
-                        tc_mma<INT8>(dcol, ad + (uint64_t)(2 * k4), bd + (uint64_t)(2 * k4), idesc, (uint32_t)((kb | k4) != 0));
-                    tc_commit(&empty[s]);                                      // frees the smem stage when these MMAs retire
-                    if (kb == KB - 1) tc_commit(&tfull[as]);                   // accumulator complete
-                }
-                __syncwarp();
-                if (++s == NS) { s = 0; ph ^= 1u; }
-            }
-            if (++as == NACC) { as = 0; aph ^= 1u; }
-        }
-    } else if (warp >= 4) {                                                    // ===== epilogue: TMEM -> registers -> threshold test
-        const int quad = warp & 3;                                             // TMEM lane quadrant this warp may read
-        const int c_lo = ((warp - 4) >> 2) * (N / EPI), c_hi = c_lo + N / EPI;  // accumulator columns of this warp
-        // this thread's row norm of the NEXT tile is loaded while the current one is tested (a global load per tile on the
-        // critical path was 7% of the epilogue's stall samples)
-        auto load_norm = [&](long long mt_) -> uint32_t {
-            const long long row_ = mt_ * kTcM + quad * 32 + lane;
-            return (row_ >= prm.r0 && row_ < prm.r1) ? reinterpret_cast<const uint32_t *>(prm.norms)[row_] : 0u;
-        };
-        uint32_t nbits_next = tw.count ? load_norm(tw.mt()) : 0u;
-        uint32_t as = 0, aph = 0;
-        for (uint32_t tl = 0; tl < tw.count; ++tl) {
-            const long long mt = tw.mt();
-            const int ng = tw.ng();
-            tw.next();
-            const long long row = mt * kTcM + quad * 32 + lane;
-            const bool rowvalid = row >= prm.r0 && row < prm.r1;
-            const uint32_t nbits = nbits_next;
-            nbits_next = (tl + 1 < tw.count) ? load_norm(tw.mt()) : 0u;
-            float rowf = 0.0f;
-            int rowi = 0;
-            if (rowvalid) {
-                if constexpr (INT8) {
-                    const int nn = (int)nbits;
-                    rowi = -nn;
-                    rowf = (KIND == TK_U8) ? __fsqrt_rn((float)(uint32_t)nn) : __fsqrt_rn((float)nn);
-                } else {
-                    const float nn = __uint_as_float(nbits);
-                    rowf = (MC == MC_L2) ? -nn * (1.0f - prm.eps) : __fsqrt_rn(nn);
-                }
-            }
-            mbar_wait_backoff(&tfull[as], aph);
-            tc_fence_after();
-            // 64 accumulator columns per step, software pipelined: the TMEM loads of step i+1 are in flight while step i
-            // is tested (TMEM reads are 64 B/clk/SM: 128x256 fp32 accumulators take >= 2048 clk to drain, which bounds
-            // small-K tiles; keeping the read pipe busy is what matters here).
-            const uint32_t tbase = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * N);
-            auto issue = [&](int cb, uint32_t *v) {
-                if constexpr (CH == 16) tmem_ld16_nowait(tbase + (uint32_t)cb, v);
-                else tmem_ld32_nowait(tbase + (uint32_t)cb, v);
-                if constexpr (CH == 64) {
-                    if (cb + 32 < c_hi) tmem_ld32_nowait(tbase + (uint32_t)cb + 32, v + 32);
-                }
-            };
-            auto process = [&](int cb, const uint32_t *v) {
-                const bool two = (CH == 64) && (cb + 32) < c_hi;
-                const uint4 *qc4 = reinterpret_cast<const uint4 *>(qc_s + ng * N + cb);
-                constexpr int C0 = CH < 32 ? CH : 32;                          // columns in the first 32-column half
-                bool any0 = false, any1 = false;
-                if constexpr (kChunkTest) {
-                    int m0 = INT_MIN, m1 = INT_MIN, m2 = INT_MIN, m3 = INT_MIN;   // four independent chains of 3-input maxima
-#pragma unroll
-                    for (int j = 0; j < 32; j += 8) {
-                        m0 = max(m0, max((int)v[j + 0], (int)v[j + 1]));
-                        m1 = max(m1, max((int)v[j + 2], (int)v[j + 3]));
-                        m2 = max(m2, max((int)v[j + 4], (int)v[j + 5]));
-                        m3 = max(m3, max((int)v[j + 6], (int)v[j + 7]));
-                    }
-                    const int m = max(max(m0, m1), max(m2, m3));
-                    const uint32_t qm = qcm_s[(ng * N + cb) >> 5];
-                    if constexpr (MC == MC_DOT) any0 = m > (int)qm;
-                    else if constexpr (MC == MC_L2) any0 = (2 * m + rowi) >= (int)qm;
-                    else any0 = !(fmaf(-__uint_as_float(qm), rowf, (float)m) < 0.0f);   // rowf >= 0: monotone in both m and the bound
-                } else {
-#pragma unroll
-                    for (int j4 = 0; j4 < C0 / 4; ++j4) {
-                        const uint4 c = qc4[j4];
-                        any0 |= tc_hit<INT8, MC>(v[4 * j4 + 0], c.x, rowf, rowi) | tc_hit<INT8, MC>(v[4 * j4 + 1], c.y, rowf, rowi) |
-                                tc_hit<INT8, MC>(v[4 * j4 + 2], c.z, rowf, rowi) | tc_hit<INT8, MC>(v[4 * j4 + 3], c.w, rowf, rowi);
-                    }
-                }
-                if constexpr (CH == 64) {
-                    if (two) {
-#pragma unroll
-                        for (int j4 = 8; j4 < 16; ++j4) {
-                            const uint4 c = qc4[j4];
-                            any1 |= tc_hit<INT8, MC>(v[4 * j4 + 0], c.x, rowf, rowi) | tc_hit<INT8, MC>(v[4 * j4 + 1], c.y, rowf, rowi) |
-                                    tc_hit<INT8, MC>(v[4 * j4 + 2], c.z, rowf, rowi) | tc_hit<INT8, MC>(v[4 * j4 + 3], c.w, rowf, rowi);
-                        }
-                    }
-                }
-                const bool any = (any0 | any1) && rowvalid;
-                if (__ballot_sync(0xFFFFFFFFu, any)) {                         // rare: append (row, query) hits, one atomic per warp
-                    const uint32_t *qc = qc_s + ng * N + cb;
-                    uint32_t mask0 = 0, mask1 = 0;
-                    if (any) {
-#pragma unroll
-                        for (int j = 0; j < C0; ++j) mask0 |= (tc_hit<INT8, MC>(v[j], qc[j], rowf, rowi) ? 1u : 0u) << j;
-                        if constexpr (CH == 64) {
-                            if (two) {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) mask1 |= (tc_hit<INT8, MC>(v[32 + j], qc[32 + j], rowf, rowi) ? 1u : 0u) << j;
-                            }
-                        }
-                        const int ncol = prm.nq - (ng * N + cb);                // padded query columns are never reported
-                        mask0 &= (ncol >= 32) ? 0xFFFFFFFFu : (ncol <= 0 ? 0u : ((1u << ncol) - 1u));
-                        mask1 &= (ncol >= 64) ? 0xFFFFFFFFu : (ncol <= 32 ? 0u : ((1u << (ncol - 32)) - 1u));
-                    }
-                    const int mine = __popc(mask0) + __popc(mask1);
-                    int incl = mine;
-                    for (int off = 1; off < 32; off <<= 1) {
-                        const int o = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-                        if (lane >= off) incl += o;
-                    }
-                    const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-                    unsigned base = 0;
-                    if (lane == 31) base = atomicAdd(prm.cand_count, (unsigned)total);
-                    base = __shfl_sync(0xFFFFFFFFu, base, 31);
-                    unsigned w = base + (unsigned)(incl - mine);
-                    while (mask0) {
-                        const int j = __ffs(mask0) - 1;
-                        mask0 &= mask0 - 1;
-                        if (w < prm.cand_cap) prm.cand[w] = make_uint2((uint32_t)row, (uint32_t)(ng * N + cb + j));
-                        ++w;
-                    }
-                    while (mask1) {
-                        const int j = __ffs(mask1) - 1;
-                        mask1 &= mask1 - 1;
-                        if (w < prm.cand_cap) prm.cand[w] = make_uint2((uint32_t)row, (uint32_t)(ng * N + cb + 32 + j));
-                        ++w;
-                    }
-                }
-            };
-            // the accumulator buffer is handed back to the MMA warp as soon as this warp's LAST TMEM load has landed in
-            // registers — before that chunk is tested: the MMA of tile t+2 waits for exactly this arrival (profiles/r02d: after the
-            // issue loops were fixed, the MMA <-> epilogue hand-over of the two buffers set the tile period, not either pipe)
-            auto release = [&]() {
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[as]);
-            };
-            uint32_t va[CH], vb[CH];
-            issue(c_lo, va);
-            for (int cb = c_lo; cb < c_hi; cb += 2 * CH) {
-                tmem_wait_ld();
-                const bool more1 = cb + CH < c_hi;
-                if (more1) issue(cb + CH, vb);
-                else release();
-                process(cb, va);
-                if (more1) {
-                    tmem_wait_ld();
-                    if (cb + 2 * CH < c_hi) issue(cb + 2 * CH, va);
-                    else release();
-                    process(cb + CH, vb);
-                }
-            }
-            if (++as == NACC) { as = 0; aph ^= 1u; }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
+
+    // ===== consumer warpgroup wg: MMAs of its 64 rows, then the threshold test from registers
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const int ra = wg * 64 + 16 * (t >> 5) + (lane >> 2);                     // tile rows ra and ra + 8
+    const int cq = 2 * (lane & 3);                                             // first of the thread's two columns in each group of 8
+    Acc d[N / 2];
+    int s = 0;
+    uint32_t ph = 0;                                                           // parity to wait for on full[s]
+    for (uint32_t tl = 0; tl < tw.count; ++tl, tw.next()) {
+        const long long mt = tw.mt();
+        const int ng = tw.ng();
+        const long long row[2] = {mt * kTcM + ra, mt * kTcM + ra + 8};
+        bool rowvalid[2];
+        uint32_t nbits[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {                                          // issued before the MMAs: the load latency hides behind them
+            rowvalid[h] = row[h] >= prm.r0 && row[h] < prm.r1;
+            nbits[h] = rowvalid[h] ? reinterpret_cast<const uint32_t *>(prm.norms)[row[h]] : 0u;
+        }
+        int prev = -1;
+        for (int kb = 0; kb < KB; ++kb) {
+            mbar_wait(&full[s], ph);
+            const uint8_t *st = stages + (size_t)s * stage_bytes;
+            const uint64_t ad = gmma_desc_sw128(st + wg * 64 * kTcKBytes), bd = gmma_desc_sw128(st + a_bytes);
+            wgmma_fence();
+#pragma unroll
+            for (int k4 = 0; k4 < kTcKBytes / 32; ++k4)                        // K = 32 bytes per MMA: advance the start address by 2 (x16 B)
+                tc_mma<KIND, N>(d, ad + (uint64_t)(2 * k4), bd + (uint64_t)(2 * k4), (uint32_t)((kb | k4) != 0));
+            wgmma_commit();
+            wgmma_wait<1>();                                                   // the previous K block's MMAs have read their stage
+            if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+            prev = s;
+            if (++s == NS) { s = 0; ph ^= 1u; }
+        }
+        wgmma_wait<0>();
+        if (t == 0) mbar_arrive(&empty[prev]);                                 // the producer refills it while the scores are tested
+
+        float rowf[2] = {0.0f, 0.0f};
+        int rowi[2] = {0, 0};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            if (!rowvalid[h]) continue;
+            if constexpr (INT8) {
+                const int nn = (int)nbits[h];
+                rowi[h] = -nn;
+                rowf[h] = (KIND == TK_U8) ? __fsqrt_rn((float)(uint32_t)nn) : __fsqrt_rn((float)nn);
+            } else {
+                const float nn = __uint_as_float(nbits[h]);
+                rowf[h] = (MC == MC_L2) ? -nn * (1.0f - prm.eps) : __fsqrt_rn(nn);
+            }
+        }
+        const uint32_t *qc = qc_s + ng * N;
+        auto bits = [&](int i) -> uint32_t {
+            if constexpr (INT8) return d[i];
+            else return __float_as_uint(d[i]);
+        };
+        auto hit = [&](int i) -> bool {                                       // accumulator i: row ra + 8 * ((i >> 1) & 1), column 8 (i >> 2) + cq + (i & 1)
+            const int h = (i >> 1) & 1, col = 8 * (i >> 2) + cq + (i & 1);
+            return rowvalid[h] && tc_hit<INT8, MC>(bits(i), qc[col], rowf[h], rowi[h]);
+        };
+        bool any = false;
+        if (chunk) {
+#pragma unroll
+            for (int c = 0; c < N / 32; ++c) {
+                const uint32_t qm = qcm_s[(ng * N >> 5) + c];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    int m = INT_MIN;
+#pragma unroll
+                    for (int j = 4 * c; j < 4 * c + 4; ++j) m = max(m, max((int)bits(4 * j + 2 * h), (int)bits(4 * j + 2 * h + 1)));
+                    bool a;
+                    if constexpr (MC == MC_DOT) a = m > (int)qm;
+                    else if constexpr (MC == MC_L2) a = (2 * m + rowi[h]) >= (int)qm;
+                    else a = !(fmaf(-__uint_as_float(qm), rowf[h], (float)m) < 0.0f);   // rowf >= 0: monotone in both m and the bound
+                    any |= a && rowvalid[h];
+                }
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const uint2 c = *reinterpret_cast<const uint2 *>(qc + 8 * j + cq);
+                any |= (rowvalid[0] && (tc_hit<INT8, MC>(bits(4 * j + 0), c.x, rowf[0], rowi[0]) | tc_hit<INT8, MC>(bits(4 * j + 1), c.y, rowf[0], rowi[0]))) ||
+                       (rowvalid[1] && (tc_hit<INT8, MC>(bits(4 * j + 2), c.x, rowf[1], rowi[1]) | tc_hit<INT8, MC>(bits(4 * j + 3), c.y, rowf[1], rowi[1])));
+            }
+        }
+        if (__ballot_sync(0xFFFFFFFFu, any)) {                                 // rare: append (row, query) hits, one atomic per warp
+            const int ncol = prm.nq - ng * N;                                  // padded query columns are never reported
+            int mine = 0;
+            if (any) {
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) mine += (hit(i) && 8 * (i >> 2) + cq + (i & 1) < ncol) ? 1 : 0;
+            }
+            int incl = mine;
+            for (int off = 1; off < 32; off <<= 1) {
+                const int o = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+                if (lane >= off) incl += o;
+            }
+            const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+            unsigned base = 0;
+            if (lane == 31) base = atomicAdd(prm.cand_count, (unsigned)total);
+            base = __shfl_sync(0xFFFFFFFFu, base, 31);
+            unsigned w = base + (unsigned)(incl - mine);
+            if (mine) {
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) {
+                    const int col = 8 * (i >> 2) + cq + (i & 1);
+                    if (hit(i) && col < ncol) {
+                        if (w < prm.cand_cap) prm.cand[w] = make_uint2((uint32_t)row[(i >> 1) & 1], (uint32_t)(ng * N + col));
+                        ++w;
+                    }
+                }
+            }
+        }
     }
 }
+
 
 // ------------------------------------------------------------------ row norms (once per resident shard)
 template <int VT>
@@ -662,7 +519,7 @@ __device__ __forceinline__ void warp_offer32(float *sd, unsigned *sr, int kcap, 
 __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
 
 // Slack of the fp tensor-core score, relative to |q||r| (>= sum |q_i r_i|).  bf16 x bf16 and f16 x f16 products are exact in
-// fp32; what is not specified is how tcgen05 adds them (block order, alignment to the largest exponent, truncation).  Any
+// fp32; what is not specified is how the tensor core adds them (block order, alignment to the largest exponent, truncation).  Any
 // scheme that keeps 24 bits relative to the largest addend of a block loses < 2^-22 * sum|terms| per addend it aligns, i.e.
 // |s_tc - s| <= dim * 2^-21 * sum|q_i r_i| over a row of `dim` products (accumulator re-aligned once per block included).  The
 // exact refine adds its own fp32 FMA-chain error (<= dim * 2^-24 * sum|terms|) and the norms carry the same relative error.

@@ -1,8 +1,8 @@
-// engine.cu — host side of the B200 scan engine behind include/vsb200.h.
+// engine.cu — host side of the H100 scan engine behind include/vsb200.h.
 //
 // Owns device residency of a column shard (the GPU counterpart of table_context.preloaded,
 // /root/reference/src/sqlite-vector.c:126-137, filled by vector_quantize_preload :1338-1404),
-// launches the sm_100a kernels in scan_kernels.cuh and finishes each query with the reference's
+// launches the sm_90a kernels in scan_kernels.cuh and finishes each query with the reference's
 // k-slot algorithm (:1808-1817, :2022-2069, :2145-2152) over the few hundred surviving candidates.
 // No CPU fallback: if CUDA is unavailable every entry point returns VSB_ENODEV.
 #include "../../include/vsb200.h"
@@ -33,7 +33,7 @@ namespace {
 
 thread_local std::string g_err;
 std::atomic<long long> g_launches{0};
-int g_opt_stage_bytes = 16384; // upper bound of one warp tile (ring stage); 12 KB tiles x 2 stages measured best (99% of HBM peak)
+int g_opt_stage_bytes = 16384; // upper bound of one warp tile (ring stage); int8 dim 384: 12 KB tiles x 2 stages (chosen on earlier hardware)
 int g_opt_direct = 0;          // 1: force the no-staging kernel
 int g_opt_ring_bytes = 0;      // 0: use all shared memory left
 int g_opt_no_batch = 0;        // 1: never take the tensor-core batch path
@@ -42,24 +42,23 @@ int g_opt_batch_m0 = 128;      // batch path: rows refined exhaustively before t
 int g_opt_merge_stream = 1;    // process exchange, batched queries: wait + merge + copy back on their own stream (overlaps the next batch's levels)
 int g_opt_batch_growth = 8;    // batch path: each tensor-core level covers rows [m, growth*m) (capped by k, see batch_growth)
 int g_opt_fuse_mb = 0;         // > 0: vsb_scan_submit_group fuses a group into ONE scan launch when one query's scan reads less than this
-                               // many MB (measured per query on one GPU: 84.0 -> 76.9 us at 0.48 GB; 2 GPUs: 285 -> 271 us at 1.92 GB).
-                               // Off by default: a persistent 8-query launch leaves the NCCL all-gather of the previous group no SM until
-                               // it ends (2 GPUs: the step-vs-scan gap grew from 3 to 14 us per query), not yet measured at 8 GPUs.
+                               // many MB (saves 7 of 8 launches for a slow launcher).  Off by default: a persistent 8-query launch leaves
+                               // the NCCL all-gather of the previous group no SM until it ends.  Not measured on H100.
 int g_opt_balance = 1;         // 1: adaptive row partition of the single-query scan (per-CTA speeds feed the next partition)
 int g_opt_epi_chunk = 1;       // 1: integer tensor-core epilogue tests 32-column chunks (max score vs weakest bound) before any per-column work
-int g_opt_epi2 = 4;            // epilogue shape of tc_scan_kernel (see launch_tc_mc): 4 = 16 epilogue warps where that variant exists (integer kinds, 256-query tiles), else 8; 2 = 8 warps; 0 = 4 warps
 int g_opt_time_kernels = 0;    // 1: bracket every kernel launch with CUDA events (bench.py roofline leg)
 int g_opt_scan_streams = 2;    // 2: consecutive scan launches alternate between two streams, so the CTAs of launch i+1 take over each SM
                                // as soon as the CTA of launch i on it exits (one scan CTA fits per SM): no grid-wide drain between
                                // launches, per-SM speed differences turn into an earlier start of the next query.  1: one stream.
-int g_opt_push_mode = 1;       // exchange: 1 (default) = a small kernel on the exchange stream pushes a finished group's heads; 0 = the filter's last block pushes its head itself (fused: costs ~2 us per query with 8 targets, profiles/r02j)
+int g_opt_push_mode = 1;       // exchange: 1 (default) = a small kernel on the exchange stream pushes a finished group's heads; 0 = the filter's last block pushes its head itself (fused: the filter stream then waits for NVLink acknowledgements; not measured on H100)
 int g_opt_push_repeat = 1;     // experiment: push every exchange target this many times (see exchange_fill_push)
-int g_opt_xwait_ms = 2000;     // exchange: how long the receiving side waits for a peer's head before it reports an error
+int g_opt_xwait_ms = 10000;    // exchange: how long the receiving side waits for a peer's head before it reports an error (a dead
+                               // peer, not a slow one: ranks sharing one GPU or a busy host can start a batch seconds apart)
 
 // cudaFuncSetAttribute costs ~1 us per call; the dynamic shared memory limit of a kernel only ever needs to grow
 int set_smem_limit(const void *fn, size_t bytes) {
     static std::mutex mu;
-    static std::vector<std::pair<const void *, size_t>> seen;     // per process; devices are identical B200s
+    static std::vector<std::pair<const void *, size_t>> seen;     // per process; devices are identical H100s
     std::lock_guard<std::mutex> lk(mu);
     int dev = 0;
     cudaGetDevice(&dev);
@@ -831,10 +830,10 @@ const char *vsb_backend_name(void) {
     static char name[160];
     std::call_once(once, [] {
         int n = vsb_device_count();
-        if (n <= 0) { snprintf(name, sizeof name, "CUDA sm_100a (no device)"); return; }
+        if (n <= 0) { snprintf(name, sizeof name, "CUDA sm_90a (no device)"); return; }
         cudaDeviceProp pr{};
         cudaGetDeviceProperties(&pr, 0);
-        snprintf(name, sizeof name, "CUDA sm_100a (%s x%d, cc %d.%d)", pr.name, n, pr.major, pr.minor);
+        snprintf(name, sizeof name, "CUDA sm_90a (%s x%d, cc %d.%d)", pr.name, n, pr.major, pr.minor);
     });
     return name;
 }
@@ -848,7 +847,6 @@ int vsb_set_option(const char *name, int value) {
     else if (!strcmp(name, "ring_bytes")) p = &g_opt_ring_bytes;
     else if (!strcmp(name, "time_kernels")) p = &g_opt_time_kernels;
     else if (!strcmp(name, "no_batch")) p = &g_opt_no_batch;
-    else if (!strcmp(name, "epi2")) p = &g_opt_epi2;
     else if (!strcmp(name, "epi_chunk")) p = &g_opt_epi_chunk;
     else if (!strcmp(name, "balance")) p = &g_opt_balance;
     else if (!strcmp(name, "fuse_mb")) p = &g_opt_fuse_mb;
@@ -893,7 +891,8 @@ static int index_create(vsb_index **out, int device, int vtype, int dim, int64_t
     CU(cudaSetDevice(device));
     cudaDeviceProp pr{};
     CU(cudaGetDeviceProperties(&pr, device));
-    if (pr.major < 9) return fail(VSB_ENODEV, "device %s (cc %d.%d) lacks TMA bulk copies; sm_100a required", pr.name, pr.major, pr.minor);
+    if (pr.major != 9 || pr.minor != 0)   // sm_90a code (wgmma, TMA) runs on compute capability 9.0 only
+        return fail(VSB_ENODEV, "device %s (cc %d.%d): this build holds sm_90a (H100) code only", pr.name, pr.major, pr.minor);
     vsb_index *ix = new (std::nothrow) vsb_index();
     if (!ix) return fail(VSB_ENOMEM, "out of host memory");
     ix->device = device; ix->vtype = vtype; ix->dim = dim; ix->esize = es;

@@ -1,4 +1,4 @@
-// scan_kernels.cuh — sm_100a kernels of the single-query (HBM-bound) distance scan.
+// scan_kernels.cuh — sm_90a kernels of the single-query (HBM-bound) distance scan.
 //
 // Replaces, for a whole resident shard at once, the per-row loop of the reference:
 //   fn = dispatch_distance_table[metric][type]; d = fn(q,row,dim); clamp; slot update
@@ -608,7 +608,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
             if (prm.kcap == 32) {
                 // k <= 32: the CTA's 8 streams are consecutive in scan order.  Sort each stream's list, then one warp merges
                 // them in stream order, recording the running k-th value BEFORE each stream (its in-CTA prefix bound), and
-                // publishes ONE sorted list per CTA: filter_kernel then walks 148 CTA lists instead of 1184 stream lists.
+                // publishes ONE sorted list per CTA: filter_kernel then walks one list per CTA instead of one per stream.
                 float v = (lane < prm.k) ? mylist[lane] : INFINITY;
                 v = warp_sort_asc(v, lane);
                 mylist[lane] = v;

@@ -1,5 +1,5 @@
 /*
- * vector_ext.c — SQLite loadable extension with sqlite-vector's SQL surface, scanning on the B200.
+ * vector_ext.c — SQLite loadable extension with sqlite-vector's SQL surface, scanning on the H100.
  *
  * Same entry point and SQL objects as the reference (src/sqlite-vector.c:2555-2638):
  *   scalar: vector_version, vector_backend, vector_init, vector_quantize (2|3 args), vector_quantize_memory,

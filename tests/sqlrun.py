@@ -40,9 +40,16 @@ print("\n@@JSON@@" + json.dumps(out), flush=True)
 
 
 def run_sql(lib_path: str, statements, timeout=600, env=None, want_launches=False):
-    """lib_path without the .so suffix is fine (sqlite appends it).  Returns a list of {"rows": ...} | {"error": ...}
+    """lib_path without the .so suffix is fine (sqlite appends it).  REF_CPU is served from tests/golden/ref_sql.json.gz where
+    oracle/_ref is not built (tests/refreplay.py).  Returns a list of {"rows": ...} | {"error": ...}
     (plus, with want_launches, the library's kernel launch count after the script as a last element)."""
-    r = _run_sql(lib_path, statements, timeout, env)
+    if os.path.abspath(lib_path) == REF_CPU:      # the reference extension: live where oracle/_ref is built, else recorded
+        from tests import refreplay
+        key = refreplay._key("sql", json.dumps(statements, sort_keys=True), json.dumps(env, sort_keys=True))
+        live = (lambda: _run_sql(lib_path, statements, timeout, env)) if os.path.exists(REF_CPU + ".so") else None
+        r = refreplay.recorded("sql", key, live)
+    else:
+        r = _run_sql(lib_path, statements, timeout, env)
     return r if want_launches else r[:-1]
 
 

@@ -90,7 +90,7 @@ def test_config5_at_size(oracle, dim):
 
 
 def test_config3_shape_bf16_dot_batch1024(oracle):
-    """bf16 DOT dim 768 k=20 B=1024 on 1M rows: the batch (tcgen05) result of every query against the oracle for a sample of
+    """bf16 DOT dim 768 k=20 B=1024 on 1M rows: the batch (wgmma) result of every query against the oracle for a sample of
     128 queries, and against the single-query CUDA-core path for all 1024"""
     import sqlite_vector_b200 as vs
     n, dim, nq, k = 1_000_000, 768, 1024, 20

@@ -1,4 +1,4 @@
-"""Batched queries (tcgen05 tensor-core path) vs the oracle and vs the per-query CUDA-core path.  -m gpu."""
+"""Batched queries (wgmma tensor-core path) vs the oracle and vs the per-query CUDA-core path.  -m gpu."""
 import numpy as np
 import pytest
 

@@ -1,4 +1,4 @@
-"""CUDA path vs the oracle through the C ABI (include/vsb200.h).  Run on the B200 box: pytest -m gpu.
+"""CUDA path vs the oracle through the C ABI (include/vsb200.h).  Run on an H100: pytest -m gpu.
 
 Bit-exact for int8/uint8 (rowids, order, distances); 1e-5 relative for fp distances
 (tolerance relative to max(|d|, sum|a_i*b_i| scale) as documented in DESIGN.md §5)."""

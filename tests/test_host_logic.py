@@ -253,9 +253,9 @@ def test_merge_result_groups_matches_oracle(oracle):
         assert np.array_equal(res[j][0], want_ids) and np.array_equal(res[j][1], want_d), j
 
 
-def test_built_kernels_use_tcgen05_and_tma_not_mma_sync():
-    """the library that travels to the GPU box: tensor-core kernels are tcgen05 (UTC*MMA + TMEM loads + TMA tensor loads), the
-    scan kernels use TMA bulk copies, nothing falls back to mma.sync (tools/sass_evidence.py over cuobjdump -sass)"""
+def test_built_kernels_use_wgmma_and_tma_not_mma_sync():
+    """the library that travels to the GPU box: tensor-core kernels are Hopper warpgroup MMAs (HGMMA / IGMMA) fed by TMA tensor
+    loads, the scan kernels use TMA bulk copies, nothing falls back to mma.sync (tools/sass_evidence.py over cuobjdump -sass)"""
     import shutil
     if not shutil.which("cuobjdump"):
         pytest.skip("no cuobjdump here")
@@ -265,7 +265,7 @@ def test_built_kernels_use_tcgen05_and_tma_not_mma_sync():
     ev = json.loads(r.stdout)
     ks = ev["kernels"]
     tc = [k for k in ks if "tc_scan_kernel" in k]
-    assert len(tc) >= 24 and all(("UTCIMMA" in ks[k] or "UTCHMMA" in ks[k]) and "UTMALDG" in ks[k] and "LDTM" in ks[k] and "UTCBAR" in ks[k] for k in tc), tc
+    assert len(tc) >= 24 and all(("IGMMA" in ks[k] or "HGMMA" in ks[k]) and "UTMALDG" in ks[k] and "WARPGROUP" in ks[k] for k in tc), tc
     staged = [k for k in ks if "scan_kernel<" in k and "tc_" not in k and k.rstrip(">").endswith("false")]
     assert len(staged) == 20 and all("UBLKCP" in ks[k] for k in staged), staged
     assert not ev["mma_sync_anywhere"]

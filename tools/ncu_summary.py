@@ -1,4 +1,4 @@
-"""Condense ncu captures (ncu --set full) into a small JSON for profiles/.
+"""Condense ncu captures (ncu --set full) into a small JSON.
    python tools/ncu_summary.py capture.ncu-rep|capture_raw.csv [...]   -> JSON on stdout: {file: {metric: [value, unit]}}
 A *_raw.csv is the output of `ncu -i x.ncu-rep --page raw --csv` (tools/gpu_job.sh exports it on the GPU box)."""
 import csv

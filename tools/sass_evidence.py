@@ -1,10 +1,10 @@
-"""Which Blackwell instructions the built kernels contain: cuobjdump -sass of lib/libvsb200.so, occurrences per kernel.
+"""Which Hopper instructions the built kernels contain: cuobjdump -sass of lib/libvsb200.so, occurrences per kernel.
 
-  python tools/sass_evidence.py > profiles/<tag>_sass_evidence.json
+  python tools/sass_evidence.py > <file>.json
 
-PTX -> SASS names (see /opt/skills/guides/B200_PROFILING.md): tcgen05.mma = UTCIMMA (kind::i8) / UTCHMMA (kind::f16),
-tcgen05.ld = LDTM, tcgen05.commit = UTCBAR, tcgen05.alloc = UTCATOMSWS, cp.async.bulk.tensor = UTMALDG, cp.async.bulk = UBLKCP,
-elect.sync = ELECT, dp4a = IDP, redux.sync = REDUX.  HMMA / IMMA (mma.sync) must not appear anywhere."""
+PTX -> SASS names: wgmma.mma_async = HGMMA (f16 / bf16) / IGMMA (s8 / u8), wgmma.fence / commit_group / wait_group = WARPGROUP,
+cp.async.bulk.tensor = UTMALDG, cp.async.bulk = UBLKCP, elect.sync = ELECT, dp4a = IDP, redux.sync = REDUX, mbarrier = SYNCS.
+HMMA / IMMA (mma.sync) must not appear anywhere."""
 import collections
 import json
 import os
@@ -13,7 +13,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-WATCH = ("UTCIMMA", "UTCHMMA", "LDTM", "UTCBAR", "UTCATOMSWS", "UTMALDG", "UBLKCP", "ELECT", "IDP", "REDUX", "HMMA", "IMMA", "SYNCS", "VIMNMX3", "STL", "LDL")
+WATCH = ("HGMMA", "IGMMA", "WARPGROUP", "UTMALDG", "UBLKCP", "ELECT", "IDP", "REDUX", "HMMA", "IMMA", "SYNCS", "STL", "LDL")
 
 
 def main():
@@ -41,7 +41,7 @@ def main():
     out = {"how": __doc__.split("\n\n")[0] + " (tools/sass_evidence.py)", "library": os.path.relpath(lib, ROOT), "kernels": {}}
     for a in mangled:
         out["kernels"][names[a]] = dict(sorted(counts[a].items()))
-    out["kernels_with_tcgen05_mma"] = sorted(k for k, v in out["kernels"].items() if "UTCIMMA" in v or "UTCHMMA" in v)
+    out["kernels_with_wgmma"] = sorted(k for k, v in out["kernels"].items() if "HGMMA" in v or "IGMMA" in v)
     out["kernels_with_tma"] = sorted(k for k, v in out["kernels"].items() if "UTMALDG" in v or "UBLKCP" in v)
     out["mma_sync_anywhere"] = any("HMMA" in v or "IMMA" in v for v in out["kernels"].values())
     out["local_memory_spills"] = sorted(k for k, v in out["kernels"].items() if "STL" in v or "LDL" in v)

@@ -1,5 +1,5 @@
 """End-to-end latency THROUGH SQL: the same statements against our extension (sqlite_vector_b200/lib/vector.so, needs a
-B200) and against the unmodified reference (oracle/_ref/avx2/vector.so, CPU), each in its own process (SQLite loads
+H100) and against the unmodified reference (oracle/_ref/avx2/vector.so, CPU), each in its own process (SQLite loads
 extensions RTLD_GLOBAL and the reference exports every symbol).
 
   python tools/sql_bench.py --n 200000 --dim 384 --queries 50 [--which ours|ref|both]

@@ -241,6 +241,18 @@ VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches,
 /* diagnostics: copies an internal device buffer of the most recent single-query scan to `out`; name in {"cta_time" (unsigned
  * cycles per scan CTA), "bounds" (int64 tile boundaries of the adaptive row partition)}.  Returns the bytes copied or < 0. */
 VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes);
+/* diagnostics: ONE tensor-core level of the batch path (tc_scan_kernel) over rows [r0, r1) of a finalized resident index
+ * (r0 a multiple of 128), for nq HOST queries whose exact distance bounds U[nq] are given instead of found by earlier levels;
+ * the per-query constants are the batch path's own (conservative_qc).  N: queries per tile, 32 / 64 / 128 (/ 256 for
+ * int8 and uint8), 0 = the batch path's choice for nq.
+ *   mode 0 (candidate log, the production kernel): out receives up to out_cap (row, query) pairs of uint32, *out_count the
+ *   number of hits the kernel counted (more than out_cap when the log was truncated).
+ *   mode 1 (scores): out[(row - r0) * nq + q] = <row, query q> as the tensor cores computed it, int32 (int8 / uint8) or
+ *   float (f16 / bf16); out_cap >= (r1 - r0) * nq.
+ * out_qc (nq x 32 bits: float, or int for the integer kinds) and out_norms (r1 - r0 row sums of squares, float / int) may be
+ * NULL.  Synchronous. */
+VSB_API int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1,
+                               int N, int mode, void *out, int64_t out_cap, void *out_qc, void *out_norms, int64_t *out_count);
 /* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","epi2","batch_debug","batch_m0","batch_growth","balance","fuse_mb","scan_streams","xwait_ms","epi_chunk","push_mode","push_repeat","merge_stream" (experiment)};
  * values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);

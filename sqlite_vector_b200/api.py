@@ -91,6 +91,7 @@ _SIGNATURES = {
     "vsb_set_option": (_i, [C.c_char_p, _i]),
     "vsb_profile_read": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vsb_debug_read": (_i, [_vp, C.c_char_p, _vp, _i64]),
+    "vsb_debug_tc_level": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i64, _i, _i, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
 }
 
 
@@ -355,6 +356,34 @@ class Index:
         if got < 0:
             self.eng.check(got)
         return out[: got // out.itemsize]
+
+    def debug_tc_level(self, metric: int, queries: np.ndarray, U: np.ndarray, r0: int, r1: int, N: int = 0, scores: bool = False,
+                       cap: int = 1 << 22):
+        """one tensor-core level of the batch path over rows [r0, r1) with the per-query bounds U (vsb_debug_tc_level).
+        scores=False: {"log": (row, query) uint32 pairs, "count": hits counted (> len(log) when truncated at cap),
+        "qc": uint32 bits [nq], "norms": row sums of squares [r1 - r0]}; scores=True: the same with "scores" [r1 - r0, nq]
+        (int32 for int8 / uint8, float32 for f16 / bf16) instead of the log"""
+        q2 = np.ascontiguousarray(queries).reshape(-1, queries.shape[-1])
+        nq = q2.shape[0]
+        u = np.ascontiguousarray(U, dtype=np.float32)
+        assert u.shape == (nq,)
+        integer = self.vtype in (U8, I8)
+        qc = np.zeros(nq, dtype=np.uint32)
+        norms = np.zeros(r1 - r0, dtype=np.int32 if integer else np.float32)
+        count = _i64()
+        if scores:
+            out = np.zeros((r1 - r0, nq), dtype=np.int32 if integer else np.float32)
+            cap = out.size
+        else:
+            out = np.zeros((cap, 2), dtype=np.uint32)
+        self.eng.check(self.eng.lib.vsb_debug_tc_level(self.h, metric, _ptr(q2), nq, _ptr(u), r0, r1, N, int(scores), _ptr(out), cap,
+                                                       _ptr(qc), _ptr(norms), C.byref(count)))
+        res = {"count": int(count.value), "qc": qc, "norms": norms}
+        if scores:
+            res["scores"] = out
+        else:
+            res["log"] = out[: min(int(count.value), cap)].copy()
+        return res
 
     def profile_read(self):
         a, b = C.c_double(), C.c_double()

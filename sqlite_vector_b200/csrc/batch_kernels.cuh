@@ -26,6 +26,9 @@ constexpr int kTcThreads = kTcConsumers * 128 + 32;
 constexpr int kTcMaxStages = 8;
 constexpr int kTcM = 128;           // corpus rows per tile
 constexpr int kTcKBytes = 128;      // one swizzle atom of K per stage
+// tc_scan_kernel<KIND, MC_TC_SCORES, N>: the same tile walk and MMAs, but every score of rows [r0, r1) x queries [0, nq) is
+// stored to TcParams::scores instead of being tested (vsb_debug_tc_level checks the scores against an exact GEMM)
+constexpr int MC_TC_SCORES = 4;
 
 struct TcParams {
     long long r0, r1;       // row range of this level (r0 multiple of 128)
@@ -43,6 +46,7 @@ struct TcParams {
     uint2 *cand;            // (row, query)
     unsigned *cand_count;
     unsigned cand_cap;
+    uint32_t *scores;       // MC_TC_SCORES only: [r1 - r0][nq] int32 / float bits
 };
 
 // ------------------------------------------------------------------ PTX wrappers (TMA / wgmma)
@@ -229,6 +233,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
         }
         wgmma_wait<0>();
         if (t == 0) mbar_arrive(&empty[prev]);                                 // the producer refills it while the scores are tested
+        if constexpr (MC == MC_TC_SCORES) {
+            const int ncol = prm.nq - ng * N;
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) {                                  // accumulator i: row ra + 8 * ((i >> 1) & 1), column 8 (i >> 2) + cq + (i & 1)
+                const int h = (i >> 1) & 1, col = 8 * (i >> 2) + cq + (i & 1);
+                uint32_t v;
+                if constexpr (INT8) v = d[i];
+                else v = __float_as_uint(d[i]);
+                if (rowvalid[h] && col < ncol) prm.scores[(size_t)(row[h] - prm.r0) * prm.nq + ng * N + col] = v;
+            }
+            continue;
+        }
 
         float rowf[2] = {0.0f, 0.0f};
         int rowi[2] = {0, 0};
@@ -563,6 +579,12 @@ __device__ inline float conservative_qc(int kind, int mc, int root, float U, con
         return qq * (1.0f - eps) - u2 * (1.0f + 0.25f * eps + 1e-6f) - 1e-30f;
     }
     return clampf((1.0f - U - eps - 2e-6f) * sqrtf(qq), -1e30f, 1e30f);             // cosine: s > (1 - U - slack) |q||r|
+}
+
+// the constants replay_kernel would derive from the bounds U[nq] (vsb_debug_tc_level: one tensor-core level in isolation)
+__global__ void conservative_qc_kernel(float *qc, const float *U, int nq, int kind, int mc, int root, const void *qnorm, float rnmax, int dim) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < nq) qc[q] = conservative_qc(kind, mc, root, U[q], qnorm, q, rnmax, dim);
 }
 
 constexpr int kReplayThreads = 128;

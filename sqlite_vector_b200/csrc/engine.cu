@@ -1242,6 +1242,15 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
     return (int)std::min<size_t>(have, (size_t)bytes);
 }
 
+int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1, int N, int mode,
+                       void *out, int64_t out_cap, void *out_qc, void *out_norms, int64_t *out_count) {
+    if (check_index(ix)) return VSB_EINVAL;
+    long long cnt = 0;
+    const int rc = batch_tc_level(ix, metric, queries, nq, U, r0, r1, N, mode, out, out_cap, out_qc, out_norms, &cnt);
+    if (rc == VSB_OK && out_count) *out_count = cnt;
+    return rc;
+}
+
 int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double *filter_ms, int *filter_launches) {
     if (check_index(ix)) return VSB_EINVAL;
     CU(cudaSetDevice(ix->device));

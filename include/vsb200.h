@@ -230,7 +230,9 @@ VSB_API int vsb_quantizer_encode(vsb_quantizer *qz, const void *rows, int64_t re
 VSB_API void vsb_quantizer_free(vsb_quantizer *qz);
 
 VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row on the device (multiple of 16) */
-/* counters since creation; name in {"queries","survivors","last_survivors","fallbacks","filter_blocks","fetch_bytes","slots","batches","batch_cands","batch_kept","tc_us","tc_rows","batch_us","stream_bytes","stream_us"}; -1 if unknown */
+/* counters since creation; name in {"queries","survivors","last_survivors","fallbacks","filter_blocks","fetch_bytes","slots","batches","batch_cands","batch_kept","tc_us","tc_rows","batch_us","stream_bytes","stream_us",
+ * "sms" (scan CTAs per launch)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */
 /* kernel launch counter (all kernels launched by this library since load) */
@@ -241,6 +243,11 @@ VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches,
 /* diagnostics: copies an internal device buffer of the most recent single-query scan to `out`; name in {"cta_time" (unsigned
  * cycles per scan CTA), "bounds" (int64 tile boundaries of the adaptive row partition)}.  Returns the bytes copied or < 0. */
 VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes);
+/* diagnostics: the counterpart of vsb_debug_read for name "bounds": plants a row partition (int64 tile boundaries, one per scan
+ * CTA plus one, non-decreasing from 0 to the tile count of the k <= 32 plan; vsb_index_stat "sms" CTAs) into every scan
+ * workspace of a resident index, so that the next single-query scans with k <= 32 use it instead of equal shares (the filter
+ * then rewrites it as usual).  Rejects an index too small for the adaptive partition.  Returns 0 or < 0. */
+VSB_API int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t bytes);
 /* diagnostics: ONE tensor-core level of the batch path (tc_scan_kernel) over rows [r0, r1) of a finalized resident index
  * (r0 a multiple of 128), for nq HOST queries whose exact distance bounds U[nq] are given instead of found by earlier levels;
  * the per-query constants are the batch path's own (conservative_qc).  N: queries per tile, 32 / 64 / 128 (/ 256 for

@@ -91,6 +91,7 @@ _SIGNATURES = {
     "vsb_set_option": (_i, [C.c_char_p, _i]),
     "vsb_profile_read": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vsb_debug_read": (_i, [_vp, C.c_char_p, _vp, _i64]),
+    "vsb_debug_write": (_i, [_vp, C.c_char_p, _vp, _i64]),
     "vsb_debug_tc_level": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i64, _i, _i, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
 }
 
@@ -356,6 +357,11 @@ class Index:
         if got < 0:
             self.eng.check(got)
         return out[: got // out.itemsize]
+
+    def debug_write(self, name: str, data: np.ndarray):
+        """plant an internal buffer (vsb_debug_write); "bounds": int64 [stat("sms") + 1] tile boundaries"""
+        a = np.ascontiguousarray(data, dtype=np.int64)
+        self.eng.check(self.eng.lib.vsb_debug_write(self.h, name.encode(), _ptr(a), a.nbytes))
 
     def debug_tc_level(self, metric: int, queries: np.ndarray, U: np.ndarray, r0: int, r1: int, N: int = 0, scores: bool = False,
                        cap: int = 1 << 22):

@@ -257,7 +257,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
                 rowf[h] = (KIND == TK_U8) ? __fsqrt_rn((float)(uint32_t)nn) : __fsqrt_rn((float)nn);
             } else {
                 const float nn = __uint_as_float(nbits[h]);
-                rowf[h] = (MC == MC_L2) ? -nn * (1.0f - prm.eps) : __fsqrt_rn(nn);
+                // L2: a row whose fp32 sum of squares overflowed (bf16 elements beyond ~2^64) can still have a finite distance;
+                // NaN makes it a hit, and the refine computes it exactly (special_row_distance)
+                if constexpr (MC == MC_L2) rowf[h] = (nn <= FLT_MAX) ? -nn * (1.0f - prm.eps) : __int_as_float(0x7FC00000);
+                else rowf[h] = __fsqrt_rn(nn);
             }
         }
         const uint32_t *qc = qc_s + ng * N;
@@ -572,6 +575,8 @@ __device__ inline float conservative_qc(int kind, int mc, int root, float U, con
     // DOT: d = -s < U.  |s_tc - s_refine| <= eps |q||r| <= eps |q| rnmax (rnmax = largest row norm, 1.0001 for its own rounding)
     if (mc == MC_DOT) return -U - (eps * sqrtf(qq) * rnmax * 1.0001f + 4e-7f * fabsf(U)) - 1e-30f;
     if (mc == MC_L2) {
+        // a query whose fp32 sum of squares overflowed: NaN makes every row a hit (the refine's distances are exact)
+        if (!(qq <= FLT_MAX)) return __int_as_float(0x7FC00000);
         // |q-r|^2 = qq + nn - 2 s: the score error is <= 2 eps_tc |q||r| <= eps_tc (qq + nn), so shrinking both norms by
         // (1 - eps) absorbs it (tc_scan_kernel shrinks nn the same way); the refine's own sum of squares is within
         // dim * 2^-23 relative of the true one, hence the factor on U^2

@@ -198,6 +198,7 @@ struct vsb_index {
     size_t dev_bytes = 0;
     long long st_queries = 0, st_survivors = 0, st_fallbacks = 0, st_last_survivors = 0;
     long long st_batches = 0, st_batch_cands = 0, st_batch_kept = 0, st_tc_us = 0, st_tc_rows = 0, st_batch_us = 0;
+    int last_log2p = -1, last_nsw = -1, last_direct = -1;   // plan of the most recent scan launch (vsb_index_stat "plan_*")
     void *batch = nullptr;   // BatchWs (tensor-core batch path workspace)
 };
 
@@ -462,6 +463,7 @@ int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries
     fn<<<ix->num_sms, kThreads, pl.smem, ss>>>(p);
     CU(cudaGetLastError());
     ++g_launches;
+    ix->last_log2p = pl.log2P; ix->last_nsw = pl.nsw; ix->last_direct = pl.direct ? 1 : 0;
     if (pev) CU(cudaEventRecord(pev[1], ss));
     if (k > 0) {
         CU(cudaEventRecord(wk->scanned, ss));
@@ -1083,6 +1085,10 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "fetch_bytes")) return (long long)kHeadBytes;
     if (!strcmp(name, "slots")) return kSlots;
     if (!strcmp(name, "filter_blocks")) return (ix->num_sms * kWarps + kFilterWarpsFast - 1) / kFilterWarpsFast;
+    if (!strcmp(name, "sms")) return ix->num_sms;
+    if (!strcmp(name, "plan_log2p")) return ix->last_log2p;
+    if (!strcmp(name, "plan_nsw")) return ix->last_nsw;
+    if (!strcmp(name, "plan_direct")) return ix->last_direct;
     return -1;
 }
 void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullptr; }
@@ -1240,6 +1246,35 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
     if (!src) return fail(VSB_EINVAL, "no scan has run yet");
     CU(cudaMemcpy(out, src, std::min<size_t>(have, (size_t)bytes), cudaMemcpyDeviceToHost));
     return (int)std::min<size_t>(have, (size_t)bytes);
+}
+
+int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t bytes) {
+    if (check_index(ix)) return VSB_EINVAL;
+    if (!name || !data) return fail(VSB_EINVAL, "bad debug write arguments");
+    if (strcmp(name, "bounds") != 0) return fail(VSB_EINVAL, "unknown debug buffer %s", name);
+    if (ix->streamed || !ix->d_vec) return fail(VSB_EINVAL, "the row partition belongs to a resident index");
+    const size_t want = sizeof(long long) * (size_t)(ix->num_sms + 1);
+    if (bytes != (int64_t)want) return fail(VSB_EINVAL, "bounds: %zu bytes expected (int64 x %d)", want, ix->num_sms + 1);
+    CU(cudaSetDevice(ix->device));
+    int rc = ensure_workspace(ix, 32);       // the k <= 32 workspaces: a later query with k <= 32 keeps them (and the plant)
+    if (rc) return rc;
+    const long long rpw = 32 >> make_plan(ix, 32).log2P;
+    const long long total_tiles = (ix->n + rpw - 1) / rpw;
+    if (total_tiles < 64ll * ix->num_sms)
+        return fail(VSB_EINVAL, "bounds: %lld tiles, the partition is used from %lld", total_tiles, 64ll * ix->num_sms);
+    const long long *b = (const long long *)data;
+    if (b[0] != 0 || b[ix->num_sms] != total_tiles) return fail(VSB_EINVAL, "bounds must run from 0 to %lld tiles", total_tiles);
+    for (int c = 0; c < ix->num_sms; ++c)
+        if (b[c + 1] < b[c]) return fail(VSB_EINVAL, "bounds must be non-decreasing (CTA %d)", c);
+    CU(cudaStreamSynchronize(ix->stream));
+    CU(cudaStreamSynchronize(ix->stream2));
+    CU(cudaStreamSynchronize(ix->fstream));
+    for (int i = 0; i < kWorks; ++i) {
+        Work &w = ix->work[i];
+        CU(cudaMemcpy(w.d_bounds, b, want, cudaMemcpyHostToDevice));
+        w.bounds_tiles = total_tiles;         // the next launch on this workspace uses the plant instead of equal shares
+    }
+    return VSB_OK;
 }
 
 int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1, int N, int mode,

@@ -254,8 +254,9 @@ __device__ __forceinline__ float finalize(const Accum &A, const QueryNorm qn, in
 template <int VT, int MC>
 __host__ __device__ constexpr bool has_special_policy() { return VT == T_F16 || (VT == T_BF16 && MC == MC_L2); }
 
-// after accum_reduce: does this row (or the query) hold a NaN / Inf?  (finite inputs cannot overflow these sums: f16 values
-// are <= 65504 and bf16 L2 sums of finite differences stay finite up to ~1e19 per element)
+// after accum_reduce: does this row (or the query) hold a NaN / Inf, or did its fp32 sum overflow?  f16 sums of finite inputs
+// cannot overflow (values <= 65504), but a bf16 L2 sum of squares does once a difference exceeds 2^64 (or the sum FLT_MAX),
+// while the reference's double LASSQ stays finite as long as the root does: special_row_distance recomputes those rows in double.
 template <int VT, int MC>
 __device__ __forceinline__ bool row_needs_exact(const Accum &A, const QueryNorm qn) {
     if constexpr (!has_special_policy<VT, MC>()) return false;
@@ -263,8 +264,9 @@ __device__ __forceinline__ bool row_needs_exact(const Accum &A, const QueryNorm 
     else return !(fabsf(A.s0 + A.s1) <= FLT_MAX);
 }
 
-// The reference's own element loop for one row, one thread, element order (fp32 accumulation instead of double: the result
-// classes — NaN, +Inf, -Inf, 1.0 — are exact, finite values agree to ~dim * 2^-24):
+// The reference's own element loop for one row, one thread, element order (f16: fp32 accumulation instead of double: the result
+// classes — NaN, +Inf, -Inf, 1.0 — are exact, finite values agree to ~dim * 2^-24; bf16 L2 accumulates in double, because a
+// finite LASSQ value can lie beyond the fp32 range of the sum of squares, up to (float)sqrt(sum) <= FLT_MAX):
 //   f16 L2 / L1 (:318-400): a lane with an infinity that is not paired with an equal-signed infinity -> +INF at once (checked
 //       BEFORE the NaN test); NaN lanes skipped; Inf - Inf poisons the sum (LASSQ: NaN unless every other difference is 0)
 //   f16 DOT (:402-432): NaN lanes skipped; the FIRST infinite product decides: -INF if positive, +INF if negative; Inf * 0 poisons
@@ -274,6 +276,7 @@ template <int VT, int MC>
 __device__ __noinline__ float special_row_distance(const uint8_t *row, const uint8_t *query, int nelem, int root) {
     const uint16_t *yb = reinterpret_cast<const uint16_t *>(row), *xb = reinterpret_cast<const uint16_t *>(query);
     float s = 0.0f, nx = 0.0f, ny = 0.0f;
+    double sd = 0.0;                                                            // bf16 L2
     bool poisoned = false, anynz = false;
     for (int e = 0; e < nelem; ++e) {
         float xf, yf;
@@ -287,7 +290,7 @@ __device__ __noinline__ float special_row_distance(const uint8_t *row, const uin
         if constexpr (VT == T_BF16) {                                           // bf16 L2
             const float d = xf - yf;
             if (isinf(d)) return INFINITY;
-            if (d == d) s = fmaf(d, d, s);
+            if (d == d) sd = fma((double)d, (double)d, sd);                     // exact square: |d| < 2^128 fits double's range
         } else if constexpr (MC == MC_L2 || MC == MC_L1) {
             const bool xi = isinf(xf), yi = isinf(yf);
             if ((xi || yi) && !(xi && yi && (xf > 0.0f) == (yf > 0.0f))) return INFINITY;
@@ -311,7 +314,9 @@ __device__ __noinline__ float special_row_distance(const uint8_t *row, const uin
         }
     }
     float d;
-    if constexpr (MC == MC_L2) {
+    if constexpr (VT == T_BF16) {
+        d = (float)(root ? sqrt(sd) : sd);                                     // rounded once, like lassq_result (+Inf beyond FLT_MAX)
+    } else if constexpr (MC == MC_L2) {
         if (poisoned) d = anynz ? __int_as_float(0x7FC00000) : 0.0f;           // LASSQ: scale == 0 -> 0 (:346 / :194)
         else d = root ? __fsqrt_rn(s) : s;
     } else if constexpr (MC == MC_L1) {

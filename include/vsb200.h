@@ -168,9 +168,10 @@ VSB_API int vsb_batch_merge(vsb_index *ix, const void *d_blocks, int world, int6
 VSB_API int vsb_index_lookup_rowids(const vsb_index *ix, const int64_t *seq, int64_t n, int64_t *out);
 /* ---- exchange over NVLink peer memory: one process per GPU (torchrun), no collective library on the data path -----------
  * The final all-gather of the shards' per-query result heads (SURVEY §8e; north_star "final allgather of per-shard top-k over
- * NVLink") is fused into the filter kernel: the block that completes a head stores it into row `rank` of EVERY peer's gather
- * buffer (cudaIpc-mapped peer memory) and raises an arrival flag; the receiver waits on the flags on its own stream and
- * copies the gathered heads to pinned host memory once per group.
+ * NVLink") is a store kernel: after a group's filters, push_heads_kernel (the default; option push_mode = 0: the filter block that
+ * completes a head) stores each head into row `rank` of EVERY peer's gather buffer (cudaIpc-mapped peer memory) and raises an
+ * arrival flag; the receiver waits on the flags on its own stream and copies the gathered heads to pinned host memory once per
+ * group.
  * setup (once): every rank calls vsb_exchange_export (allocates its gather buffer, returns a 64-byte cudaIpc handle), the
  * launcher all-gathers the handles (any transport: they are 64 bytes), every rank calls vsb_exchange_attach with all of them.
  * per group of 1..8 independent queries (the same call sequence on every rank): vsb_exchange_submit launches scan + filter
@@ -260,7 +261,7 @@ VSB_API int vsb_debug_write(vsb_index *ix, const char *name, const void *data, i
  * NULL.  Synchronous. */
 VSB_API int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1,
                                int N, int mode, void *out, int64_t out_cap, void *out_qc, void *out_norms, int64_t *out_count);
-/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","epi2","batch_debug","batch_m0","batch_growth","balance","fuse_mb","scan_streams","xwait_ms","epi_chunk","push_mode","push_repeat","merge_stream" (experiment)};
+/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","fuse_mb","scan_streams","xwait_ms","epi_chunk","push_mode","merge_stream" (experiment)};
  * values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);
 

@@ -51,7 +51,6 @@ int g_opt_scan_streams = 2;    // 2: consecutive scan launches alternate between
                                // as soon as the CTA of launch i on it exits (one scan CTA fits per SM): no grid-wide drain between
                                // launches, per-SM speed differences turn into an earlier start of the next query.  1: one stream.
 int g_opt_push_mode = 1;       // exchange: 1 (default) = a small kernel on the exchange stream pushes a finished group's heads; 0 = the filter's last block pushes its head itself (fused: the filter stream then waits for NVLink acknowledgements; not measured on H100)
-int g_opt_push_repeat = 1;     // experiment: push every exchange target this many times (see exchange_fill_push)
 int g_opt_xwait_ms = 10000;    // exchange: how long the receiving side waits for a peer's head before it reports an error (a dead
                                // peer, not a slow one: ranks sharing one GPU or a busy host can start a batch seconds apart)
 
@@ -109,17 +108,6 @@ constexpr int kMaxK = 256;               // candidate path; larger k uses the al
 constexpr int kSlots = 32;               // result slots: queries in flight (the sharded exchange moves groups of them; a rank may have at most
                                          // kSlots / 2 queries in flight so that a peer never overwrites a gather row that is still being read)
 
-// result block of one query, written by filter_kernel into DEVICE memory and fetched with one async copy:
-//   head = [hdr: 16 ints][table: kTableCap x int2][first kFirstFetch survivors x uint2]   (kHeadBytes, what travels)
-//   tail = the (rare) survivors beyond kFirstFetch, fetched by a second copy.
-// The heads of all slots are ONE contiguous allocation (slot s at s * kHeadBytes), so a launcher can all-gather the
-// heads of a group of consecutive slots with a single collective.  (Zero-copy writes of ~300 scattered 8-byte records
-// over PCIe made the filter kernel 5x slower than writing to HBM and copying once.)
-constexpr int kTableCap = 512;
-constexpr int kFirstFetch = 1024;
-constexpr size_t kResHdrBytes = 64 + sizeof(int2) * kTableCap;
-constexpr size_t kHeadBytes = kResHdrBytes + sizeof(uint2) * kFirstFetch;
-
 // scan workspace of ONE query (per-stream k-lists / CTA lists, in-CTA bounds, candidate logs): written by scan_kernel,
 // read by filter_kernel
 struct QWork {
@@ -140,17 +128,18 @@ struct Work {
 };
 constexpr int kWorks = 4;
 
+// A query's result head (ResultHead, scan_kernels.cuh) is written by filter_kernel into DEVICE memory and fetched with one
+// async copy; the (rare) survivors beyond kFirstFetch go to the slot's tail and are fetched by a second copy.  The heads of
+// all slots are ONE contiguous allocation (slot s at s * kHeadBytes), so a launcher can all-gather the heads of a group of
+// consecutive slots with a single collective.  (Zero-copy writes of ~300 scattered 8-byte records over PCIe made the filter
+// kernel 5x slower than writing to HBM and copying once.)
 struct Slot {
-    uint8_t *d_res = nullptr, *h_res = nullptr;      // this slot's head inside vsb_index::d_heads / h_heads
-    uint2 *h_out = nullptr, *d_out = nullptr;        // first kFirstFetch survivors (inside the head)
+    ResultHead *d_head = nullptr, *h_head = nullptr; // this slot's head inside vsb_index::d_heads / h_heads
     uint2 *h_tail = nullptr, *d_tail = nullptr;      // survivors kFirstFetch.. (inside vsb_index::d_tails / h_tails)
-    int2 *h_table = nullptr, *d_table = nullptr;
-    int *h_hdr = nullptr, *d_hdr = nullptr;
     uint8_t *h_query = nullptr, *d_query = nullptr;  // pinned staging + device copy of the query
     int *d_ctrl = nullptr;
     cudaEvent_t done = nullptr;   // recorded after the result block of this slot has been copied to the host
     int seq = 0;
-    int nblocks = 0;
 };
 
 }  // namespace
@@ -310,13 +299,10 @@ int ensure_slots_alloc(vsb_index *ix) {
     CU(cudaMemset(dc, 0, sizeof(int) * 4 * kSlots));
     for (int i = 0; i < kSlots; ++i) {
         Slot &s = ix->slot[i];
-        s.d_res = ix->d_heads + kHeadBytes * i;
-        s.h_res = ix->h_heads + kHeadBytes * i;
+        s.d_head = (ResultHead *)(ix->d_heads + kHeadBytes * i);
+        s.h_head = (ResultHead *)(ix->h_heads + kHeadBytes * i);
         s.d_tail = (uint2 *)(ix->d_tails + tail_bytes * i);
         s.h_tail = (uint2 *)(ix->h_tails + tail_bytes * i);
-        s.d_hdr = (int *)s.d_res; s.h_hdr = (int *)s.h_res;
-        s.d_table = (int2 *)(s.d_res + 64); s.h_table = (int2 *)(s.h_res + 64);
-        s.d_out = (uint2 *)(s.d_res + kResHdrBytes); s.h_out = (uint2 *)(s.h_res + kResHdrBytes);
         s.h_query = hq + (size_t)ix->pitch * i;
         s.d_query = dq + (size_t)ix->pitch * i;
         s.d_ctrl = dc + 4 * i;
@@ -333,32 +319,45 @@ int ensure_slots(vsb_index *ix) {
     return VSB_OK;
 }
 
+// waits for the scan streams and the filter stream of ix
+int drain(vsb_index *ix) {
+    CU(cudaStreamSynchronize(ix->stream));
+    CU(cudaStreamSynchronize(ix->stream2));
+    CU(cudaStreamSynchronize(ix->fstream));
+    return VSB_OK;
+}
+
+// the device buffers of a workspace (its events stay)
+void free_work(Work &w) {
+    for (QWork &q : w.q) {
+        cudaFree(q.d_lists);
+        cudaFree(q.d_logs);
+        cudaFree(q.d_counts);
+        cudaFree(q.d_tlocal);
+        q = QWork();
+    }
+    cudaFree(w.d_bounds);
+    cudaFree(w.d_cta_time);
+    w.d_bounds = nullptr; w.d_cta_time = nullptr;
+}
+
 int ensure_workspace(vsb_index *ix, int k) {
     const int kcap = (k + 31) & ~31;
     const int logcap = std::max(256, 12 * k);
     const int streams = ix->num_sms * kWarps;
     if (ix->ws_kcap >= kcap && ix->ws_logcap >= logcap && ix->ws_streams == streams) return VSB_OK;
-    CU(cudaStreamSynchronize(ix->stream));       // queries in flight still use the old workspaces
-    CU(cudaStreamSynchronize(ix->stream2));
-    CU(cudaStreamSynchronize(ix->fstream));
+    const int rc = drain(ix);       // queries in flight still use the old workspaces
+    if (rc) return rc;
     ix->ws_kcap = 0;
     for (int i = 0; i < kWorks; ++i) {
         Work &w = ix->work[i];
-        for (int g = 0; g < kMaxGroup; ++g) {
-            QWork &q = w.q[g];
-            if (q.d_lists) cudaFree(q.d_lists);
-            if (q.d_logs) cudaFree(q.d_logs);
-            if (q.d_counts) cudaFree(q.d_counts);
-            if (q.d_tlocal) cudaFree(q.d_tlocal);
-            q.d_lists = nullptr; q.d_logs = nullptr; q.d_counts = nullptr; q.d_tlocal = nullptr;
+        free_work(w);
+        for (QWork &q : w.q) {
             CU(cudaMalloc((void **)&q.d_lists, sizeof(float) * (size_t)streams * kcap));
             CU(cudaMalloc((void **)&q.d_logs, sizeof(uint2) * (size_t)streams * logcap));
             CU(cudaMalloc((void **)&q.d_counts, sizeof(int) * (size_t)streams));
             CU(cudaMalloc((void **)&q.d_tlocal, sizeof(float) * (size_t)streams));
         }
-        if (w.d_bounds) cudaFree(w.d_bounds);
-        if (w.d_cta_time) cudaFree(w.d_cta_time);
-        w.d_bounds = nullptr; w.d_cta_time = nullptr;
         w.bounds_tiles = -1;
         w.in_use = false;
         CU(cudaMalloc((void **)&w.d_bounds, sizeof(long long) * (size_t)(ix->num_sms + 1)));
@@ -492,15 +491,14 @@ int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries
             q.tlocal = wk->q[g].d_tlocal;
             q.logs = wk->q[g].d_logs;
             q.counts = wk->q[g].d_counts;
-            q.out = slot->d_out;
+            q.out = head_survivors(slot->d_head);
             q.out_tail = slot->d_tail;
-            q.table = slot->d_table;
-            q.hdr = slot->d_hdr;
+            q.table = head_table(slot->d_head);
+            q.hdr = slot->d_head;
             q.ctrl = slot->d_ctrl;
             q.seqno = ++slot->seq;
             q.xslot = (int)(slot - ix->slot);
             q.xseq = push ? exchange_next_seq(ix, q.xslot) : 0u;
-            slot->nblocks = nblocks;
         }
         f.bounds = balance ? wk->d_bounds : nullptr;
         f.cta_time = wk->d_cta_time;
@@ -523,10 +521,10 @@ int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries
         wk->in_use = true;
         if (fetch) {   // the heads of consecutive slots are contiguous: one copy when the group's slots are
             bool contiguous = true;
-            for (int g = 1; g < nq; ++g) contiguous = contiguous && slots[g]->d_res == slots[g - 1]->d_res + kHeadBytes;
-            if (contiguous) CU(cudaMemcpyAsync(slots[0]->h_res, slots[0]->d_res, kHeadBytes * (size_t)nq, cudaMemcpyDeviceToHost, ix->fstream));
+            for (int g = 1; g < nq; ++g) contiguous = contiguous && slots[g] == slots[g - 1] + 1;
+            if (contiguous) CU(cudaMemcpyAsync(slots[0]->h_head, slots[0]->d_head, kHeadBytes * (size_t)nq, cudaMemcpyDeviceToHost, ix->fstream));
             else
-                for (int g = 0; g < nq; ++g) CU(cudaMemcpyAsync(slots[g]->h_res, slots[g]->d_res, kHeadBytes, cudaMemcpyDeviceToHost, ix->fstream));
+                for (int g = 0; g < nq; ++g) CU(cudaMemcpyAsync(slots[g]->h_head, slots[g]->d_head, kHeadBytes, cudaMemcpyDeviceToHost, ix->fstream));
         }
         for (int g = 0; g < nq; ++g) CU(cudaEventRecord(slots[g]->done, ix->fstream));
     }
@@ -582,32 +580,83 @@ inline int slots_finish(SlotState &s) {  // exchange sort + INF trim (:2051-2069
     if (s.dist[s.k - 1] == inf) ++unused;
     return s.k - unused;
 }
+// offers candidates as the kernels write them, (distance bits, local row), in order; row -> rowid through to_id
+template <class ToId>
+void slots_offer_cands(SlotState &s, const uint2 *c, size_t n, ToId to_id) {
+    for (size_t i = 0; i < n; ++i) {
+        float d;
+        memcpy(&d, &c[i].x, 4);
+        slots_offer(s, d, to_id(c[i].y));
+    }
+}
+// one query through the k slots: feed(s) offers its candidates in scan order and returns VSB_OK or an error code.  *mi (null:
+// 0) is the max_index cursor the slots start from; it is updated only when feed succeeds.  Returns the row count or the error.
+template <class Feed>
+int slots_replay(int k, int *mi, double *dist, int64_t *ids, Feed feed) {
+    SlotState s{k, mi ? *mi : 0, dist, ids};
+    slots_begin(s);
+    const int rc = feed(s);
+    if (rc) return rc;
+    if (mi) *mi = s.mi;
+    return slots_finish(s);
+}
+// the max_index cursor of a scan of nq queries: a single query continues the caller's cursor and hands it back; the queries of
+// a batch are independent, like nq separate cursors that each start at 0, and leave the caller's cursor alone
+struct QueryCursor {
+    int *caller;
+    int nq, mi;
+    QueryCursor(int *max_index, int nq) : caller(max_index), nq(nq), mi(max_index ? *max_index : 0) {}
+    int *next() {   // the cursor of the next query
+        if (nq > 1) mi = 0;
+        return &mi;
+    }
+    void finish() const {
+        if (caller && nq == 1) *caller = mi;
+    }
+};
 
-// gather the survivors of a finished slot in scan order; returns count or <0
-int gather_survivors(vsb_index *ix, Slot *slot, std::vector<uint2> &out, bool *overflow) {
+// survivors a head holds itself: its headcap field when that is in (0, kFirstFetch], else kFirstFetch
+int head_capacity(const ResultHead *h) { return (h->headcap > 0 && h->headcap <= kFirstFetch) ? h->headcap : kFirstFetch; }
+
+// visits the survivors of one head in block-table order (= scan order): survivor i sits in the head below head_capacity(h),
+// else at tail[i - head_capacity(h)].  VSB_ECUDA when the block count does not fit the table (`shard` names the head).
+template <class Visit>
+int for_each_survivor(const ResultHead *h, const uint2 *tail, int shard, Visit visit) {
+    const int nblocks = h->nblocks;
+    if (nblocks < 0 || nblocks > kTableCap) return fail(VSB_ECUDA, "malformed result head from shard %d", shard);
+    const int headcap = head_capacity(h);
+    const int2 *table = head_table(h);
+    const uint2 *out = head_survivors(h);
+    for (int b = 0; b < nblocks; ++b)
+        for (int i = 0; i < table[b].y; ++i) {
+            const int at = table[b].x + i;
+            visit(at < headcap ? out[at] : tail[at - headcap]);
+        }
+    return VSB_OK;
+}
+
+// waits for the query of a slot and visits its survivors in scan order; *overflow: its candidates overflowed, nothing is visited
+template <class Visit>
+int visit_survivors(vsb_index *ix, Slot *slot, bool *overflow, Visit visit) {
+    CU(cudaEventSynchronize(slot->done));
     *overflow = false;
-    if (slot->h_hdr[2] != slot->seq) return fail(VSB_ECUDA, "scan result header not published (seq %d != %d)", slot->h_hdr[2], slot->seq);
-    if (slot->h_hdr[1]) { *overflow = true; return 0; }
-    const int total = slot->h_hdr[0];
-    if (total > kFirstFetch) {  // rare: fetch the tail of the survivor list
-        if (cudaMemcpyAsync(slot->h_tail, slot->d_tail, sizeof(uint2) * (size_t)(total - kFirstFetch),
+    const ResultHead *h = slot->h_head;
+    if (h->seq != slot->seq) return fail(VSB_ECUDA, "scan result header not published (seq %d != %d)", h->seq, slot->seq);
+    if (h->flags) { *overflow = true; return VSB_OK; }
+    const int total = h->total, headcap = head_capacity(h);
+    if (total > headcap) {  // rare: fetch the tail of the survivor list
+        if (cudaMemcpyAsync(slot->h_tail, slot->d_tail, sizeof(uint2) * (size_t)(total - headcap),
                             cudaMemcpyDeviceToHost, ix->fstream) != cudaSuccess ||
             cudaStreamSynchronize(ix->fstream) != cudaSuccess)
             return fail(VSB_ECUDA, "fetching %d survivors failed: %s", total, cudaGetErrorString(cudaGetLastError()));
     }
-    out.clear();
-    out.reserve((size_t)total);
-    for (int b = 0; b < slot->nblocks; ++b) {
-        const int2 t = slot->h_table[b];
-        for (int i = 0; i < t.y; ++i) {
-            const int at = t.x + i;
-            out.push_back(at < kFirstFetch ? slot->h_out[at] : slot->h_tail[at - kFirstFetch]);
-        }
-    }
+    long long n = 0;
+    const int rc = for_each_survivor(h, slot->h_tail, 0, [&](uint2 c) { ++n; visit(c); });
+    if (rc) return rc;
     ix->st_queries++;
-    ix->st_survivors += (long long)out.size();
-    ix->st_last_survivors = (long long)out.size();
-    return (int)out.size();
+    ix->st_survivors += n;
+    ix->st_last_survivors = n;
+    return VSB_OK;
 }
 
 int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *out_dist);
@@ -690,80 +739,68 @@ int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *
 
 // candidates of a streamed index: every window's survivors, in scan order, rows made column-global
 int streamed_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k, std::vector<uint2> &cands, bool *overflow) {
-    cands.clear();
     *overflow = false;
     const int depth = 4;                                  // result slots 0..3 rotate over the windows
-    std::vector<uint2> part;
     return stream_windows(ix, depth,
         [&](long long, const uint8_t *vec, long long rows, int s) {
             Slot *slot = &ix->slot[s];
             return launch_scan_group(ix, metric, &d_query, 1, k, &slot, nullptr, true, ix->stream, false, vec, rows);
         },
         [&](long long, long long r0, long long, int s) {
-            Slot *slot = &ix->slot[s];
-            CU(cudaEventSynchronize(slot->done));
             bool ovf = false;
-            const int n = gather_survivors(ix, slot, part, &ovf);
-            if (n < 0) return n;
+            const int rc = visit_survivors(ix, &ix->slot[s], &ovf, [&](uint2 c) { cands.push_back(make_uint2(c.x, c.y + (uint32_t)r0)); });
+            if (rc) return rc;
             if (ovf) *overflow = true;
-            for (const uint2 &c : part) cands.push_back(make_uint2(c.x, c.y + (uint32_t)r0));
             return (int)VSB_OK;
         });
+}
+
+// the all-distances fallback (k > kMaxK, candidate overflow): every row is a candidate, in scan order
+int all_candidates(vsb_index *ix, int metric, const uint8_t *d_query, std::vector<uint2> &cands) {
+    ix->st_fallbacks++;
+    std::vector<float> dist;
+    const int rc = scan_all_into(ix, metric, d_query, dist);
+    if (rc) return rc;
+    cands.resize((size_t)ix->n);
+    for (long long i = 0; i < ix->n; ++i) {
+        uint32_t bits;
+        memcpy(&bits, &dist[(size_t)i], 4);
+        cands[(size_t)i] = make_uint2(bits, (uint32_t)i);
+    }
+    return VSB_OK;
+}
+
+// stages one host query on ix->stream into the slot of the synchronous calls (streamed: slots 0..3 rotate over the windows,
+// the query is parked in the last one)
+int stage_host_query(vsb_index *ix, const void *query, Slot **slot) {
+    CU(cudaSetDevice(ix->device));
+    const int rc = ensure_slots(ix);
+    if (rc) return rc;
+    *slot = &ix->slot[ix->streamed ? kSlots - 1 : 0];
+    return stage_query(ix, *slot, query, ix->stream);
 }
 
 // one query, host in / candidates out (sorted by scan order).  Falls back to the all-distances kernel when the
 // candidate log overflowed or k is larger than the candidate path supports (still GPU-computed distances).
 int query_candidates(vsb_index *ix, int metric, const void *query, int k, std::vector<uint2> &cands) {
-    CU(cudaSetDevice(ix->device));
-    int rc = ensure_slots(ix);
+    Slot *slot = nullptr;
+    int rc = stage_host_query(ix, query, &slot);   // synchronous call: one stream (a possible all-distances fallback reads d_query on it)
     if (rc) return rc;
-    Slot *slot = &ix->slot[ix->streamed ? kSlots - 1 : 0];   // streamed: slots 0..3 rotate over the windows, the query is parked in the last one
-    rc = stage_query(ix, slot, query, ix->stream);   // synchronous call: one stream (a possible all-distances fallback reads d_query on it)
-    if (rc) return rc;
+    cands.clear();
+    cands.reserve(kFirstFetch);                    // one allocation for the usual few hundred survivors
     bool overflow = (k > kMaxK);
-    if (ix->streamed) {
-        if (!overflow) {
-            rc = ensure_workspace(ix, k);
-            if (rc) return rc;
-            rc = streamed_candidates(ix, metric, slot->d_query, k, cands, &overflow);
-            if (rc) return rc;
-        }
-        if (overflow) {
-            ix->st_fallbacks++;
-            std::vector<float> dist;
-            rc = scan_all_into(ix, metric, slot->d_query, dist);
-            if (rc) return rc;
-            cands.resize((size_t)ix->n);
-            for (long long i = 0; i < ix->n; ++i) {
-                uint32_t bits;
-                memcpy(&bits, &dist[(size_t)i], 4);
-                cands[(size_t)i] = make_uint2(bits, (uint32_t)i);
-            }
-        }
-        return VSB_OK;
-    }
     if (!overflow) {
         rc = ensure_workspace(ix, k);
         if (rc) return rc;
-        rc = launch_scan(ix, metric, slot->d_query, k, slot, nullptr, true, ix->stream);
-        if (rc) return rc;
-        CU(cudaEventSynchronize(slot->done));
-        int n = gather_survivors(ix, slot, cands, &overflow);
-        if (n < 0) return n;
-    }
-    if (overflow) {
-        ix->st_fallbacks++;
-        std::vector<float> dist;
-        rc = scan_all_into(ix, metric, slot->d_query, dist);
-        if (rc) return rc;
-        cands.resize((size_t)ix->n);
-        for (long long i = 0; i < ix->n; ++i) {
-            uint32_t bits;
-            memcpy(&bits, &dist[(size_t)i], 4);
-            cands[(size_t)i] = make_uint2(bits, (uint32_t)i);
+        if (ix->streamed) {
+            rc = streamed_candidates(ix, metric, slot->d_query, k, cands, &overflow);
+        } else {
+            rc = launch_scan(ix, metric, slot->d_query, k, slot, nullptr, true, ix->stream);
+            if (rc == VSB_OK) rc = visit_survivors(ix, slot, &overflow, [&](uint2 c) { cands.push_back(c); });
         }
+        if (rc) return rc;
     }
-    return VSB_OK;
+    return overflow ? all_candidates(ix, metric, slot->d_query, cands) : VSB_OK;
 }
 
 int check_index(const vsb_index *ix) {
@@ -858,7 +895,6 @@ int vsb_set_option(const char *name, int value) {
     else if (!strcmp(name, "batch_debug")) p = &g_opt_batch_debug;
     else if (!strcmp(name, "scan_streams")) p = &g_opt_scan_streams;
     else if (!strcmp(name, "xwait_ms")) p = &g_opt_xwait_ms;
-    else if (!strcmp(name, "push_repeat")) p = &g_opt_push_repeat;
     else if (!strcmp(name, "push_mode")) p = &g_opt_push_mode;
     if (!p) return fail(VSB_EINVAL, "unknown option %s", name);
     if (value < 0) return fail(VSB_EINVAL, "option %s: values are non-negative", name);   // so that a negative return is always an error
@@ -954,6 +990,21 @@ static int stage_acquire(vsb_index *ix, int *which) {
     return VSB_OK;
 }
 
+// explicit rowids from now on: the implicit ids of the rows appended so far become a list
+static void materialise_rowids(vsb_index *ix) {
+    if (!ix->implicit_ids) return;
+    ix->h_rowids.resize((size_t)ix->n);
+    for (long long i = 0; i < ix->n; ++i) ix->h_rowids[(size_t)i] = ix->first_seq + i + 1;
+    ix->implicit_ids = false;
+}
+
+// the little-endian int64 rowid in front of a preloaded vector (INT64_FROM_INT8PTR, :86-94)
+static int64_t inline_rowid(const uint8_t *row) {
+    uint64_t v = 0;
+    for (int i = 7; i >= 0; --i) v = (v << 8) | row[i];
+    return (int64_t)v;
+}
+
 // src_stride: bytes between rows in host memory; src_off: offset of the vector inside a row
 static int append_rows(vsb_index *ix, const uint8_t *src, size_t src_stride, size_t src_off, const int64_t *rowids,
                        bool ids_inline, int64_t nrows) {
@@ -962,13 +1013,7 @@ static int append_rows(vsb_index *ix, const uint8_t *src, size_t src_stride, siz
     CU(cudaSetDevice(ix->device));
     const size_t rowbytes = (size_t)ix->dim * ix->esize;
     const size_t pitch = (size_t)ix->pitch;
-    const bool have_ids = ids_inline || rowids != nullptr;
-    if (have_ids && ix->implicit_ids) {
-        // materialise the implicit ids of rows appended so far
-        ix->h_rowids.resize((size_t)ix->n);
-        for (long long i = 0; i < ix->n; ++i) ix->h_rowids[(size_t)i] = ix->first_seq + i + 1;
-        ix->implicit_ids = false;
-    }
+    if (ids_inline || rowids != nullptr) materialise_rowids(ix);
     if (pitch > kStageBuf) return fail(VSB_ERANGE, "row pitch %zu exceeds the %zu-byte staging buffer", pitch, (size_t)kStageBuf);
     const int64_t per_buf = (int64_t)(kStageBuf / pitch);
     int64_t done = 0;
@@ -978,11 +1023,7 @@ static int append_rows(vsb_index *ix, const uint8_t *src, size_t src_stride, siz
             uint8_t *dst = ix->h_arena + (size_t)(ix->n + r) * pitch;
             memcpy(dst, row + src_off, rowbytes);
             if (pitch > rowbytes) memset(dst + rowbytes, 0, pitch - rowbytes);
-            if (ids_inline) {
-                uint64_t v = 0;
-                for (int i = 7; i >= 0; --i) v = (v << 8) | row[i];
-                ix->h_rowids.push_back((int64_t)v);
-            }
+            if (ids_inline) ix->h_rowids.push_back(inline_rowid(row));
         }
         done = nrows;
     }
@@ -996,11 +1037,7 @@ static int append_rows(vsb_index *ix, const uint8_t *src, size_t src_stride, siz
             const uint8_t *row = src + (size_t)(done + r) * src_stride;
             memcpy(dst + (size_t)r * pitch, row + src_off, rowbytes);
             if (pitch > rowbytes) memset(dst + (size_t)r * pitch + rowbytes, 0, pitch - rowbytes);
-            if (ids_inline) {
-                uint64_t v = 0;  // little-endian int64 rowid in front of the vector (INT64_FROM_INT8PTR, :86-94)
-                for (int i = 7; i >= 0; --i) v = (v << 8) | row[i];
-                ix->h_rowids.push_back((int64_t)v);
-            }
+            if (ids_inline) ix->h_rowids.push_back(inline_rowid(row));
         }
         CU(cudaMemcpyAsync(ix->d_vec + (size_t)(ix->n + done) * pitch, dst, (size_t)m * pitch, cudaMemcpyHostToDevice, ix->stream));
         CU(cudaEventRecord(ix->stage_ev[b], ix->stream));
@@ -1039,11 +1076,7 @@ int vsb_index_append_device(vsb_index *ix, const void *d_vectors, const int64_t 
     CU(cudaMemcpy2DAsync(ix->d_vec + (size_t)ix->n * ix->pitch, (size_t)ix->pitch, d_vectors, rowbytes, rowbytes, (size_t)nrows,
                          cudaMemcpyDeviceToDevice, ix->stream));
     if (d_rowids) {
-        if (ix->implicit_ids) {
-            ix->h_rowids.resize((size_t)ix->n);
-            for (long long i = 0; i < ix->n; ++i) ix->h_rowids[(size_t)i] = ix->first_seq + i + 1;
-            ix->implicit_ids = false;
-        }
+        materialise_rowids(ix);
         ix->h_rowids.resize((size_t)(ix->n + nrows));
         CU(cudaMemcpyAsync(ix->h_rowids.data() + ix->n, d_rowids, sizeof(int64_t) * (size_t)nrows, cudaMemcpyDeviceToHost, ix->stream));
     } else if (!ix->implicit_ids) {
@@ -1096,26 +1129,16 @@ void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullpt
 void vsb_index_free(vsb_index *ix) {
     if (!ix) return;
     cudaSetDevice(ix->device);
-    if (ix->stream) cudaStreamSynchronize(ix->stream);
-    if (ix->stream2) cudaStreamSynchronize(ix->stream2);
-    if (ix->fstream) cudaStreamSynchronize(ix->fstream);
-    if (ix->xstream) cudaStreamSynchronize(ix->xstream);
+    drain(ix);                      // the streams exist: index_create deletes an index whose streams it could not create
+    cudaStreamSynchronize(ix->xstream);
     exchange_free(ix);
     for (int b = 0; b < 2; ++b) {
         if (ix->stage[b]) cudaFreeHost(ix->stage[b]);
         if (ix->stage_ev[b]) cudaEventDestroy(ix->stage_ev[b]);
     }
     free_slots(ix);
-    for (int i = 0; i < kWorks; ++i) {
-        Work &w = ix->work[i];
-        for (int g = 0; g < kMaxGroup; ++g) {
-            if (w.q[g].d_lists) cudaFree(w.q[g].d_lists);
-            if (w.q[g].d_logs) cudaFree(w.q[g].d_logs);
-            if (w.q[g].d_counts) cudaFree(w.q[g].d_counts);
-            if (w.q[g].d_tlocal) cudaFree(w.q[g].d_tlocal);
-        }
-        if (w.d_bounds) cudaFree(w.d_bounds);
-        if (w.d_cta_time) cudaFree(w.d_cta_time);
+    for (Work &w : ix->work) {
+        free_work(w);
         if (w.scanned) cudaEventDestroy(w.scanned);
         if (w.drained) cudaEventDestroy(w.drained);
     }
@@ -1156,36 +1179,28 @@ int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k,
         ix->st_fallbacks++;                      // capacity exceeded: per-query path below
     }
     std::vector<uint2> cands;
-    int mi = max_index ? *max_index : 0;
+    QueryCursor cur(max_index, nq);
     for (int b = 0; b < nq; ++b) {
-        if (nq > 1) mi = 0;                      // batches: independent queries, like B separate cursors
         int rc = query_candidates(ix, metric, (const uint8_t *)queries + (size_t)b * qbytes, k, cands);
         if (rc) return rc;
-        SlotState s{k, mi, out_dist + (size_t)b * k, out_rowids + (size_t)b * k};
-        slots_begin(s);
-        for (const uint2 &c : cands) {
-            float d;
-            memcpy(&d, &c.x, 4);
-            slots_offer(s, d, rowid_of(ix, c.y));
-        }
-        mi = s.mi;
-        const int cnt = slots_finish(s);
+        const int cnt = slots_replay(k, cur.next(), out_dist + (size_t)b * k, out_rowids + (size_t)b * k, [&](SlotState &s) {
+            slots_offer_cands(s, cands.data(), cands.size(), [&](uint32_t row) { return rowid_of(ix, row); });
+            return (int)VSB_OK;
+        });
         if (out_counts) out_counts[b] = cnt;
     }
-    if (max_index && nq == 1) *max_index = mi;
+    cur.finish();
     return VSB_OK;
 }
 
 int vsb_scan_all(vsb_index *ix, int metric, const void *query, float *out_dist, int64_t *out_rowids) {
     if (check_index(ix)) return VSB_EINVAL;
     if (!query || !out_dist) return fail(VSB_EINVAL, "bad scan arguments");
-    CU(cudaSetDevice(ix->device));
-    int rc = ensure_slots(ix);
-    if (rc) return rc;
-    rc = stage_query(ix, &ix->slot[0], query, ix->stream);
+    Slot *slot = nullptr;
+    int rc = stage_host_query(ix, query, &slot);
     if (rc) return rc;
     std::vector<float> dist;
-    rc = scan_all_into(ix, metric, ix->slot[0].d_query, dist);
+    rc = scan_all_into(ix, metric, slot->d_query, dist);
     if (rc) return rc;
     memcpy(out_dist, dist.data(), sizeof(float) * (size_t)ix->n);
     if (out_rowids)
@@ -1223,20 +1238,18 @@ int vsb_scan_candidates(vsb_index *ix, int metric, const void *queries, int nq, 
 int vsb_replay_topk(const vsb_candidate *cands, int n, int k, int *max_index, int64_t *out_rowids, double *out_dist) {
     if (k <= 0) return 0;
     if ((!cands && n > 0) || !out_rowids || !out_dist) return fail(VSB_EINVAL, "bad replay arguments");
-    SlotState s{k, max_index ? *max_index : 0, out_dist, out_rowids};
-    slots_begin(s);
-    for (int i = 0; i < n; ++i) slots_offer(s, cands[i].dist, cands[i].rowid);
-    if (max_index) *max_index = s.mi;
-    return slots_finish(s);
+    return slots_replay(k, max_index, out_dist, out_rowids, [&](SlotState &s) {
+        for (int i = 0; i < n; ++i) slots_offer(s, cands[i].dist, cands[i].rowid);
+        return (int)VSB_OK;
+    });
 }
 
 int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
     if (check_index(ix)) return VSB_EINVAL;
     if (!name || !out || bytes <= 0) return fail(VSB_EINVAL, "bad debug read arguments");
     CU(cudaSetDevice(ix->device));
-    CU(cudaStreamSynchronize(ix->stream));
-    CU(cudaStreamSynchronize(ix->stream2));
-    CU(cudaStreamSynchronize(ix->fstream));
+    const int rc = drain(ix);
+    if (rc) return rc;
     const Work &w = ix->work[(ix->ws_next + kWorks - 1) % kWorks];     // the workspace of the most recent query
     const void *src = nullptr;
     size_t have = 0;
@@ -1266,9 +1279,8 @@ int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t b
     if (b[0] != 0 || b[ix->num_sms] != total_tiles) return fail(VSB_EINVAL, "bounds must run from 0 to %lld tiles", total_tiles);
     for (int c = 0; c < ix->num_sms; ++c)
         if (b[c + 1] < b[c]) return fail(VSB_EINVAL, "bounds must be non-decreasing (CTA %d)", c);
-    CU(cudaStreamSynchronize(ix->stream));
-    CU(cudaStreamSynchronize(ix->stream2));
-    CU(cudaStreamSynchronize(ix->fstream));
+    rc = drain(ix);
+    if (rc) return rc;
     for (int i = 0; i < kWorks; ++i) {
         Work &w = ix->work[i];
         CU(cudaMemcpy(w.d_bounds, b, want, cudaMemcpyHostToDevice));
@@ -1289,9 +1301,8 @@ int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, c
 int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double *filter_ms, int *filter_launches) {
     if (check_index(ix)) return VSB_EINVAL;
     CU(cudaSetDevice(ix->device));
-    CU(cudaStreamSynchronize(ix->stream));
-    CU(cudaStreamSynchronize(ix->stream2));
-    CU(cudaStreamSynchronize(ix->fstream));
+    const int rc = drain(ix);
+    if (rc) return rc;
     double a = 0, b = 0;
     int na = 0, nb = 0;
     for (size_t i = 0; i < ix->prof_kind.size(); ++i) {
@@ -1355,7 +1366,7 @@ int vsb_result_block(vsb_index *ix, int slot_id, void **d_block, int64_t *bytes)
     CU(cudaSetDevice(ix->device));
     int rc = ensure_slots(ix);
     if (rc) return rc;
-    if (d_block) *d_block = ix->slot[slot_id].d_res;
+    if (d_block) *d_block = ix->slot[slot_id].d_head;
     if (bytes) *bytes = (int64_t)kHeadBytes;
     return VSB_OK;
 }
@@ -1428,20 +1439,12 @@ int vsb_collect(vsb_index *ix, int slot_id, int k, int64_t *out_rowids, double *
     if (check_index(ix)) return VSB_EINVAL;
     if (slot_id < 0 || slot_id >= kSlots || !ix->slots_ready) return fail(VSB_EINVAL, "bad slot");
     CU(cudaSetDevice(ix->device));
-    CU(cudaEventSynchronize(ix->slot[slot_id].done));   // only this query's result; a later launch may still be running
-    std::vector<uint2> cands;
     bool overflow = false;
-    int n = gather_survivors(ix, &ix->slot[slot_id], cands, &overflow);
-    if (n < 0) return n;
+    const int cnt = slots_replay(k, nullptr, out_dist, out_rowids, [&](SlotState &s) {   // waits for this query only; a later launch may still run
+        return visit_survivors(ix, &ix->slot[slot_id], &overflow, [&](uint2 c) { slots_offer_cands(s, &c, 1, [&](uint32_t row) { return rowid_of(ix, row); }); });
+    });
+    if (cnt < 0) return cnt;
     if (overflow) return fail(VSB_ERANGE, "candidate log overflowed; use vsb_scan_topk (host query) for this input");
-    SlotState s{k, 0, out_dist, out_rowids};
-    slots_begin(s);
-    for (const uint2 &c : cands) {
-        float d;
-        memcpy(&d, &c.x, 4);
-        slots_offer(s, d, rowid_of(ix, c.y));
-    }
-    const int cnt = slots_finish(s);
     if (out_count) *out_count = cnt;
     return VSB_OK;
 }

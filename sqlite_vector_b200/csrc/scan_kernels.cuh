@@ -20,6 +20,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <float.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace vsb {
@@ -650,6 +651,36 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
 // bound.  We use  min( k-th smallest over all streams of earlier segments,
 //                      k-th smallest over the earlier streams of the same segment ),
 // both built from the streams' final k-lists (each contains the k smallest values of its stream).
+// Result head of one query, written by filter_kernel; this is what a host copy or a peer push moves:
+//   [ResultHead, 64 B][block table: kTableCap x int2 (base, count)][first kFirstFetch survivors x uint2 (dist bits, local row)]
+// The survivors of block b are base .. base + count - 1 of the survivor list, and the blocks in table order are the scan order.
+// Survivors beyond the head's capacity go to a separate tail area.
+constexpr int kTableCap = 512;
+constexpr int kFirstFetch = 1024;
+constexpr int kHeadOverflow = 1;    // flags: the candidate log or the survivor list overflowed (all-distances fallback)
+constexpr int kHeadPeerLate = 8;    // flags: exchange_wait_kernel gave up waiting for this head (set with a plain store)
+struct ResultHead {
+    int total;          // survivors
+    int flags;          // kHeadOverflow, kHeadPeerLate
+    int seq;            // the slot's query sequence number
+    int nblocks;        // filter blocks = entries of the block table
+    int xseq;           // exchange sequence number (pushed heads)
+    int src;            // shard that wrote the head (pushed heads)
+    int headcap;        // survivors stored in the head itself
+    int pad[9];
+};
+static_assert(sizeof(ResultHead) == 64, "the header is 8 uint2 words (push_one_head)");
+static_assert(offsetof(ResultHead, total) == 0 && offsetof(ResultHead, flags) == 4 && offsetof(ResultHead, seq) == 8 &&
+                  offsetof(ResultHead, nblocks) == 12 && offsetof(ResultHead, xseq) == 16 && offsetof(ResultHead, src) == 20 &&
+                  offsetof(ResultHead, headcap) == 24,
+              "tests/test_result_head.py builds heads with these offsets");
+constexpr size_t kResHdrBytes = sizeof(ResultHead) + sizeof(int2) * kTableCap;
+constexpr size_t kHeadBytes = kResHdrBytes + sizeof(uint2) * kFirstFetch;
+inline int2 *head_table(ResultHead *h) { return reinterpret_cast<int2 *>(h + 1); }
+inline const int2 *head_table(const ResultHead *h) { return reinterpret_cast<const int2 *>(h + 1); }
+inline uint2 *head_survivors(ResultHead *h) { return reinterpret_cast<uint2 *>(reinterpret_cast<uint8_t *>(h) + kResHdrBytes); }
+inline const uint2 *head_survivors(const ResultHead *h) { return reinterpret_cast<const uint2 *>(reinterpret_cast<const uint8_t *>(h) + kResHdrBytes); }
+
 struct FilterQuery {    // per-query pointers of a (group) launch: blockIdx.y selects the query
     const float *lists; // k <= 32: [S / kWarps][32] sorted CTA lists; else [S][kcap] stream lists
     const float *tlocal;// k <= 32: [S] in-CTA prefix bound of each stream (from scan_kernel)
@@ -658,25 +689,25 @@ struct FilterQuery {    // per-query pointers of a (group) launch: blockIdx.y se
     uint2 *out;         // survivors (dist bits, local row), grouped by block in stream order: the first headcap of them
     uint2 *out_tail;    //   go to out (inside the slot's head, the part that travels), the rest to out_tail
     int2 *table;        // [gridDim.x] (base, count) of each block's survivors in out
-    int *hdr;           // hdr[0] = total survivors, hdr[1] = overflow flag, hdr[2] = sequence number
+    ResultHead *hdr;
     int *ctrl;          // device: [0] cursor, [1] overflow from scan_kernel, [2] blocks done
     int seqno;
     int xslot;          // push: slot row of the targets' gather buffers
-    unsigned xseq;      // push: exchange sequence number published with the head (hdr[4]) and raised on the flags
+    unsigned xseq;      // push: exchange sequence number published with the head (ResultHead::xseq) and raised on the flags
 };
 
-// NVLink peer-memory all-gather, fused into the filter: the block that completes a query's result head copies the used part
-// of it (header, block table, survivors) straight into the gather buffer of every target GPU — peer memory mapped through
-// cudaIpc (one process per GPU) or cudaDeviceEnablePeerAccess (one process, several GPUs) — and then raises that target's
-// arrival flag with a system-scope release store.  No NCCL kernel, no extra launch, no host synchronisation: the receiving
-// side waits on the flags with exchange_wait_kernel on ITS stream and copies the gathered heads to the host.
+// NVLink peer-memory all-gather: push_heads_kernel after a group's filters (default), or the filter block that completes a
+// query's result head (option push_mode = 0), copies the used part of the head (header, block table, survivors) straight into
+// the gather buffer of every target GPU — peer memory mapped through cudaIpc (one process per GPU) or
+// cudaDeviceEnablePeerAccess (one process, several GPUs) — and then raises that target's arrival flag with a system-scope
+// release store.  No NCCL kernel, no host synchronisation: the receiving side waits on the flags with exchange_wait_kernel on
+// ITS stream and copies the gathered heads to the host.
 constexpr int kMaxPeers = 16;
 struct PushParams {
     int ntargets;                 // 0: nothing is pushed (single shard)
     int src;                      // this shard's index inside a slot's gather row
-    int world;                    // shards per slot in the gather layout [slots][world][head_bytes]
-    int head_bytes, res_hdr_bytes;// layout of a head: [hdr 64 B][table][survivors from res_hdr_bytes on]
-    int tailcap;                  // survivors beyond the head's headcap travel to a separate tail row of this many entries
+    int world;                    // shards per slot in the gather layout [slots][world][kHeadBytes]
+    int tailcap;                 // survivors beyond the head's headcap travel to a separate tail row of this many entries
     uint8_t *gather[kMaxPeers];   // target t: base of its gather buffer
     unsigned *flags[kMaxPeers];   // target t: [slots][world] arrival flags (the exchange sequence number of the slot)
     uint2 *tails[kMaxPeers];      // target t: [slots][world][tailcap] tail rows (k > 32 on large shards: > headcap survivors)
@@ -692,12 +723,12 @@ __device__ __forceinline__ unsigned ld_acquire_sys(const unsigned *p) {
 }
 
 // receiving side: one thread per (slot of the group, source shard) spins until that shard's flag carries the expected
-// sequence number.  Bounded: after `timeout` clock cycles the missing head is marked (hdr[1] |= 8) so that the merge reports
-// an error instead of the GPU hanging on a peer that died.
+// sequence number.  Bounded: after `timeout` clock cycles the missing head's flags are set to kHeadPeerLate (a plain store:
+// whatever else the head holds is stale) so that the merge reports an error instead of the GPU hanging on a peer that died.
 struct WaitParams {
     const unsigned *flags;        // [slots][world]
-    uint8_t *gather;              // [slots][world][head_bytes] (local)
-    int world, first_slot, nq, head_bytes;
+    uint8_t *gather;              // [slots][world][kHeadBytes] (local)
+    int world, first_slot, nq;
     unsigned xseq[kMaxGroup];
     long long timeout;
 };
@@ -709,7 +740,7 @@ __global__ void exchange_wait_kernel(const WaitParams wp) {
     const long long t0 = clock64();
     while (ld_acquire_sys(wp.flags + at) != wp.xseq[j]) {
         if (clock64() - t0 > wp.timeout) {
-            reinterpret_cast<int *>(wp.gather + at * wp.head_bytes)[1] = 8;
+            reinterpret_cast<ResultHead *>(wp.gather + at * kHeadBytes)->flags = kHeadPeerLate;
             break;
         }
         __nanosleep(200);
@@ -720,18 +751,18 @@ __global__ void exchange_wait_kernel(const WaitParams wp) {
 // headcap from the slot's tail area) into row (xslot, src) of every target and raises the targets' flags.  All threads of the
 // block call it; the caller guarantees that the head is complete and visible (filter_kernel: last block; push_heads_kernel:
 // stream order after the filters).
-__device__ __forceinline__ void push_one_head(const PushParams &pp, const int *hdr, const uint2 *out, const uint2 *out_tail, int xslot, unsigned xseq,
-                                              int headcap) {
-    const int total = max(__ldcg(hdr), 0), nblocks = __ldcg(hdr + 3);
-    const int nhead = 8 + nblocks;                                         // uint2 words of header + block table
+__device__ __forceinline__ void push_one_head(const PushParams &pp, const ResultHead *hdr, const uint2 *out, const uint2 *out_tail, int xslot,
+                                              unsigned xseq, int headcap) {
+    const int total = max(__ldcg(&hdr->total), 0), nblocks = __ldcg(&hdr->nblocks);
+    const int nhead = (int)(sizeof(ResultHead) / sizeof(uint2)) + nblocks;   // uint2 words of header + block table
     const int nsurv = min(total, headcap);
     const int ntail = min(max(total - headcap, 0), pp.tailcap);
     const uint2 *src_head = reinterpret_cast<const uint2 *>(hdr);
     const size_t row = (size_t)xslot * pp.world + pp.src;
     for (int t = 0; t < pp.ntargets; ++t) {
-        uint8_t *dst = pp.gather[t] + row * (size_t)pp.head_bytes;
+        uint8_t *dst = pp.gather[t] + row * kHeadBytes;
         uint2 *dh = reinterpret_cast<uint2 *>(dst);
-        uint2 *ds = reinterpret_cast<uint2 *>(dst + pp.res_hdr_bytes);
+        uint2 *ds = reinterpret_cast<uint2 *>(dst + kResHdrBytes);
         for (int i = (int)threadIdx.x; i < nhead; i += (int)blockDim.x) dh[i] = __ldcg(src_head + i);
         for (int i = (int)threadIdx.x; i < nsurv; i += (int)blockDim.x) ds[i] = __ldcg(out + i);
         if (ntail > 0) {
@@ -749,7 +780,7 @@ __device__ __forceinline__ void push_one_head(const PushParams &pp, const int *h
 struct PushGroupParams {
     PushParams push;
     int nq, headcap;
-    const int *hdr[kMaxGroup];
+    const ResultHead *hdr[kMaxGroup];
     const uint2 *out[kMaxGroup];
     const uint2 *out_tail[kMaxGroup];
     int xslot[kMaxGroup];
@@ -1000,13 +1031,13 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
             __threadfence();
             const int total = atomicAdd(&fq.ctrl[0], 0);
             const int ovf = atomicAdd(&fq.ctrl[1], 0);
-            fq.hdr[0] = total;
-            fq.hdr[1] = (ovf != 0 || total > fp.outcap) ? 1 : 0;
-            fq.hdr[2] = fq.seqno;
-            fq.hdr[3] = (int)gridDim.x;
-            fq.hdr[4] = (int)fq.xseq;
-            fq.hdr[5] = fp.push.src;
-            fq.hdr[6] = fp.headcap;
+            fq.hdr->total = total;
+            fq.hdr->flags = (ovf != 0 || total > fp.outcap) ? kHeadOverflow : 0;
+            fq.hdr->seq = fq.seqno;
+            fq.hdr->nblocks = (int)gridDim.x;
+            fq.hdr->xseq = (int)fq.xseq;
+            fq.hdr->src = fp.push.src;
+            fq.hdr->headcap = fp.headcap;
             fq.ctrl[0] = 0; fq.ctrl[1] = 0; fq.ctrl[2] = 0;
         }
         is_last = last;

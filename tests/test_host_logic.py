@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from oracle import pyoracle as po
+from tests.test_result_head import HEAD_BYTES, make_head
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -200,23 +201,14 @@ def test_merge_result_blocks_matches_oracle(oracle):
     x = rng.integers(-3, 4, (n, dim)).astype(np.int8)
     q = rng.integers(-3, 4, dim).astype(np.int8)
     bounds = [0, 400, 1100, n]
-    HDR, TABLE, FIRST = 64, 512 * 8, 1024
-    stride = HDR + TABLE + FIRST * 8
-    blocks = np.zeros(world * stride, dtype=np.uint8)
+    heads = []
     for r in range(world):
         lo, hi = bounds[r], bounds[r + 1]
         diff = x[lo:hi].astype(np.int32) - q.astype(np.int32)
         d = np.sqrt((diff * diff).sum(1).astype(np.float32))
-        blk = blocks[r * stride:(r + 1) * stride]
-        hdr = blk[:HDR].view(np.int32)
-        hdr[0], hdr[1], hdr[2], hdr[3] = hi - lo, 0, 1, 2            # total, overflow, seq, filter blocks
-        table = blk[HDR:HDR + TABLE].view(np.int32).reshape(-1, 2)
         half = (hi - lo) // 2
-        table[0] = (0, half); table[1] = (half, hi - lo - half)      # two "filter blocks", contiguous in scan order
-        out = blk[HDR + TABLE:].view(np.uint32).reshape(-1, 2)
-        out[:hi - lo, 0] = d.view(np.uint32)
-        out[:hi - lo, 1] = np.arange(hi - lo, dtype=np.uint32)
-    ids, dist = eng.merge_result_blocks(blocks, world, stride, np.array(bounds[:world]), k)
+        heads.append(make_head(d, [(0, half), (half, hi - lo - half)]))   # two "filter blocks", contiguous in scan order
+    ids, dist = eng.merge_result_blocks(np.concatenate(heads), world, HEAD_BYTES, np.array(bounds[:world]), k)
     want_ids, want_d = oracle.scan_dense(po.L2, po.I8, q, x, np.arange(1, n + 1, dtype=np.int64), k)
     assert np.array_equal(ids, want_ids) and np.array_equal(dist, want_d)
 
@@ -231,22 +223,14 @@ def test_merge_result_groups_matches_oracle(oracle):
     x = rng.integers(-3, 4, (n, dim)).astype(np.int8)
     qs = rng.integers(-3, 4, (G, dim)).astype(np.int8)
     bounds = [0, 250, 610, n]
-    HDR, TABLE, FIRST = 64, 512 * 8, 1024
-    stride = HDR + TABLE + FIRST * 8
-    blocks = np.zeros(world * G * stride, dtype=np.uint8)
+    heads = []
     for r in range(world):
         lo, hi = bounds[r], bounds[r + 1]
         for j in range(G):
             diff = x[lo:hi].astype(np.int32) - qs[j].astype(np.int32)
             d = np.sqrt((diff * diff).sum(1).astype(np.float32))
-            blk = blocks[(r * G + j) * stride:(r * G + j + 1) * stride]
-            hdr = blk[:HDR].view(np.int32)
-            hdr[0], hdr[1], hdr[2], hdr[3] = hi - lo, 0, 1, 1
-            blk[HDR:HDR + TABLE].view(np.int32).reshape(-1, 2)[0] = (0, hi - lo)
-            out = blk[HDR + TABLE:].view(np.uint32).reshape(-1, 2)
-            out[:hi - lo, 0] = d.view(np.uint32)
-            out[:hi - lo, 1] = np.arange(hi - lo, dtype=np.uint32)
-    res = eng.merge_result_groups(blocks, world, G * stride, stride, G, np.array(bounds[:world]), k)
+            heads.append(make_head(d, [(0, hi - lo)]))
+    res = eng.merge_result_groups(np.concatenate(heads), world, G * HEAD_BYTES, HEAD_BYTES, G, np.array(bounds[:world]), k)
     assert len(res) == G
     for j in range(G):
         want_ids, want_d = oracle.scan_dense(po.L2, po.I8, qs[j], x, np.arange(1, n + 1, dtype=np.int64), k)

@@ -85,7 +85,9 @@ __global__ void quant_encode_kernel(const uint8_t *rows, const long long *rowids
         }
         uint8_t *o = out + (size_t)r * (8 + (size_t)dim);
         o[8 + c] = q;
-        if (c < 8) o[c] = (uint8_t)((unsigned long long)rowids[r] >> (8 * c));       // little-endian rowid (INT64_TO_INT8PTR, :75-85)
+        // little-endian rowid (INT64_TO_INT8PTR, :75-85): the row's threads cover bytes c, c + dim, ... < 8, so all 8 are written
+        // even when dim < 8
+        for (int b = c; b < 8; b += dim) o[b] = (uint8_t)((unsigned long long)rowids[r] >> (8 * b));
     }
 }
 

@@ -3,7 +3,7 @@ in its own process: the vector_as_* encoders on drawn JSON / BLOB inputs (number
 arguments) and vector_quantize builds on drawn tables (5 source types, dims 1..40, NULL rows, NaN / Inf / huge values, constant
 and non-negative columns, both qtypes, several max_memory settings) — rows, error strings, shadow-table bytes and metadata
 must be identical.  CPU only (without a GPU vector_quantize runs its host loops; the GPU loops are pinned to the same bytes by
-test_gpu_parity.py / test_sql_surface.py).  Seeds are fixed; 24 000 encoder statements and 240 table scripts were run once
+test_gpu_parity.py / test_sql_surface.py / test_gpu_quantizer.py, which also runs the quantize scripts below on the GPU).  Seeds are fixed; 24 000 encoder statements and 240 table scripts were run once
 offline without a mismatch."""
 import os
 import random

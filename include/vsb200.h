@@ -261,6 +261,23 @@ VSB_API int vsb_debug_write(vsb_index *ix, const char *name, const void *data, i
  * NULL.  Synchronous. */
 VSB_API int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1,
                                int N, int mode, void *out, int64_t out_cap, void *out_qc, void *out_norms, int64_t *out_count);
+/* diagnostics: ONE launch of the batch path's exact refinement (refine_kernel, production grid) over npairs (row, query) uint32
+ * pairs given by the caller (at most 16 Mi; only the first cand_cap are refined, like a truncated candidate log), with the
+ * per-query bounds U[nq] (kept when distance < U).  out_bucket: nq x 2048 (row, distance bits) uint32 pairs, each query's
+ * kept entries unordered, the rest all ones; out_bcount[nq]: entries appended (more than 2048 when the bucket overflowed);
+ * out_stats[3]: candidates refined, 0, flags (1: pairs beyond cand_cap).  Synchronous. */
+VSB_API int vsb_debug_refine(vsb_index *ix, int metric, const void *queries, int nq, const uint32_t *pairs, int64_t npairs, const float *U,
+                             int64_t cand_cap, uint32_t *out_bucket, uint32_t *out_bcount, uint32_t *out_stats);
+/* diagnostics: ONE launch of the batch path's slot replay (replay_kernel) for k in 1..256 on planted buckets (nq x 2048 (row,
+ * distance bits); bcount[q] entries, more than 2048 flags an overflow).  Slots are kcap = round_up(k, 32) per query:
+ * slot_d / slot_row / slot_mi are read when level0 == 0 (slot_mi in [0, k), else VSB_EINVAL) and always written back.
+ * acc_log (nq x acc_cap (distance bits, row) uint32 pairs) and acc_count[nq] may both be NULL, or carry the entry log in
+ * and out (acc_count is taken as 0 at level0).  final_sort != 0 then runs the final exchange sort on the slots.  Out: U and
+ * qc bits per query (the next level's bound and tensor-core constant), bcount after the call, stats[3]: 0, entries
+ * replayed, flags (2: a bucket overflowed).  Synchronous. */
+VSB_API int vsb_debug_replay(vsb_index *ix, int metric, const void *queries, int nq, int k, int level0, const uint32_t *bucket,
+                             const uint32_t *bcount, float *slot_d, uint32_t *slot_row, int *slot_mi, int acc_cap, uint32_t *acc_log,
+                             int *acc_count, int final_sort, float *out_U, uint32_t *out_qc, uint32_t *out_bcount, uint32_t *out_stats);
 /* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","fuse_mb","scan_streams","xwait_ms","epi_chunk","push_mode","merge_stream" (experiment)};
  * values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);

@@ -93,7 +93,11 @@ _SIGNATURES = {
     "vsb_debug_read": (_i, [_vp, C.c_char_p, _vp, _i64]),
     "vsb_debug_write": (_i, [_vp, C.c_char_p, _vp, _i64]),
     "vsb_debug_tc_level": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i64, _i, _i, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
+    "vsb_debug_refine": (_i, [_vp, _i, _vp, _i, _vp, _i64, _vp, _i64, _vp, _vp, _vp]),
+    "vsb_debug_replay": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
 }
+
+BUCKET_CAP = 2048              # kept candidates per query and level of the batch path (kBucketCap)
 
 
 def _ptr(a):
@@ -389,6 +393,56 @@ class Index:
             res["scores"] = out
         else:
             res["log"] = out[: min(int(count.value), cap)].copy()
+        return res
+
+    def debug_refine(self, metric: int, queries: np.ndarray, pairs: np.ndarray, U: np.ndarray, cand_cap: int | None = None):
+        """one launch of the batch path's exact refinement over (row, query) pairs [npairs, 2] with the bounds U
+        (vsb_debug_refine).  Returns {"bucket": uint32 [nq, BUCKET_CAP, 2] (row, distance bits; unused entries all ones),
+        "bcount": uint32 [nq] entries appended, "stats": uint32 [3]}"""
+        q2 = np.ascontiguousarray(queries).reshape(-1, queries.shape[-1])
+        nq = q2.shape[0]
+        p = np.ascontiguousarray(pairs, dtype=np.uint32).reshape(-1, 2)
+        u = np.ascontiguousarray(U, dtype=np.float32)
+        assert u.shape == (nq,)
+        bucket = np.zeros((nq, BUCKET_CAP, 2), dtype=np.uint32)
+        bcount = np.zeros(nq, dtype=np.uint32)
+        stats = np.zeros(3, dtype=np.uint32)
+        cap = p.shape[0] if cand_cap is None else cand_cap
+        self.eng.check(self.eng.lib.vsb_debug_refine(self.h, metric, _ptr(q2), nq, _ptr(p), p.shape[0], _ptr(u), cap, _ptr(bucket),
+                                                     _ptr(bcount), _ptr(stats)))
+        return {"bucket": bucket, "bcount": bcount, "stats": stats}
+
+    def debug_replay(self, metric: int, queries: np.ndarray, k: int, bucket: np.ndarray, bcount: np.ndarray, level0: bool = True,
+                     slot_d=None, slot_row=None, slot_mi=None, acc_cap: int = 0, acc_log=None, acc_count=None, final_sort: bool = False):
+        """one launch of the batch path's slot replay (vsb_debug_replay) on planted buckets [nq, BUCKET_CAP, 2] (row, distance
+        bits) with bcount [nq] entries each.  level0=False continues from slot_d / slot_row [nq, kcap] and slot_mi [nq];
+        acc_cap > 0 carries the entry log (acc_log [nq, acc_cap, 2] (distance bits, row), acc_count [nq]; zeros by default).
+        Returns {"slot_d", "slot_row" [nq, kcap], "slot_mi", "U", "qc" (uint32 bits), "bcount", "stats" [3], and with a log
+        "acc_log", "acc_count"}"""
+        q2 = np.ascontiguousarray(queries).reshape(-1, queries.shape[-1])
+        nq = q2.shape[0]
+        kcap = (k + 31) & ~31
+        b = np.ascontiguousarray(bucket, dtype=np.uint32)
+        assert b.shape == (nq, BUCKET_CAP, 2)
+        bc = np.ascontiguousarray(bcount, dtype=np.uint32)
+        sd = np.zeros((nq, kcap), np.float32) if slot_d is None else np.array(slot_d, dtype=np.float32, order="C")
+        sr = np.zeros((nq, kcap), np.uint32) if slot_row is None else np.array(slot_row, dtype=np.uint32, order="C")
+        mi = np.zeros(nq, np.int32) if slot_mi is None else np.array(slot_mi, dtype=np.int32)
+        assert sd.shape == (nq, kcap) and sr.shape == (nq, kcap) and mi.shape == (nq,)
+        log = cnt = None
+        if acc_cap > 0:
+            log = np.zeros((nq, acc_cap, 2), np.uint32) if acc_log is None else np.array(acc_log, dtype=np.uint32, order="C")
+            cnt = np.zeros(nq, np.int32) if acc_count is None else np.array(acc_count, dtype=np.int32)
+        U = np.zeros(nq, np.float32)
+        qc = np.zeros(nq, np.uint32)
+        bout = np.zeros(nq, np.uint32)
+        stats = np.zeros(3, np.uint32)
+        self.eng.check(self.eng.lib.vsb_debug_replay(self.h, metric, _ptr(q2), nq, k, int(level0), _ptr(b), _ptr(bc), _ptr(sd), _ptr(sr),
+                                                     _ptr(mi), acc_cap, _ptr(log), _ptr(cnt), int(final_sort), _ptr(U), _ptr(qc),
+                                                     _ptr(bout), _ptr(stats)))
+        res = {"slot_d": sd, "slot_row": sr, "slot_mi": mi, "U": U, "qc": qc, "bcount": bout, "stats": stats}
+        if log is not None:
+            res["acc_log"], res["acc_count"] = log, cnt
         return res
 
     def profile_read(self):

@@ -504,8 +504,9 @@ struct ReplayParams {
 
 // The reference's slot update for up to 32 (distance, row) offers held one per lane, in lane order:
 // strict '<' against the slot at max_index (src/sqlite-vector.c:2145), then vFullScanFindMaxIndex (:2022-2049, first
-// index of the maximum).  sd/sr: this query's slots (kcap entries, entries >= k hold -INF); on_accept(dist, row) is
-// called by the whole warp for every offer that enters.
+// index of the maximum).  sd/sr: this query's slots (kcap entries, a multiple of 32; entries >= k hold -INF); on_accept(dist,
+// row) is called by the whole warp for every offer that enters.  Each lane starts from its own first slot, so when every
+// slot is -INF the maximum is slot 0, as in the reference (a lane starting from -INF would never update and leave no index).
 template <class F>
 __device__ __forceinline__ void warp_offer32(float *sd, unsigned *sr, int kcap, int lane, float d, unsigned row, int &mi, float &cur,
                                              F on_accept) {
@@ -518,9 +519,9 @@ __device__ __forceinline__ void warp_offer32(float *sd, unsigned *sr, int kcap, 
         if (dv < cur) {
             if (lane == 0) { sd[mi] = dv; sr[mi] = rv; }
             __syncwarp();
-            float best = -INFINITY;
-            int bi = 0x7FFFFFFF;
-            for (int j = lane; j < kcap; j += 32) {
+            float best = sd[lane];
+            int bi = lane;
+            for (int j = lane + 32; j < kcap; j += 32) {
                 const float v = sd[j];
                 if (v > best) { best = v; bi = j; }
             }
@@ -672,7 +673,8 @@ struct MergeParams {
     const long long *first_seq; // [world] global scan-order index of each shard's first row (device)
     float *slot_d;              // [nq][kcap] out
     unsigned *slot_row;         // [nq][kcap] out: GLOBAL row index
-    int *status;                // [0] |= 1 when a shard's log overflowed, |= 2 on a malformed block
+    int *status;                // [0] |= 1 when a shard's log overflowed, |= 2 on a malformed block, |= 8 when a global row
+                                // (first_seq + local row) does not fit 32 bits
 };
 
 // one warp per query: the shards' logs, in shard (= scan) order, through the reference's slot update
@@ -703,11 +705,15 @@ __global__ void merge_logs_kernel(const MergeParams mp) {
             return;
         }
         const uint2 *lg = reinterpret_cast<const uint2 *>(blk + acc_block_log_off(mp.nq)) + (size_t)q * mp.acc_cap;
-        const unsigned base_row = (unsigned)mp.first_seq[r];
+        const unsigned long long base_row = (unsigned long long)mp.first_seq[r];
         for (int base = 0; base < cnt; base += 32) {
             const int i = base + lane;
             const uint2 e = (i < cnt) ? lg[i] : make_uint2(0x7F800000u, 0u);
-            warp_offer32(sd, sr, mp.kcap, lane, __uint_as_float(e.x), base_row + e.y, mi, cur, [](float, unsigned) {});
+            if (__any_sync(0xFFFFFFFFu, i < cnt && base_row + e.y > 0xFFFFFFFFull)) {   // the slots carry 32-bit global rows
+                if (lane == 0) atomicOr(mp.status, 8);
+                return;
+            }
+            warp_offer32(sd, sr, mp.kcap, lane, __uint_as_float(e.x), (unsigned)(base_row + e.y), mi, cur, [](float, unsigned) {});
         }
     }
 }

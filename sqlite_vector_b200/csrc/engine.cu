@@ -1298,6 +1298,20 @@ int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, c
     return rc;
 }
 
+int vsb_debug_refine(vsb_index *ix, int metric, const void *queries, int nq, const uint32_t *pairs, int64_t npairs, const float *U,
+                     int64_t cand_cap, uint32_t *out_bucket, uint32_t *out_bcount, uint32_t *out_stats) {
+    if (check_index(ix)) return VSB_EINVAL;
+    return batch_debug_refine(ix, metric, queries, nq, pairs, npairs, U, cand_cap, out_bucket, out_bcount, out_stats);
+}
+
+int vsb_debug_replay(vsb_index *ix, int metric, const void *queries, int nq, int k, int level0, const uint32_t *bucket, const uint32_t *bcount,
+                     float *slot_d, uint32_t *slot_row, int *slot_mi, int acc_cap, uint32_t *acc_log, int *acc_count, int final_sort,
+                     float *out_U, uint32_t *out_qc, uint32_t *out_bcount, uint32_t *out_stats) {
+    if (check_index(ix)) return VSB_EINVAL;
+    return batch_debug_replay(ix, metric, queries, nq, k, level0, bucket, bcount, slot_d, slot_row, slot_mi, acc_cap, acc_log, acc_count,
+                              final_sort, out_U, out_qc, out_bcount, out_stats);
+}
+
 int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double *filter_ms, int *filter_launches) {
     if (check_index(ix)) return VSB_EINVAL;
     CU(cudaSetDevice(ix->device));

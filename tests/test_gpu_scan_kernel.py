@@ -198,7 +198,7 @@ def _chain_len(nc, log2p, esz):
     return -(-nc // P) * E // 2 + log2p + 1
 
 
-def _fp_bound_and_exact(metric, vtype, xr, qv, nc, log2p):
+def _fp_bound_and_exact(metric, vtype, xr, qv, nc, log2p, q_lanes=32):
     """float64 exact distances and the bound |d_gpu - d| <= bound, from the kernel's order of summation.
 
     Sums S = sum t_i (DOT: x_i y_i; L2SQ: (x_i - y_i)^2; L1: |x_i - y_i|): every term passes through at most L roundings of
@@ -206,7 +206,8 @@ def _fp_bound_and_exact(metric, vtype, xr, qv, nc, log2p):
         |S_gpu - S| <= (L + 2) 2^-24 sum |t_i|          (first order; the factor 1.001 below covers the rest).
     L2 = sqrt(S):  |sqrt(S') - sqrt(S)| <= min(sqrt(E_S), E_S / sqrt(S)), plus the sqrt's own rounding 2^-24 sqrt(S').
     COSINE = 1 - s / (sqrt(qq) sqrt(ny)): s has E_s as above; the row norm ny is ONE chain per lane (L_n = ceil(nc/P) E +
-    log2 P + 1 roundings), the query norm is lane-strided over 32 lanes (L_q = ceil(nc/32) E + 6); with c = s / (|q||r|)
+    log2 P + 1 roundings), the query norm is lane-strided over q_lanes lanes (L_q = ceil(nc/q_lanes) E + log2 q_lanes + 1:
+    32 lanes in the scan kernel, the refine's 8); with c = s / (|q||r|)
         |c' - c| <= E_s / (|q||r|) + |c| (E_qq / 2qq + E_ny / 2ny + 4 * 2^-24),  then 1 - c' adds 2^-24 |d|."""
     esz = po.ELEM_SIZE[vtype]
     E = 16 // esz
@@ -233,7 +234,7 @@ def _fp_bound_and_exact(metric, vtype, xr, qv, nc, log2p):
     ny = (xr * xr).sum(1)
     qq = float(qv @ qv)
     Eny = 1.001 * (-(-nc // P) * E + log2p + 2) * U * ny
-    Eqq = 1.001 * (-(-nc // 32) * E + 6) * U * qq
+    Eqq = 1.001 * (-(-nc // q_lanes) * E + q_lanes.bit_length()) * U * qq
     den = np.sqrt(ny * qq)
     zero = (ny == 0) | (qq == 0)
     with np.errstate(divide="ignore", invalid="ignore"):

@@ -37,6 +37,14 @@ ixb = index(api.BF16, xb)
 ixb.scan_topk(api.DOT, xb[:32].copy(), 10)
 ixb.scan_topk(api.L2, xb[0].copy(), 10)
 ixb.close()
+# f16 DOT, k = 1: row 5 holds +Inf against all-positive queries, so every query's only slot is -Inf after level 0 and the
+# later levels start from max_index 0
+xh = rng.standard_normal((20000, 64)).astype(np.float16).view(np.uint16)
+xh[5, 0] = 0x7C00
+qh = (np.abs(rng.standard_normal((32, 64))) + 0.5).astype(np.float16).view(np.uint16)
+ixh = index(api.F16, xh)
+ixh.scan_topk(api.DOT, qh, 1)
+ixh.close()
 xw = rng.standard_normal((600, 20000)).astype(np.float32)     # DIRECT kernel (rows larger than the staging ring)
 ixw = index(api.F32, xw)
 ixw.scan_topk(api.L2, xw[3].copy(), 7)

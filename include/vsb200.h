@@ -94,7 +94,8 @@ VSB_API void vsb_index_free(vsb_index *ix);
  * max_index (in/out, may be NULL, nq == 1 only): the cursor's slot index quirk (:1808-1813 never resets it).
  * nq > 1 has no counterpart in the reference (one vector per xFilter); each query then behaves like a fresh cursor.
  * For nq >= 16 on f16/bf16/int8/uint8 columns with L2/SQUARED_L2/COSINE/DOT the scores are computed on the tensor
- * cores (wgmma) and refined exactly; results are the same as nq single calls. */
+ * cores (wgmma), and with L1 on any column type by a CUDA-core batch kernel over the same tiles; either way they are
+ * refined exactly and results are the same as nq single calls. */
 VSB_API int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k, int64_t *out_rowids,
                           double *out_dist, int *out_counts, int *max_index);
 
@@ -151,8 +152,8 @@ VSB_API int vsb_merge_result_groups(const void *blocks, int world, int64_t rank_
                                     const int64_t *first_seq, int k, int64_t *out_rowids, double *out_dist, int *out_counts);
 
 /* ---- batched queries on a row-sharded column (BASELINE config 4: one shard per GPU) ----------------------------
- * step 1, on every shard: the tensor-core batch path of vsb_scan_topk (same conditions: nq >= 16, f16/bf16/int8/uint8,
- * not L1) over this shard, leaving in DEVICE memory one block with, per query, the rows that entered the shard-local
+ * step 1, on every shard: the batch path of vsb_scan_topk (same conditions: nq >= 16; f16/bf16/int8/uint8, or L1 on any
+ * type) over this shard, leaving in DEVICE memory one block with, per query, the rows that entered the shard-local
  * slots in scan order (distance bits, local row).  *d_block / *bytes describe it (the same size on every shard for the
  * same nq and k) so that a launcher can all-gather the blocks (NCCL).  Returns VSB_ERANGE when the batch path does not
  * apply or a capacity was exceeded: use the per-query path (vsb_scan_candidates / vsb_scan_submit) then. */
@@ -185,8 +186,8 @@ VSB_API int vsb_exchange_submit(vsb_index *ix, int metric, const void *queries, 
 VSB_API int vsb_exchange_collect(vsb_index *ix, int first_slot, int nq, const int64_t *first_seq /* [world] */, int k,
                                  int64_t *out_rowids, double *out_dist, int *out_counts);
 
-/* batched queries over the same exchange (BASELINE config 4 between processes): every rank runs the tensor-core levels with entry
- * logs over its shard, pushes its log block into every peer's log area over NVLink (push_logs_kernel), waits for the peers'
+/* batched queries over the same exchange (BASELINE config 4 between processes): every rank runs the batch levels (tensor cores;
+ * L1: the CUDA-core batch kernel, any column type) with entry logs over its shard, pushes its log block into every peer's log area over NVLink (push_logs_kernel), waits for the peers'
  * flags on the device and replays all logs in shard order on its GPU — the result of one scan over the whole column on every
  * rank, no collective library, ONE host wait per batch.  submit returns a ticket (0 / 1: two batches may be in flight) or a
  * negative code (VSB_ERANGE: the batch path does not apply — use vsb_exchange_submit per query); collect returns VSB_ERANGE on
@@ -249,16 +250,16 @@ VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t b
  * workspace of a resident index, so that the next single-query scans with k <= 32 use it instead of equal shares (the filter
  * then rewrites it as usual).  Rejects an index too small for the adaptive partition.  Returns 0 or < 0. */
 VSB_API int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t bytes);
-/* diagnostics: ONE tensor-core level of the batch path (tc_scan_kernel) over rows [r0, r1) of a finalized resident index
- * (r0 a multiple of 128), for nq HOST queries whose exact distance bounds U[nq] are given instead of found by earlier levels;
- * the per-query constants are the batch path's own (conservative_qc).  N: queries per tile, 32 / 64 / 128 (/ 256 for
- * int8 and uint8), 0 = the batch path's choice for nq.
+/* diagnostics: ONE tensor-core level of the batch path (tc_scan_kernel; metric VSB_L1: l1_batch_kernel, any column type) over
+ * rows [r0, r1) of a finalized resident index (r0 a multiple of 128), for nq HOST queries whose exact distance bounds U[nq] are
+ * given instead of found by earlier levels; the per-query constants are the batch path's own (conservative_qc).  N: queries
+ * per tile, 32 / 64 / 128 (/ 256 for int8 and uint8, not L1), 0 = the batch path's choice for nq.
  *   mode 0 (candidate log, the production kernel): out receives up to out_cap (row, query) pairs of uint32, *out_count the
  *   number of hits the kernel counted (more than out_cap when the log was truncated).
- *   mode 1 (scores): out[(row - r0) * nq + q] = <row, query q> as the tensor cores computed it, int32 (int8 / uint8) or
- *   float (f16 / bf16); out_cap >= (r1 - r0) * nq.
- * out_qc (nq x 32 bits: float, or int for the integer kinds) and out_norms (r1 - r0 row sums of squares, float / int) may be
- * NULL.  Synchronous. */
+ *   mode 1 (scores): out[(row - r0) * nq + q] = <row, query q> as the tensor cores computed it (L1: sum |row - query q|),
+ *   int32 (int8 / uint8) or float (f32 / f16 / bf16); out_cap >= (r1 - r0) * nq.
+ * out_qc (nq x 32 bits: float, or int for the integer kinds; L1: float) and out_norms (r1 - r0 row sums of squares, float /
+ * int; left untouched for L1) may be NULL.  Synchronous. */
 VSB_API int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1,
                                int N, int mode, void *out, int64_t out_cap, void *out_qc, void *out_norms, int64_t *out_count);
 /* diagnostics: ONE launch of the batch path's exact refinement (refine_kernel, production grid) over npairs (row, query) uint32

@@ -369,10 +369,11 @@ class Index:
 
     def debug_tc_level(self, metric: int, queries: np.ndarray, U: np.ndarray, r0: int, r1: int, N: int = 0, scores: bool = False,
                        cap: int = 1 << 22):
-        """one tensor-core level of the batch path over rows [r0, r1) with the per-query bounds U (vsb_debug_tc_level).
+        """one tensor-core level of the batch path over rows [r0, r1) with the per-query bounds U (vsb_debug_tc_level; metric
+        L1: one level of the CUDA-core L1 batch kernel, any column type).
         scores=False: {"log": (row, query) uint32 pairs, "count": hits counted (> len(log) when truncated at cap),
-        "qc": uint32 bits [nq], "norms": row sums of squares [r1 - r0]}; scores=True: the same with "scores" [r1 - r0, nq]
-        (int32 for int8 / uint8, float32 for f16 / bf16) instead of the log"""
+        "qc": uint32 bits [nq], "norms": row sums of squares [r1 - r0] (zeros for L1)}; scores=True: the same with "scores"
+        [r1 - r0, nq] (int32 for int8 / uint8, float32 for f32 / f16 / bf16) instead of the log"""
         q2 = np.ascontiguousarray(queries).reshape(-1, queries.shape[-1])
         nq = q2.shape[0]
         u = np.ascontiguousarray(U, dtype=np.float32)

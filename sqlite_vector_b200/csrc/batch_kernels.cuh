@@ -38,7 +38,7 @@ struct TcParams {
     int NG;                 // query groups = ceil(nq / N)
     int KB;                 // 128-byte K blocks per row
     int nstages;            // ring depth (2..kTcMaxStages)
-    int mc;                 // MC_L2 / MC_COS / MC_DOT
+    int mc;                 // MC_L2 / MC_COS / MC_DOT (l1_batch_kernel: MC_L1), or MC_TC_SCORES
     int chunk_test;         // integer kinds: test 32-column chunks before single scores (see tc_scan_kernel)
     float eps;              // fp kinds: relative slack of the tensor-core score, see tc_fp_eps
     const float *qc;        // [NG*N] per-query constant (float, or int bit pattern for the integer kinds)
@@ -328,6 +328,189 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
     }
 }
 
+// ------------------------------------------------------------------ L1 scores on the CUDA cores
+// sum |row_i - q_i| has no GEMM form, but over a batch it is the same dense all-pairs work, compute-bound once the corpus is
+// read once per level.  l1_batch_kernel walks the tiles of tc_scan_kernel (TileWalk, the same TMA producer warp and stage ring:
+// 128 corpus rows and N queries per 128-byte K slice, 128B swizzle, full / empty mbarriers) and adds the sums on the CUDA
+// cores.  Consumer warp w owns queries [w N/8, (w + 1) N/8) of the tile and lane l the rows l + 32 i, i < 4: a thread keeps
+// 4 x N/8 sums in registers.  Every 16-byte chunk is one LDS.128; the query chunks a warp reads are broadcasts, and chunk c of
+// row r sits at c ^ (r & 7), so the 8 lanes of one LDS.128 phase hit 8 different 16-byte bank groups.
+//   int8 / uint8: VABSDIFF4 + IDP.4A per 4 element pairs, exact int32 (the same instructions as accum16).
+//   f32 / f16 / bf16: s += |x - y| in fp32, every term formed with one rounding, like accum16 (only the order of the sum differs).
+// The epilogue tests every (row, query) against qc[query] from registers and appends hits to the candidate log with one atomic
+// per warp, as tc_scan_kernel does: integer types (float)S < qc with qc = U, exactly the refine's keep condition; fp types
+// !(s >= qc) with the conservative constant of conservative_qc (NaN scores are hits).  Padded query columns are never
+// reported.  prm.mc == MC_TC_SCORES stores every score of rows [r0, r1) instead (vsb_debug_tc_level mode 1).
+constexpr int kL1Warps = 8;
+constexpr int kL1Threads = kL1Warps * 32 + 32;   // warps 0-7: consumers, warp 8: TMA producer
+
+template <int VT, int N>
+__global__ void __launch_bounds__(kL1Threads, 1) l1_batch_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                 const __grid_constant__ CUtensorMap tmB, const TcParams prm) {
+    constexpr bool INT8 = (VT == T_I8 || VT == T_U8);
+    constexpr int C = N / kL1Warps;                                            // queries per warp
+    constexpr int R = kTcM / 32;                                               // rows per lane
+    constexpr int NE = (VT == T_F32) ? 4 : 8;                                  // elements per 16-byte chunk (fp types)
+    using Acc = typename std::conditional<INT8, uint32_t, float>::type;
+    extern __shared__ __align__(1024) uint8_t lsm[];
+    const int NS = prm.nstages;
+    constexpr uint32_t a_bytes = kTcM * kTcKBytes, b_bytes = (uint32_t)N * kTcKBytes;
+    constexpr uint32_t stage_bytes = a_bytes + b_bytes;
+    uint8_t *stages = lsm;                                                     // [NS][A | B], 1024-aligned
+    uint64_t *full = reinterpret_cast<uint64_t *>(lsm + (size_t)NS * stage_bytes);
+    uint64_t *empty = full + kTcMaxStages;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < kTcMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kL1Warps); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    TileWalk tw;
+    tw.init(prm);
+    const int KB = prm.KB;
+
+    if (warp == kL1Warps) {                                                    // ===== TMA producer (as in tc_scan_kernel)
+        int s = 0;
+        uint32_t ph = 1;
+        for (uint32_t tl = 0; tl < tw.count; ++tl, tw.next()) {
+            const int row0 = (int)(tw.mt() * kTcM), col0 = tw.ng() * N;
+            for (int kb = 0; kb < KB; ++kb) {
+                mbar_wait(&empty[s], ph);
+                if (elect_one()) {
+                    mbar_expect_tx(&full[s], stage_bytes);
+                    uint8_t *st = stages + (size_t)s * stage_bytes;
+                    tma_load_2d(st, &tmA, kb * kTcKBytes, row0, &full[s]);
+                    tma_load_2d(st + a_bytes, &tmB, kb * kTcKBytes, col0, &full[s]);
+                }
+                __syncwarp();
+                if (++s == NS) { s = 0; ph ^= 1u; }
+            }
+        }
+        return;
+    }
+
+    // ===== consumer warp: queries q0 .. q0 + C - 1 of the tile, rows lane + 32 i
+    const int q0 = warp * C;
+    const uint32_t rsw = (uint32_t)(lane & 7);                                 // swizzle of all this lane's rows
+    int s = 0;
+    uint32_t ph = 0;
+    for (uint32_t tl = 0; tl < tw.count; ++tl, tw.next()) {
+        const long long mt = tw.mt();
+        const int ng = tw.ng();
+        const int ncol = prm.nq - ng * N - q0;                                 // real queries of this warp (C or fewer, maybe none)
+        Acc acc[R][C];
+#pragma unroll
+        for (int i = 0; i < R; ++i)
+#pragma unroll
+            for (int j = 0; j < C; ++j) acc[i][j] = 0;
+        for (int kb = 0; kb < KB; ++kb) {
+            mbar_wait(&full[s], ph);
+            if (ncol > 0) {                                                    // warp-uniform: padding-only warps just pass the stage on
+                const uint8_t *A = stages + (size_t)s * stage_bytes + lane * kTcKBytes;
+                const uint8_t *B = stages + (size_t)s * stage_bytes + a_bytes + q0 * kTcKBytes;
+#pragma unroll 2
+                for (uint32_t c = 0; c < kTcKBytes / 16; ++c) {
+                    uint4 rv[R];
+#pragma unroll
+                    for (int i = 0; i < R; ++i) rv[i] = *reinterpret_cast<const uint4 *>(A + i * 32 * kTcKBytes + ((c ^ rsw) << 4));
+                    if constexpr (INT8) {
+#pragma unroll
+                        for (int j = 0; j < C; ++j) {
+                            const uint4 qv = *reinterpret_cast<const uint4 *>(B + j * kTcKBytes + ((c ^ (uint32_t)((q0 + j) & 7)) << 4));
+                            const uint32_t qw[4] = {qv.x, qv.y, qv.z, qv.w};
+#pragma unroll
+                            for (int i = 0; i < R; ++i) {
+                                const uint32_t rw[4] = {rv[i].x, rv[i].y, rv[i].z, rv[i].w};
+#pragma unroll
+                                for (int e = 0; e < 4; ++e) {
+                                    const uint32_t ad = (VT == T_U8) ? __vabsdiffu4(rw[e], qw[e]) : __vabsdiffs4(rw[e], qw[e]);
+                                    acc[i][j] = __dp4a(ad, 0x01010101u, acc[i][j]);
+                                }
+                            }
+                        }
+                    } else {
+                        float y[R][8];
+#pragma unroll
+                        for (int i = 0; i < R; ++i) unpack8<VT>(rv[i], y[i]);
+#pragma unroll
+                        for (int j = 0; j < C; ++j) {
+                            const uint4 qv = *reinterpret_cast<const uint4 *>(B + j * kTcKBytes + ((c ^ (uint32_t)((q0 + j) & 7)) << 4));
+                            float x[8];
+                            unpack8<VT>(qv, x);
+#pragma unroll
+                            for (int i = 0; i < R; ++i)
+#pragma unroll
+                                for (int e = 0; e < NE; ++e) acc[i][j] += fabsf(x[e] - y[i][e]);
+                        }
+                    }
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);                             // this warp has read the stage
+            if (++s == NS) { s = 0; ph ^= 1u; }
+        }
+        if (ncol <= 0) continue;
+        long long row[R];
+        bool rowvalid[R];
+#pragma unroll
+        for (int i = 0; i < R; ++i) {
+            row[i] = mt * kTcM + lane + 32 * i;
+            rowvalid[i] = row[i] >= prm.r0 && row[i] < prm.r1;
+        }
+        const int qbase = ng * N + q0;
+        if (prm.mc == MC_TC_SCORES) {
+#pragma unroll
+            for (int i = 0; i < R; ++i)
+#pragma unroll
+                for (int j = 0; j < C; ++j) {
+                    uint32_t v;
+                    if constexpr (INT8) v = acc[i][j];
+                    else v = __float_as_uint(acc[i][j]);
+                    if (rowvalid[i] && j < ncol) prm.scores[(size_t)(row[i] - prm.r0) * prm.nq + qbase + j] = v;
+                }
+            continue;
+        }
+        float qc[C];
+#pragma unroll
+        for (int j = 0; j < C; ++j) qc[j] = __ldg(prm.qc + qbase + j);         // padded columns: +INF from the upload
+        auto hit = [&](int i, int j) -> bool {
+            bool h;
+            if constexpr (INT8) h = (float)acc[i][j] < qc[j];
+            else h = !(acc[i][j] >= qc[j]);
+            return h && rowvalid[i] && j < ncol;
+        };
+        int mine = 0;
+#pragma unroll
+        for (int i = 0; i < R; ++i)
+#pragma unroll
+            for (int j = 0; j < C; ++j) mine += hit(i, j) ? 1 : 0;
+        if (__ballot_sync(0xFFFFFFFFu, mine != 0)) {                           // rare: append (row, query) hits, one atomic per warp
+            int incl = mine;
+            for (int off = 1; off < 32; off <<= 1) {
+                const int o = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+                if (lane >= off) incl += o;
+            }
+            const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+            unsigned base = 0;
+            if (lane == 31) base = atomicAdd(prm.cand_count, (unsigned)total);
+            base = __shfl_sync(0xFFFFFFFFu, base, 31);
+            unsigned w = base + (unsigned)(incl - mine);
+            if (mine) {
+#pragma unroll
+                for (int i = 0; i < R; ++i)
+#pragma unroll
+                    for (int j = 0; j < C; ++j)
+                        if (hit(i, j)) {
+                            if (w < prm.cand_cap) prm.cand[w] = make_uint2((uint32_t)row[i], (uint32_t)(qbase + j));
+                            ++w;
+                        }
+            }
+        }
+    }
+}
+
 
 // ------------------------------------------------------------------ row norms (once per resident shard)
 template <int VT>
@@ -347,10 +530,11 @@ __global__ void row_norm_kernel(const uint8_t *vec, long long n, int pitch, void
             iq = __dp4a((int)q.x, (int)q.x, iq); iq = __dp4a((int)q.y, (int)q.y, iq);
             iq = __dp4a((int)q.z, (int)q.z, iq); iq = __dp4a((int)q.w, (int)q.w, iq);
         } else {
+            constexpr int NE = (VT == T_F32) ? 4 : 8;                           // unpack8 writes 4 floats for f32
             float x[8];
             unpack8<VT>(q, x);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) f = fmaf(x[j], x[j], f);
+            for (int j = 0; j < NE; ++j) f = fmaf(x[j], x[j], f);
         }
     }
     for (int off = 16; off >= 1; off >>= 1) {
@@ -388,6 +572,13 @@ struct RefineParams {
 
 constexpr unsigned kBucketCap = 2048;   // kept candidates per query and level (replay_kernel sorts them in shared memory)
 
+// f16 L1 rows of refine_kernel: a copy of special_row_distance of its own.  A noinline function shared with
+// scan_kernel<T_F16, MC_L1> is register-allocated for every caller, so sharing it would change the single-query kernel's code.
+template <int VT, int MC>
+__device__ __noinline__ float refine_special_row_distance(const uint8_t *row, const uint8_t *query, int nelem, int root) {
+    return special_row_distance_body<VT, MC>(row, query, nelem, root);
+}
+
 // eight lanes per candidate (four candidates per warp step): the reference distance with the arithmetic of the
 // single-query kernel; survivors go to their query's bucket (one atomic each on nq different counters; no global sort
 // and no host round trip per level: replay_kernel orders each bucket by row itself).
@@ -424,10 +615,11 @@ __global__ void refine_kernel(const RefineParams rp) {
                     qn.i = __dp4a((int)qv.x, (int)qv.x, qn.i); qn.i = __dp4a((int)qv.y, (int)qv.y, qn.i);
                     qn.i = __dp4a((int)qv.z, (int)qv.z, qn.i); qn.i = __dp4a((int)qv.w, (int)qv.w, qn.i);
                 } else if constexpr (MC == MC_COS) {
+                    constexpr int NE = (VT == T_F32) ? 4 : 8;                   // unpack8 writes 4 floats for f32
                     float x[8];
                     unpack8<VT>(qv, x);
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) qn.f = fmaf(x[j], x[j], qn.f);
+                    for (int j = 0; j < NE; ++j) qn.f = fmaf(x[j], x[j], qn.f);
                 }
             }
         }
@@ -438,8 +630,11 @@ __global__ void refine_kernel(const RefineParams rp) {
         }
         float d = finalize<VT, MC>(A, qn, rp.root);
         if constexpr (has_special_policy<VT, MC>()) {       // rows (or queries) holding NaN / Inf: the reference's own element loop
-            if (live && sub == 0 && row_needs_exact<VT, MC>(A, qn))
-                d = special_row_distance<VT, MC>(reinterpret_cast<const uint8_t *>(rowp), reinterpret_cast<const uint8_t *>(qp), rp.pitch / 2, rp.root);
+            if (live && sub == 0 && row_needs_exact<VT, MC>(A, qn)) {
+                const uint8_t *r8 = reinterpret_cast<const uint8_t *>(rowp), *q8 = reinterpret_cast<const uint8_t *>(qp);
+                if constexpr (MC == MC_L1) d = refine_special_row_distance<VT, MC>(r8, q8, rp.pitch / 2, rp.root);
+                else d = special_row_distance<VT, MC>(r8, q8, rp.pitch / 2, rp.root);
+            }
         }
         const bool keep = live && sub == 0 && d < rp.U[cq.y];
         if (keep) {
@@ -489,7 +684,7 @@ struct ReplayParams {
     int *slot_mi;           // [nq] max_index
     float *U;               // [nq] out: running k-th distance after this level
     float *qc;              // [NGN] out: conservative constant for the next level
-    int mc, kind, root;
+    int mc, vt, root;       // vt: element type (T_*)
     const void *qnorm;      // [nq] float / int sum of squares of each query
     float rnmax;            // max row norm (fp kinds, DOT slack)
     int dim;                // elements per row (fp kinds: slack of the tensor-core score)
@@ -547,13 +742,29 @@ __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fm
 // dim * 2^-24 * ... only up to dim ~ 1600: the verdict's weak item 1.)
 __host__ __device__ inline float tc_fp_eps(int dim) { return (float)dim * 9.5367431640625e-7f; }
 
-// conservative per-query constant for tc_hit from the exact bound U (see DESIGN.md §3.4): every row whose exact (refine)
-// distance is < U satisfies tc_hit with this constant
-__device__ inline float conservative_qc(int kind, int mc, int root, float U, const void *qnorm, int q, float rnmax, int dim) {
-    const bool INT8 = (kind == TK_I8 || kind == TK_U8);
+// Bound of the fp L1 score.  l1_batch_kernel and the refine both add the same dim non-negative terms t_i = fl(|x_i - y_i|)
+// (one rounding each; padding terms are exact zeros), in different orders.  With u = 2^-24, every term is within u of
+// |x_i - y_i| and any summation order of dim terms within gamma_(dim-1) of their sum, so for ANY order the computed sum s
+// obeys |s - S| <= gamma S, S = sum |x_i - y_i| exact, gamma = m u / (1 - m u), m = dim + 1 (one to spare).  The refine's
+// distance d is s clamped by nearly_zero_float32 (sums <= 8 FLT_EPSILON become 0), so d < U  =>  s_refine <= B = max(U,
+// 8 FLT_EPSILON)  =>  S <= B / (1 - gamma)  =>  s_kernel <= B (1 + gamma) / (1 - gamma).  The constant is that bound computed
+// in double, widened by 2^-40 for the double arithmetic and rounded up to float, so the kernel's test !(s >= qc) keeps every
+// such pair.  A bound beyond FLT_MAX (or U = +INF) returns NaN: every pair is a hit then, also a sum that overflowed to +INF.
+__device__ inline float l1_fp_qc(float U, int dim) {
+    if (!(U <= FLT_MAX)) return __int_as_float(0x7FC00000);
+    const double mu = (double)(dim + 1) * 0x1p-24, gamma = mu / (1.0 - mu);
+    const double b = fmax((double)U, 8.0 * (double)FLT_EPSILON) * (1.0 + gamma) / (1.0 - gamma) * (1.0 + 0x1p-40);
+    return (b < (double)FLT_MAX) ? __double2float_ru(b) : __int_as_float(0x7FC00000);
+}
+
+// conservative per-query constant for tc_hit (or the L1 test of l1_batch_kernel) from the exact bound U (see DESIGN.md §3.4):
+// every row whose exact (refine) distance is < U passes the kernel's test with this constant.  vt: element type (T_*).
+__device__ inline float conservative_qc(int vt, int mc, int root, float U, const void *qnorm, int q, float rnmax, int dim) {
+    const bool INT8 = (vt == T_I8 || vt == T_U8);
+    if (mc == MC_L1) return INT8 ? U : l1_fp_qc(U, dim);   // integer sums are exact: the kernel tests (float)S < U like the refine
     if (INT8) {
         const int qi = reinterpret_cast<const int *>(qnorm)[q];
-        const double qq = (kind == TK_U8) ? (double)(uint32_t)qi : (double)qi;
+        const double qq = (vt == T_U8) ? (double)(uint32_t)qi : (double)qi;
         if (mc == MC_DOT) {          // d = -(float)s < U  <=  s > -U - 1 - 2e-7|U|
             double b = -(double)U - 1.0 - 2e-7 * fabs((double)U);
             if (!(U < 3.0e38f)) b = -2147483647.0;
@@ -588,9 +799,9 @@ __device__ inline float conservative_qc(int kind, int mc, int root, float U, con
 }
 
 // the constants replay_kernel would derive from the bounds U[nq] (vsb_debug_tc_level: one tensor-core level in isolation)
-__global__ void conservative_qc_kernel(float *qc, const float *U, int nq, int kind, int mc, int root, const void *qnorm, float rnmax, int dim) {
+__global__ void conservative_qc_kernel(float *qc, const float *U, int nq, int vt, int mc, int root, const void *qnorm, float rnmax, int dim) {
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q < nq) qc[q] = conservative_qc(kind, mc, root, U[q], qnorm, q, rnmax, dim);
+    if (q < nq) qc[q] = conservative_qc(vt, mc, root, U[q], qnorm, q, rnmax, dim);
 }
 
 constexpr int kReplayThreads = 128;
@@ -649,7 +860,7 @@ __global__ void __launch_bounds__(kReplayThreads) replay_kernel(const ReplayPara
         if (lane == 0) {
             rp.slot_mi[q] = mi;
             rp.U[q] = cur;
-            rp.qc[q] = conservative_qc(rp.kind, rp.mc, rp.root, cur, rp.qnorm, q, rp.rnmax, rp.dim);
+            rp.qc[q] = conservative_qc(rp.vt, rp.mc, rp.root, cur, rp.qnorm, q, rp.rnmax, rp.dim);
             if (rp.acc_log != nullptr) rp.acc_count[q] = acc_n;
             rp.bcount[q] = 0;
             atomicAdd(&rp.stats[1], c);

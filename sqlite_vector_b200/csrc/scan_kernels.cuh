@@ -274,7 +274,7 @@ __device__ __forceinline__ bool row_needs_exact(const Accum &A, const QueryNorm 
 //   f16 COSINE (:434-466): NaN lanes skipped; any infinity -> 1; bad denominator / non-finite dot -> 1; clamp to [-1, 1]
 //   bf16 L2 (:164-197): float difference; infinite difference -> +INF; NaN difference skipped
 template <int VT, int MC>
-__device__ __noinline__ float special_row_distance(const uint8_t *row, const uint8_t *query, int nelem, int root) {
+__device__ __forceinline__ float special_row_distance_body(const uint8_t *row, const uint8_t *query, int nelem, int root) {
     const uint16_t *yb = reinterpret_cast<const uint16_t *>(row), *xb = reinterpret_cast<const uint16_t *>(query);
     float s = 0.0f, nx = 0.0f, ny = 0.0f;
     double sd = 0.0;                                                            // bf16 L2
@@ -330,6 +330,11 @@ __device__ __noinline__ float special_row_distance(const uint8_t *row, const uin
         else d = 1.0f - fminf(1.0f, fmaxf(-1.0f, __fdiv_rn(s, den)));
     }
     return (fabsf(d) <= 8.0f * FLT_EPSILON) ? 0.0f : d;
+}
+// out of line: the rare path stays out of the hot loop's registers
+template <int VT, int MC>
+__device__ __noinline__ float special_row_distance(const uint8_t *row, const uint8_t *query, int nelem, int root) {
+    return special_row_distance_body<VT, MC>(row, query, nelem, root);
 }
 
 __device__ __forceinline__ void accum_reduce(Accum &A, int P) {

@@ -1320,7 +1320,8 @@ static int vt_filter_quant_stream(sqlite3_vtab_cursor *c, int n, const char *s, 
  * No counterpart in the reference (one vector per xFilter, :1774-1776); this is the SQL door to vsb_scan_topk's batch path:
  * `vectors` is a BLOB of B x dimension elements of the column's type back to back, or a flat JSON array of B x dimension
  * numbers.  Rows are (query, id, distance) with query = 0 .. B-1, each query's rows exactly those of the single-query function
- * in the same order.  B >= 16 on F16/BF16/INT8/UINT8 data (not L1) is scored on the tensor cores. */
+ * in the same order.  B >= 16 on F16/BF16/INT8/UINT8 data is scored on the tensor cores, except L1, which is batched on the
+ * CUDA cores for every column type (FLOAT32 too). */
 enum { BCOL_QUERY = 4, BCOL_ID = 5, BCOL_DISTANCE = 6 };
 
 static int vt_connect_batch(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {

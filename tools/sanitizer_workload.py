@@ -1,5 +1,5 @@
 """Small invocations of every kernel family for compute-sanitizer (memcheck / racecheck): single-query scans (staged + DIRECT,
-k <= 32 and generic filters, all-distances), group launches, the tensor-core batch path (int8 + bf16), sharded merge."""
+k <= 32 and generic filters, all-distances), group launches, the tensor-core and L1 batch paths (int8 + bf16), sharded merge."""
 import os
 import sys
 
@@ -31,10 +31,12 @@ ix.scan_submit_group(api.L2, np.ascontiguousarray(q[:8]), q.strides[0], 8, 20, F
 for j in range(8):
     ix.collect(j, 20)
 ix.scan_topk(api.L2, q, 20)          # tensor-core batch path (int8)
+ix.scan_topk(api.L1, q, 20)          # L1 batch path (l1_batch_kernel, int8)
 ix.close()
 xb = (rng.standard_normal((20000, 200)).astype(np.float32).view(np.uint32) >> 16).astype(np.uint16)
 ixb = index(api.BF16, xb)
 ixb.scan_topk(api.DOT, xb[:32].copy(), 10)
+ixb.scan_topk(api.L1, xb[:32].copy(), 10)
 ixb.scan_topk(api.L2, xb[0].copy(), 10)
 ixb.close()
 # f16 DOT, k = 1: row 5 holds +Inf against all-positive queries, so every query's only slot is -Inf after level 0 and the

@@ -127,6 +127,71 @@ struct TileWalk {
     }
 };
 
+// The stage ring of both scoring kernels: NS stages [A | B] of one 128-byte K slice each (A = the 128 corpus rows of a tile,
+// B = its N queries; 128B-swizzled, 1024-aligned, filled by TMA), then the full / empty mbarriers of kTcMaxStages stages.
+// full[s] completes on the producer's arrival plus the stage's bytes, empty[s] on `consumers` arrivals of the consumers that
+// have read stage s.  end() is the first byte after the barriers.
+template <int N>
+struct StageRing {
+    static constexpr uint32_t a_bytes = kTcM * kTcKBytes, b_bytes = (uint32_t)N * kTcKBytes;
+    static constexpr uint32_t stage_bytes = a_bytes + b_bytes;
+    uint8_t *stages;
+    uint64_t *full, *empty;
+    __device__ __forceinline__ StageRing(uint8_t *smem, int NS)
+        : stages(smem), full(reinterpret_cast<uint64_t *>(smem + (size_t)NS * stage_bytes)), empty(full + kTcMaxStages) {}
+    __device__ __forceinline__ uint8_t *stage(int s) const { return stages + (size_t)s * stage_bytes; }
+    __device__ __forceinline__ uint8_t *end() const { return reinterpret_cast<uint8_t *>(empty + kTcMaxStages); }
+    __device__ __forceinline__ void init(int consumers) const {   // thread 0; the caller syncs the block before any use
+        if (threadIdx.x == 0) {
+            for (int i = 0; i < kTcMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], consumers); }
+            fence_barrier_init();
+        }
+    }
+    // the TMA producer: the whole warp walks the tiles, one lane issues each stage's two loads
+    __device__ __forceinline__ void produce(TileWalk tw, int KB, int NS, const CUtensorMap *tmA, const CUtensorMap *tmB) const {
+        int s = 0;
+        uint32_t ph = 1;                                                       // parity to wait for on empty[s]: the first pass is free
+        for (uint32_t tl = 0; tl < tw.count; ++tl, tw.next()) {
+            const int row0 = (int)(tw.mt() * kTcM), col0 = tw.ng() * N;
+            for (int kb = 0; kb < KB; ++kb) {
+                mbar_wait(&empty[s], ph);
+                if (elect_one()) {
+                    mbar_expect_tx(&full[s], stage_bytes);
+                    uint8_t *st = stage(s);
+                    tma_load_2d(st, tmA, kb * kTcKBytes, row0, &full[s]);
+                    tma_load_2d(st + a_bytes, tmB, kb * kTcKBytes, col0, &full[s]);
+                }
+                __syncwarp();
+                if (++s == NS) { s = 0; ph ^= 1u; }
+            }
+        }
+    }
+};
+
+// Appends the calling lane's `mine` hits to the candidate log with one atomic per warp (call it from the whole warp, inside
+// the warp's ballot that some lane may have hits): an inclusive scan of the counts, one atomicAdd by lane 31, then every lane
+// writes its hits from its offset on; positions at or past cand_cap are counted but not stored.  visit(emit) calls
+// emit(row, query) once for each of the lane's hits.
+template <class Visit>
+__device__ __forceinline__ void append_hits(const TcParams &prm, int lane, int mine, Visit visit) {
+    int incl = mine;
+    for (int off = 1; off < 32; off <<= 1) {
+        const int o = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+        if (lane >= off) incl += o;
+    }
+    const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+    unsigned base = 0;
+    if (lane == 31) base = atomicAdd(prm.cand_count, (unsigned)total);
+    base = __shfl_sync(0xFFFFFFFFu, base, 31);
+    unsigned w = base + (unsigned)(incl - mine);
+    if (mine) {
+        visit([&](long long row, int query) {
+            if (w < prm.cand_cap) prm.cand[w] = make_uint2((uint32_t)row, (uint32_t)query);
+            ++w;
+        });
+    }
+}
+
 // Accumulator layout of one consumer warpgroup (m64nN, PTX ISA "wgmma register fragments"): thread t of the warpgroup holds
 // rows  ra = 16 * (t / 32) + (t % 32) / 4  and  ra + 8  of its 64 rows; d[4j + 0/1] are row ra, columns 8j + 2 (t % 4) + 0/1,
 // d[4j + 2/3] row ra + 8, the same columns.
@@ -141,21 +206,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
     using Acc = typename std::conditional<INT8, uint32_t, float>::type;
     extern __shared__ __align__(1024) uint8_t tsm[];
     const int NS = prm.nstages;
-    constexpr uint32_t a_bytes = kTcM * kTcKBytes, b_bytes = (uint32_t)N * kTcKBytes;
-    constexpr uint32_t stage_bytes = a_bytes + b_bytes;
-    uint8_t *stages = tsm;                                                     // [NS][A | B], 1024-aligned
-    uint8_t *tail = tsm + (size_t)NS * stage_bytes;
-    uint64_t *full = reinterpret_cast<uint64_t *>(tail);
-    uint64_t *empty = full + kTcMaxStages;
-    uint32_t *qc_s = reinterpret_cast<uint32_t *>(empty + kTcMaxStages);      // [NG*N]
+    const StageRing<N> ring(tsm, NS);
+    uint32_t *qc_s = reinterpret_cast<uint32_t *>(ring.end());                // [NG*N]
     uint32_t *qcm_s = qc_s + prm.NG * N;                                       // [NG*N/32] weakest bound of each 32-column chunk
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kTcMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kTcConsumers); }
-        fence_barrier_init();
-    }
+    ring.init(kTcConsumers);                                                   // one arrival per consumer warpgroup
     for (int i = threadIdx.x; i < prm.NG * N; i += kTcThreads) qc_s[i] = __float_as_uint(prm.qc[i]);
     __syncthreads();
     const bool chunk = INT8 && prm.chunk_test;
@@ -178,23 +235,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
     tw.init(prm);
     const int KB = prm.KB;
 
-    if (warp == kTcConsumers * 4) {                                            // ===== TMA producer: the whole warp walks, one lane issues
-        int s = 0;
-        uint32_t ph = 1;                                                       // parity to wait for on empty[s]: the first pass is free
-        for (uint32_t tl = 0; tl < tw.count; ++tl, tw.next()) {
-            const int row0 = (int)(tw.mt() * kTcM), col0 = tw.ng() * N;
-            for (int kb = 0; kb < KB; ++kb) {
-                mbar_wait(&empty[s], ph);
-                if (elect_one()) {
-                    mbar_expect_tx(&full[s], stage_bytes);
-                    uint8_t *st = stages + (size_t)s * stage_bytes;
-                    tma_load_2d(st, &tmA, kb * kTcKBytes, row0, &full[s]);
-                    tma_load_2d(st + a_bytes, &tmB, kb * kTcKBytes, col0, &full[s]);
-                }
-                __syncwarp();
-                if (++s == NS) { s = 0; ph ^= 1u; }
-            }
-        }
+    if (warp == kTcConsumers * 4) {                                            // ===== TMA producer
+        ring.produce(tw, KB, NS, &tmA, &tmB);
         return;
     }
 
@@ -218,21 +260,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
         }
         int prev = -1;
         for (int kb = 0; kb < KB; ++kb) {
-            mbar_wait(&full[s], ph);
-            const uint8_t *st = stages + (size_t)s * stage_bytes;
-            const uint64_t ad = gmma_desc_sw128(st + wg * 64 * kTcKBytes), bd = gmma_desc_sw128(st + a_bytes);
+            mbar_wait(&ring.full[s], ph);
+            const uint8_t *st = ring.stage(s);
+            const uint64_t ad = gmma_desc_sw128(st + wg * 64 * kTcKBytes), bd = gmma_desc_sw128(st + ring.a_bytes);
             wgmma_fence();
 #pragma unroll
             for (int k4 = 0; k4 < kTcKBytes / 32; ++k4)                        // K = 32 bytes per MMA: advance the start address by 2 (x16 B)
                 tc_mma<KIND, N>(d, ad + (uint64_t)(2 * k4), bd + (uint64_t)(2 * k4), (uint32_t)((kb | k4) != 0));
             wgmma_commit();
             wgmma_wait<1>();                                                   // the previous K block's MMAs have read their stage
-            if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
+            if (prev >= 0 && t == 0) mbar_arrive(&ring.empty[prev]);
             prev = s;
             if (++s == NS) { s = 0; ph ^= 1u; }
         }
         wgmma_wait<0>();
-        if (t == 0) mbar_arrive(&empty[prev]);                                 // the producer refills it while the scores are tested
+        if (t == 0) mbar_arrive(&ring.empty[prev]);                                // the producer refills it while the scores are tested
         if constexpr (MC == MC_TC_SCORES) {
             const int ncol = prm.nq - ng * N;
 #pragma unroll
@@ -297,48 +339,35 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
                        (rowvalid[1] && (tc_hit<INT8, MC>(bits(4 * j + 2), c.x, rowf[1], rowi[1]) | tc_hit<INT8, MC>(bits(4 * j + 3), c.y, rowf[1], rowi[1])));
             }
         }
-        if (__ballot_sync(0xFFFFFFFFu, any)) {                                 // rare: append (row, query) hits, one atomic per warp
+        if (__ballot_sync(0xFFFFFFFFu, any)) {                                 // rare: append (row, query) hits
             const int ncol = prm.nq - ng * N;                                  // padded query columns are never reported
             int mine = 0;
             if (any) {
 #pragma unroll
                 for (int i = 0; i < N / 2; ++i) mine += (hit(i) && 8 * (i >> 2) + cq + (i & 1) < ncol) ? 1 : 0;
             }
-            int incl = mine;
-            for (int off = 1; off < 32; off <<= 1) {
-                const int o = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-                if (lane >= off) incl += o;
-            }
-            const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-            unsigned base = 0;
-            if (lane == 31) base = atomicAdd(prm.cand_count, (unsigned)total);
-            base = __shfl_sync(0xFFFFFFFFu, base, 31);
-            unsigned w = base + (unsigned)(incl - mine);
-            if (mine) {
+            append_hits(prm, lane, mine, [&](auto emit) {
 #pragma unroll
                 for (int i = 0; i < N / 2; ++i) {
                     const int col = 8 * (i >> 2) + cq + (i & 1);
-                    if (hit(i) && col < ncol) {
-                        if (w < prm.cand_cap) prm.cand[w] = make_uint2((uint32_t)row[(i >> 1) & 1], (uint32_t)(ng * N + col));
-                        ++w;
-                    }
+                    if (hit(i) && col < ncol) emit(row[(i >> 1) & 1], ng * N + col);
                 }
-            }
+            });
         }
     }
 }
 
 // ------------------------------------------------------------------ L1 scores on the CUDA cores
 // sum |row_i - q_i| has no GEMM form, but over a batch it is the same dense all-pairs work, compute-bound once the corpus is
-// read once per level.  l1_batch_kernel walks the tiles of tc_scan_kernel (TileWalk, the same TMA producer warp and stage ring:
-// 128 corpus rows and N queries per 128-byte K slice, 128B swizzle, full / empty mbarriers) and adds the sums on the CUDA
-// cores.  Consumer warp w owns queries [w N/8, (w + 1) N/8) of the tile and lane l the rows l + 32 i, i < 4: a thread keeps
+// read once per level.  l1_batch_kernel walks the tiles of tc_scan_kernel (TileWalk, and StageRing's TMA producer warp and
+// stage ring: 128 corpus rows and N queries per 128-byte K slice, 128B swizzle, full / empty mbarriers) and adds the sums on
+// the CUDA cores.  Consumer warp w owns queries [w N/8, (w + 1) N/8) of the tile and lane l the rows l + 32 i, i < 4: a thread keeps
 // 4 x N/8 sums in registers.  Every 16-byte chunk is one LDS.128; the query chunks a warp reads are broadcasts, and chunk c of
 // row r sits at c ^ (r & 7), so the 8 lanes of one LDS.128 phase hit 8 different 16-byte bank groups.
 //   int8 / uint8: VABSDIFF4 + IDP.4A per 4 element pairs, exact int32 (the same instructions as accum16).
 //   f32 / f16 / bf16: s += |x - y| in fp32, every term formed with one rounding, like accum16 (only the order of the sum differs).
 // The epilogue tests every (row, query) against qc[query] from registers and appends hits to the candidate log with one atomic
-// per warp, as tc_scan_kernel does: integer types (float)S < qc with qc = U, exactly the refine's keep condition; fp types
+// per warp (append_hits): integer types (float)S < qc with qc = U, exactly the refine's keep condition; fp types
 // !(s >= qc) with the conservative constant of conservative_qc (NaN scores are hits).  Padded query columns are never
 // reported.  prm.mc == MC_TC_SCORES stores every score of rows [r0, r1) instead (vsb_debug_tc_level mode 1).
 constexpr int kL1Warps = 8;
@@ -354,40 +383,18 @@ __global__ void __launch_bounds__(kL1Threads, 1) l1_batch_kernel(const __grid_co
     using Acc = typename std::conditional<INT8, uint32_t, float>::type;
     extern __shared__ __align__(1024) uint8_t lsm[];
     const int NS = prm.nstages;
-    constexpr uint32_t a_bytes = kTcM * kTcKBytes, b_bytes = (uint32_t)N * kTcKBytes;
-    constexpr uint32_t stage_bytes = a_bytes + b_bytes;
-    uint8_t *stages = lsm;                                                     // [NS][A | B], 1024-aligned
-    uint64_t *full = reinterpret_cast<uint64_t *>(lsm + (size_t)NS * stage_bytes);
-    uint64_t *empty = full + kTcMaxStages;
+    const StageRing<N> ring(lsm, NS);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kTcMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kL1Warps); }
-        fence_barrier_init();
-    }
+    ring.init(kL1Warps);                                                       // one arrival per consumer warp
     __syncthreads();
 
     TileWalk tw;
     tw.init(prm);
     const int KB = prm.KB;
 
-    if (warp == kL1Warps) {                                                    // ===== TMA producer (as in tc_scan_kernel)
-        int s = 0;
-        uint32_t ph = 1;
-        for (uint32_t tl = 0; tl < tw.count; ++tl, tw.next()) {
-            const int row0 = (int)(tw.mt() * kTcM), col0 = tw.ng() * N;
-            for (int kb = 0; kb < KB; ++kb) {
-                mbar_wait(&empty[s], ph);
-                if (elect_one()) {
-                    mbar_expect_tx(&full[s], stage_bytes);
-                    uint8_t *st = stages + (size_t)s * stage_bytes;
-                    tma_load_2d(st, &tmA, kb * kTcKBytes, row0, &full[s]);
-                    tma_load_2d(st + a_bytes, &tmB, kb * kTcKBytes, col0, &full[s]);
-                }
-                __syncwarp();
-                if (++s == NS) { s = 0; ph ^= 1u; }
-            }
-        }
+    if (warp == kL1Warps) {                                                    // ===== TMA producer
+        ring.produce(tw, KB, NS, &tmA, &tmB);
         return;
     }
 
@@ -406,10 +413,10 @@ __global__ void __launch_bounds__(kL1Threads, 1) l1_batch_kernel(const __grid_co
 #pragma unroll
             for (int j = 0; j < C; ++j) acc[i][j] = 0;
         for (int kb = 0; kb < KB; ++kb) {
-            mbar_wait(&full[s], ph);
+            mbar_wait(&ring.full[s], ph);
             if (ncol > 0) {                                                    // warp-uniform: padding-only warps just pass the stage on
-                const uint8_t *A = stages + (size_t)s * stage_bytes + lane * kTcKBytes;
-                const uint8_t *B = stages + (size_t)s * stage_bytes + a_bytes + q0 * kTcKBytes;
+                const uint8_t *A = ring.stage(s) + lane * kTcKBytes;
+                const uint8_t *B = ring.stage(s) + ring.a_bytes + q0 * kTcKBytes;
 #pragma unroll 2
                 for (uint32_t c = 0; c < kTcKBytes / 16; ++c) {
                     uint4 rv[R];
@@ -448,7 +455,7 @@ __global__ void __launch_bounds__(kL1Threads, 1) l1_batch_kernel(const __grid_co
                 }
             }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[s]);                             // this warp has read the stage
+            if (lane == 0) mbar_arrive(&ring.empty[s]);                        // this warp has read the stage
             if (++s == NS) { s = 0; ph ^= 1u; }
         }
         if (ncol <= 0) continue;
@@ -486,27 +493,14 @@ __global__ void __launch_bounds__(kL1Threads, 1) l1_batch_kernel(const __grid_co
         for (int i = 0; i < R; ++i)
 #pragma unroll
             for (int j = 0; j < C; ++j) mine += hit(i, j) ? 1 : 0;
-        if (__ballot_sync(0xFFFFFFFFu, mine != 0)) {                           // rare: append (row, query) hits, one atomic per warp
-            int incl = mine;
-            for (int off = 1; off < 32; off <<= 1) {
-                const int o = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-                if (lane >= off) incl += o;
-            }
-            const int total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-            unsigned base = 0;
-            if (lane == 31) base = atomicAdd(prm.cand_count, (unsigned)total);
-            base = __shfl_sync(0xFFFFFFFFu, base, 31);
-            unsigned w = base + (unsigned)(incl - mine);
-            if (mine) {
+        if (__ballot_sync(0xFFFFFFFFu, mine != 0)) {                           // rare: append (row, query) hits
+            append_hits(prm, lane, mine, [&](auto emit) {
 #pragma unroll
                 for (int i = 0; i < R; ++i)
 #pragma unroll
                     for (int j = 0; j < C; ++j)
-                        if (hit(i, j)) {
-                            if (w < prm.cand_cap) prm.cand[w] = make_uint2((uint32_t)row[i], (uint32_t)(qbase + j));
-                            ++w;
-                        }
-            }
+                        if (hit(i, j)) emit(row[i], qbase + j);
+            });
         }
     }
 }

@@ -777,6 +777,36 @@ def test_batch_all_slots_neg_inf_end_to_end(oracle, vtype, k):
         ix.close()
 
 
+# ---------------------------------------------------------------------------------------------- tile widths of the scoring kernels
+def test_tc_level_tile_widths():
+    """vsb_debug_tc_level takes exactly the query tiles a scoring kernel exists for: N = 32 .. 256 for int8 / uint8 on the
+    tensor cores, 32 .. 128 for f16 / bf16 and for L1 on every type, N = 0 (the production width) wherever a kernel exists;
+    every other N, and f32 with a tensor-core metric, is VSB_EINVAL"""
+    vs = _vs()
+    rng = np.random.Generator(np.random.PCG64(120))
+    n, dim, nq = 256, 64, 40
+    for vtype in (po.F32, po.F16, po.BF16, po.U8, po.I8):
+        make = (lambda m: _int_data(vtype, m, dim, rng)) if vtype in (po.I8, po.U8) else (lambda m: fam.make("normal", vtype, m, dim, rng))
+        ix = _index(vtype, make(n))
+        q = make(nq)
+        for metric in (po.L2, po.DOT, po.COS, po.L1):
+            if metric == po.L1:
+                widths = {32, 64, 128}
+            elif vtype == po.F32:
+                widths = set()
+            else:
+                widths = {32, 64, 128, 256} if vtype in (po.I8, po.U8) else {32, 64, 128}
+            for N in (0, 16, 32, 48, 64, 128, 256, 512):
+                ok = N in widths or (N == 0 and bool(widths))
+                try:
+                    ix.debug_tc_level(metric, q, np.full(nq, np.inf, np.float32), 0, 128, N=N, cap=1 << 16)
+                    rc = 0
+                except vs.VsbError as e:
+                    rc = e.rc
+                assert rc == (0 if ok else vs.api.EINVAL), (vtype, metric, N, rc)
+        ix.close()
+
+
 # ---------------------------------------------------------------------------------------------- (h) row norms
 @pytest.mark.parametrize("vtype,dim", [(po.I8, 16), (po.I8, 100), (po.I8, 4096), (po.U8, 16), (po.U8, 100), (po.U8, 4096), (po.U8, 33040)])
 def test_row_norms_int_exact(vtype, dim):

@@ -279,8 +279,9 @@ VSB_API int vsb_debug_refine(vsb_index *ix, int metric, const void *queries, int
 VSB_API int vsb_debug_replay(vsb_index *ix, int metric, const void *queries, int nq, int k, int level0, const uint32_t *bucket,
                              const uint32_t *bcount, float *slot_d, uint32_t *slot_row, int *slot_mi, int acc_cap, uint32_t *acc_log,
                              int *acc_count, int final_sort, float *out_U, uint32_t *out_qc, uint32_t *out_bcount, uint32_t *out_stats);
-/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","fuse_mb","scan_streams","xwait_ms","epi_chunk","push_mode","merge_stream" (experiment)};
- * values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
+/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","fuse_mb","scan_streams","xwait_ms","epi_chunk","push_mode","merge_stream" (experiment),"f32_batch"};
+ * "f32_batch" = 1: f32 columns batch L2 / cosine / dot queries on the tensor cores in TF32 (default 0, or VSB_F32_BATCH=1 in the
+ * environment when the library loads; per process).  Values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);
 
 #ifdef __cplusplus

@@ -19,7 +19,7 @@
 
 namespace vsb {
 
-enum { TK_BF16 = 0, TK_F16 = 1, TK_I8 = 2, TK_U8 = 3 };
+enum { TK_BF16 = 0, TK_F16 = 1, TK_I8 = 2, TK_U8 = 3, TK_TF32 = 4 };   // TK_TF32: f32 columns (option f32_batch)
 // warps 0-7: two consumer warpgroups (rows 0-63 and 64-127 of the corpus tile), warp 8: TMA producer
 constexpr int kTcConsumers = 2;
 constexpr int kTcThreads = kTcConsumers * 128 + 32;
@@ -40,7 +40,7 @@ struct TcParams {
     int nstages;            // ring depth (2..kTcMaxStages)
     int mc;                 // MC_L2 / MC_COS / MC_DOT (l1_batch_kernel: MC_L1), or MC_TC_SCORES
     int chunk_test;         // integer kinds: test 32-column chunks before single scores (see tc_scan_kernel)
-    float eps;              // fp kinds: relative slack of the tensor-core score, see tc_fp_eps
+    float eps;              // fp kinds: relative slack of the tensor-core score, see tc_eps
     const float *qc;        // [NG*N] per-query constant (float, or int bit pattern for the integer kinds)
     const void *norms;      // [n] float (fp kinds) or int (integer kinds): sum of squares of each row
     uint2 *cand;            // (row, query)
@@ -76,7 +76,8 @@ __device__ __forceinline__ void tc_mma(Acc (&d)[N / 2], uint64_t a, uint64_t b, 
     if constexpr (KIND == TK_BF16) Wgmma<N>::bf16(d, a, b, scale_d);
     else if constexpr (KIND == TK_F16) Wgmma<N>::f16(d, a, b, scale_d);
     else if constexpr (KIND == TK_I8) Wgmma<N>::s8(d, a, b, scale_d);
-    else Wgmma<N>::u8(d, a, b, scale_d);
+    else if constexpr (KIND == TK_U8) Wgmma<N>::u8(d, a, b, scale_d);
+    else Wgmma<N>::tf32(d, a, b, scale_d);
 }
 
 // the per-element candidate test.  fp kinds use negated comparisons so that NaN scores count as hits.
@@ -736,6 +737,16 @@ __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fm
 // dim * 2^-24 * ... only up to dim ~ 1600: the verdict's weak item 1.)
 __host__ __device__ inline float tc_fp_eps(int dim) { return (float)dim * 9.5367431640625e-7f; }
 
+// Slack of the TF32 score of f32 columns (TK_TF32), relative to |q||r| like tc_fp_eps.  PTX does not say how the tensor core
+// reduces the f32 words in shared memory to tf32; assume truncation to 10 explicit mantissa bits, which also covers rounding to
+// nearest: q~ = q (1 + a), r~ = r (1 + b), |a|, |b| < 2^-10.  A product of two tf32 values (11 x 11 significant bits) is exact in
+// fp32, so per term |q~ r~ - q r| <= (2^-9 + 2^-20) |q r|, at most (2^-9 + 2^-20) sum |q_i r_i| over the row.  The accumulation
+// of the (slightly larger) products, the refine's own fp32 chain and the norms add the same dim-proportional terms as in the
+// bf16 analysis above, which tc_fp_eps covers.  eps = 2^-8 + dim * 2^-20: twice the operand term plus tc_fp_eps (exact in
+// float for any dim below 2^24 - 2^12).
+__host__ __device__ inline float tc_tf32_eps(int dim) { return 0.00390625f + tc_fp_eps(dim); }
+__host__ __device__ inline float tc_eps(int vt, int dim) { return vt == T_F32 ? tc_tf32_eps(dim) : tc_fp_eps(dim); }   // vt: T_*
+
 // Bound of the fp L1 score.  l1_batch_kernel and the refine both add the same dim non-negative terms t_i = fl(|x_i - y_i|)
 // (one rounding each; padding terms are exact zeros), in different orders.  With u = 2^-24, every term is within u of
 // |x_i - y_i| and any summation order of dim terms within gamma_(dim-1) of their sum, so for ANY order the computed sum s
@@ -777,7 +788,7 @@ __device__ inline float conservative_qc(int vt, int mc, int root, float U, const
     }
     const float qq = reinterpret_cast<const float *>(qnorm)[q];
     if (!(U < 3.0e38f)) return (mc == MC_COS) ? -1e30f : -INFINITY;
-    const float eps = tc_fp_eps(dim);
+    const float eps = tc_eps(vt, dim);
     // DOT: d = -s < U.  |s_tc - s_refine| <= eps |q||r| <= eps |q| rnmax (rnmax = largest row norm, 1.0001 for its own rounding)
     if (mc == MC_DOT) return -U - (eps * sqrtf(qq) * rnmax * 1.0001f + 4e-7f * fabsf(U)) - 1e-30f;
     if (mc == MC_L2) {

@@ -15,6 +15,7 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <limits>
 #include <mutex>
@@ -51,6 +52,12 @@ int g_opt_scan_streams = 2;    // 2: consecutive scan launches alternate between
                                // as soon as the CTA of launch i on it exits (one scan CTA fits per SM): no grid-wide drain between
                                // launches, per-SM speed differences turn into an earlier start of the next query.  1: one stream.
 int g_opt_push_mode = 1;       // exchange: 1 (default) = a small kernel on the exchange stream pushes a finished group's heads; 0 = the filter's last block pushes its head itself (fused: the filter stream then waits for NVLink acknowledgements; not measured on H100)
+// 1: f32 columns batch L2 / cosine / dot queries on the tensor cores in TF32 (tc_kind_of); 0: per query.  Set at load from
+// VSB_F32_BATCH, so that users of the SQLite extension can turn it on; per process
+int g_opt_f32_batch = [] {
+    const char *e = getenv("VSB_F32_BATCH");
+    return (e && atoi(e) > 0) ? 1 : 0;
+}();
 int g_opt_xwait_ms = 10000;    // exchange: how long the receiving side waits for a peer's head before it reports an error (a dead
                                // peer, not a slow one: ranks sharing one GPU or a busy host can start a batch seconds apart)
 
@@ -896,6 +903,7 @@ int vsb_set_option(const char *name, int value) {
     else if (!strcmp(name, "scan_streams")) p = &g_opt_scan_streams;
     else if (!strcmp(name, "xwait_ms")) p = &g_opt_xwait_ms;
     else if (!strcmp(name, "push_mode")) p = &g_opt_push_mode;
+    else if (!strcmp(name, "f32_batch")) p = &g_opt_f32_batch;
     if (!p) return fail(VSB_EINVAL, "unknown option %s", name);
     if (value < 0) return fail(VSB_EINVAL, "option %s: values are non-negative", name);   // so that a negative return is always an error
     int old = *p;

@@ -141,9 +141,7 @@ VSB_API int vsb_merge_result_blocks(const void *blocks, int world, int64_t block
                                     int64_t *out_rowids, double *out_dist);
 /* the same for a GROUP of nq independent queries in one call (query j at queries + j * query_stride; slots first_slot ..
  * first_slot + nq - 1): what the sharded launcher uses so that its per-query host cost stays far below one shard scan.
- * With option "fuse_mb" > 0 (off by default) and one query reading fewer MB than that, up to 8 queries share ONE scan
- * launch: every CTA starts the next query as soon as its streams are done (no launch gap, the TMA ring runs across the
- * boundary); results are unchanged. */
+ * Each query gets its own scan and filter launch, exactly as from vsb_scan_submit. */
 VSB_API int vsb_scan_submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device,
                                   int k, int fetch, int first_slot);
 /* vsb_merge_result_blocks for a gathered group: query j's block of shard r is at blocks + r * rank_stride + j * block_stride;
@@ -169,10 +167,9 @@ VSB_API int vsb_batch_merge(vsb_index *ix, const void *d_blocks, int world, int6
 VSB_API int vsb_index_lookup_rowids(const vsb_index *ix, const int64_t *seq, int64_t n, int64_t *out);
 /* ---- exchange over NVLink peer memory: one process per GPU (torchrun), no collective library on the data path -----------
  * The final all-gather of the shards' per-query result heads (SURVEY §8e; north_star "final allgather of per-shard top-k over
- * NVLink") is a store kernel: after a group's filters, push_heads_kernel (the default; option push_mode = 0: the filter block that
- * completes a head) stores each head into row `rank` of EVERY peer's gather buffer (cudaIpc-mapped peer memory) and raises an
- * arrival flag; the receiver waits on the flags on its own stream and copies the gathered heads to pinned host memory once per
- * group.
+ * NVLink") is a store kernel: after a group's filters, push_heads_kernel stores each head into row `rank` of EVERY peer's
+ * gather buffer (cudaIpc-mapped peer memory) and raises an arrival flag; the receiver waits on the flags on its own stream and
+ * copies the gathered heads to pinned host memory once per group.
  * setup (once): every rank calls vsb_exchange_export (allocates its gather buffer, returns a 64-byte cudaIpc handle), the
  * launcher all-gathers the handles (any transport: they are 64 bytes), every rank calls vsb_exchange_attach with all of them.
  * per group of 1..8 independent queries (the same call sequence on every rank): vsb_exchange_submit launches scan + filter
@@ -279,7 +276,7 @@ VSB_API int vsb_debug_refine(vsb_index *ix, int metric, const void *queries, int
 VSB_API int vsb_debug_replay(vsb_index *ix, int metric, const void *queries, int nq, int k, int level0, const uint32_t *bucket,
                              const uint32_t *bcount, float *slot_d, uint32_t *slot_row, int *slot_mi, int acc_cap, uint32_t *acc_log,
                              int *acc_count, int final_sort, float *out_U, uint32_t *out_qc, uint32_t *out_bcount, uint32_t *out_stats);
-/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","fuse_mb","scan_streams","xwait_ms","epi_chunk","push_mode","merge_stream" (experiment),"f32_batch"};
+/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","scan_streams","xwait_ms","epi_chunk","f32_batch"};
  * "f32_batch" = 1: f32 columns batch L2 / cosine / dot queries on the tensor cores in TF32 (default 0, or VSB_F32_BATCH=1 in the
  * environment when the library loads; per process).  Values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);

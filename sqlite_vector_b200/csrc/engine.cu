@@ -40,18 +40,13 @@ int g_opt_ring_bytes = 0;      // 0: use all shared memory left
 int g_opt_no_batch = 0;        // 1: never take the tensor-core batch path
 int g_opt_batch_debug = 0;     // 1: print per-stage timings of the batch path to stderr (serialises the stages)
 int g_opt_batch_m0 = 128;      // batch path: rows refined exhaustively before the first tensor-core level
-int g_opt_merge_stream = 1;    // process exchange, batched queries: wait + merge + copy back on their own stream (overlaps the next batch's levels)
 int g_opt_batch_growth = 8;    // batch path: each tensor-core level covers rows [m, growth*m) (capped by k, see batch_growth)
-int g_opt_fuse_mb = 0;         // > 0: vsb_scan_submit_group fuses a group into ONE scan launch when one query's scan reads less than this
-                               // many MB (saves 7 of 8 launches for a slow launcher).  Off by default: a persistent 8-query launch leaves
-                               // the NCCL all-gather of the previous group no SM until it ends.  Not measured on H100.
 int g_opt_balance = 1;         // 1: adaptive row partition of the single-query scan (per-CTA speeds feed the next partition)
 int g_opt_epi_chunk = 1;       // 1: integer tensor-core epilogue tests 32-column chunks (max score vs weakest bound) before any per-column work
 int g_opt_time_kernels = 0;    // 1: bracket every kernel launch with CUDA events (bench.py roofline leg)
 int g_opt_scan_streams = 2;    // 2: consecutive scan launches alternate between two streams, so the CTAs of launch i+1 take over each SM
                                // as soon as the CTA of launch i on it exits (one scan CTA fits per SM): no grid-wide drain between
                                // launches, per-SM speed differences turn into an earlier start of the next query.  1: one stream.
-int g_opt_push_mode = 1;       // exchange: 1 (default) = a small kernel on the exchange stream pushes a finished group's heads; 0 = the filter's last block pushes its head itself (fused: the filter stream then waits for NVLink acknowledgements; not measured on H100)
 // 1: f32 columns batch L2 / cosine / dot queries on the tensor cores in TF32 (tc_kind_of); 0: per query.  Set at load from
 // VSB_F32_BATCH, so that users of the SQLite extension can turn it on; per process
 int g_opt_f32_batch = [] {
@@ -115,17 +110,12 @@ constexpr int kMaxK = 256;               // candidate path; larger k uses the al
 constexpr int kSlots = 32;               // result slots: queries in flight (the sharded exchange moves groups of them; a rank may have at most
                                          // kSlots / 2 queries in flight so that a peer never overwrites a gather row that is still being read)
 
-// scan workspace of ONE query (per-stream k-lists / CTA lists, in-CTA bounds, candidate logs): written by scan_kernel,
-// read by filter_kernel
-struct QWork {
+// Scan workspace of one query (per-stream k-lists / CTA lists, in-CTA bounds, candidate logs): written by scan_kernel, read
+// by filter_kernel.  The Works rotate so that the filter of launch i (filter stream) overlaps the scan of launch i+1.
+struct Work {
     float *d_lists = nullptr, *d_tlocal = nullptr;
     uint2 *d_logs = nullptr;
     int *d_counts = nullptr;
-};
-// One launch scans up to kMaxGroup independent queries back to back (scan_kernel); a Work holds their workspaces plus what
-// is per launch.  Two Works alternate so that the filters of launch i (filter stream) overlap the scan of launch i+1.
-struct Work {
-    QWork q[kMaxGroup];
     long long *d_bounds = nullptr;   // [CTAs + 1] adaptive tile partition used by the NEXT scan on this workspace
     unsigned *d_cta_time = nullptr;  // [CTAs] cycles each scan CTA took (written by scan_kernel, read by filter_kernel)
     long long bounds_tiles = -1;     // total tiles the bounds were laid out for (-1: not initialised)
@@ -188,7 +178,6 @@ struct vsb_index {
     // optional per-kernel event timing (vsb_profile_read)
     std::vector<cudaEvent_t> prof_ev;   // quadruples: before scan, after scan (scan stream), before filter, after filter (filter stream)
     std::vector<int> prof_kind;         // 1 = scan only, 2 = scan + filter
-    std::vector<int> prof_nq;           // queries scanned by the timed launch
     size_t prof_used = 0;
     unsigned prof_tick = 0;
     size_t dev_bytes = 0;
@@ -246,7 +235,9 @@ Plan make_plan(const vsb_index *ix, int kcap) {
     const int pitch = ix->pitch;
     int log2P = 0;
     while (log2P < 5 && (32 >> log2P) * (long long)pitch > g_opt_stage_bytes) ++log2P;
-    const size_t fixed = kBarrierBytes + (((size_t)2 * pitch + (size_t)2 * kWarps * kcap * 4 + 127) & ~(size_t)127);   // 2 query + 2 list buffers
+    // Room for 2 query + 2 list buffers, although scan_kernel uses one of each.  Giving the ring that room would change the
+    // plan at many shapes (some dims would turn from DIRECT to staged) and needs its own measurement (DESIGN §8).
+    const size_t fixed = kBarrierBytes + (((size_t)2 * pitch + (size_t)2 * kWarps * kcap * 4 + 127) & ~(size_t)127);
     size_t avail = (size_t)ix->max_smem > fixed ? (size_t)ix->max_smem - fixed : 0;
     if (g_opt_ring_bytes > 0 && (size_t)g_opt_ring_bytes < avail) avail = (size_t)g_opt_ring_bytes;
     const size_t wtile = (size_t)(32 >> log2P) * pitch;
@@ -336,15 +327,13 @@ int drain(vsb_index *ix) {
 
 // the device buffers of a workspace (its events stay)
 void free_work(Work &w) {
-    for (QWork &q : w.q) {
-        cudaFree(q.d_lists);
-        cudaFree(q.d_logs);
-        cudaFree(q.d_counts);
-        cudaFree(q.d_tlocal);
-        q = QWork();
-    }
+    cudaFree(w.d_lists);
+    cudaFree(w.d_logs);
+    cudaFree(w.d_counts);
+    cudaFree(w.d_tlocal);
     cudaFree(w.d_bounds);
     cudaFree(w.d_cta_time);
+    w.d_lists = nullptr; w.d_tlocal = nullptr; w.d_logs = nullptr; w.d_counts = nullptr;
     w.d_bounds = nullptr; w.d_cta_time = nullptr;
 }
 
@@ -359,12 +348,10 @@ int ensure_workspace(vsb_index *ix, int k) {
     for (int i = 0; i < kWorks; ++i) {
         Work &w = ix->work[i];
         free_work(w);
-        for (QWork &q : w.q) {
-            CU(cudaMalloc((void **)&q.d_lists, sizeof(float) * (size_t)streams * kcap));
-            CU(cudaMalloc((void **)&q.d_logs, sizeof(uint2) * (size_t)streams * logcap));
-            CU(cudaMalloc((void **)&q.d_counts, sizeof(int) * (size_t)streams));
-            CU(cudaMalloc((void **)&q.d_tlocal, sizeof(float) * (size_t)streams));
-        }
+        CU(cudaMalloc((void **)&w.d_lists, sizeof(float) * (size_t)streams * kcap));
+        CU(cudaMalloc((void **)&w.d_logs, sizeof(uint2) * (size_t)streams * logcap));
+        CU(cudaMalloc((void **)&w.d_counts, sizeof(int) * (size_t)streams));
+        CU(cudaMalloc((void **)&w.d_tlocal, sizeof(float) * (size_t)streams));
         w.bounds_tiles = -1;
         w.in_use = false;
         CU(cudaMalloc((void **)&w.d_bounds, sizeof(long long) * (size_t)(ix->num_sms + 1)));
@@ -381,20 +368,20 @@ int merge_blocks_strided(const uint8_t *blocks, int world, size_t stride, const 
 void exchange_free(vsb_index *ix);
 int exchange_fill_push(vsb_index *ix, PushParams *pp);
 
-// launches ONE scan kernel for nq independent queries (device pointers, pitch bytes each) on ix->stream and, when k > 0,
-// one filter launch (grid.y = nq) on ix->fstream.  slots[g] receives query g's result.
-// fetch: copy the slots' heads to pinned host memory afterwards (false when the heads are all-gathered on the device)
-// ss: the scan stream of this launch (next_scan_stream); push: the filter also pushes each head into the exchange targets
+// launches the scan kernel for one query (device pointer, pitch bytes) on ss and, when k > 0, the filter on ix->fstream;
+// slot receives the result.
+// fetch: copy the slot's head to pinned host memory afterwards (false when the heads are all-gathered on the device)
+// ss: the scan stream of this launch (next_scan_stream); push: the head is labelled for the exchange (shard index and
+// exchange sequence number); push_heads_kernel moves it (exchange_push)
 // view_vec / view_n: scan these rows instead of the resident column (the windows of a streamed index)
-int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries, int nq, int k, Slot *const *slots, float *d_dist_all,
-                      bool fetch, cudaStream_t ss, bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1) {
+int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *slot, float *d_dist_all, bool fetch, cudaStream_t ss,
+                bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1) {
     const uint8_t *scan_vec = view_vec ? view_vec : ix->d_vec;
     const long long scan_n = view_vec ? view_n : ix->n;
     if (!scan_vec) return fail(VSB_EINVAL, "this entry point needs a resident (not streamed) index");
     int root = 0;
     const int mc = metric_class(metric, &root);
     if (mc < 0) return fail(VSB_EINVAL, "unknown distance metric %d", metric);
-    if (nq < 1 || nq > kMaxGroup) return fail(VSB_EINVAL, "a launch scans 1..%d queries", kMaxGroup);
     // per-launch list stride: the workspace may have been sized by an earlier, larger k (ensure_workspace never shrinks), but
     // the scan's list layout, the filter's FAST/generic choice and its shared-memory layout all follow THIS query's k
     const int kcap = k > 0 ? ((k + 31) & ~31) : 0;
@@ -438,17 +425,13 @@ int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries
     p.k = k;
     p.kcap = kcap;
     p.logcap = ix->ws_logcap;
-    p.nq = nq;
-    for (int g = 0; g < nq; ++g) {
-        ScanQuery &q = p.q[g];
-        q.query = d_queries[g];
-        q.lists = wk ? wk->q[g].d_lists : nullptr;
-        q.tlocal = wk ? wk->q[g].d_tlocal : nullptr;
-        q.logs = wk ? wk->q[g].d_logs : nullptr;
-        q.counts = wk ? wk->q[g].d_counts : nullptr;
-        q.ctrl = slots ? slots[g]->d_ctrl : nullptr;
-        q.dist_all = d_dist_all;
-    }
+    p.query = d_query;
+    p.lists = wk ? wk->d_lists : nullptr;
+    p.tlocal = wk ? wk->d_tlocal : nullptr;
+    p.logs = wk ? wk->d_logs : nullptr;
+    p.counts = wk ? wk->d_counts : nullptr;
+    p.ctrl = slot ? slot->d_ctrl : nullptr;
+    p.dist_all = d_dist_all;
     p.bounds = balance ? wk->d_bounds : nullptr;
     p.cta_time = balance ? wk->d_cta_time : nullptr;
     cudaEvent_t *pev = nullptr;
@@ -463,7 +446,6 @@ int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries
         pev = &ix->prof_ev[ix->prof_used];
         ix->prof_used += 4;
         ix->prof_kind.push_back(k > 0 ? 2 : 1);
-        ix->prof_nq.push_back(nq);
         CU(cudaEventRecord(pev[0], ss));
     }
     fn<<<ix->num_sms, kThreads, pl.smem, ss>>>(p);
@@ -476,9 +458,10 @@ int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries
         CU(cudaStreamWaitEvent(ix->fstream, wk->scanned, 0));
         FilterParams f{};
         if (push) {
-            const int rc = exchange_fill_push(ix, &f.push);
+            PushParams pp{};
+            const int rc = exchange_fill_push(ix, &pp);
             if (rc) return rc;
-            if (g_opt_push_mode == 1) f.push.ntargets = 0;      // the heads are pushed by push_heads_kernel (exchange_push); src / world still label the header
+            f.src = pp.src;
         }
         f.S = ix->ws_streams;
         f.k = k;
@@ -486,60 +469,43 @@ int launch_scan_group(vsb_index *ix, int metric, const uint8_t *const *d_queries
         f.logcap = ix->ws_logcap;
         f.headcap = kFirstFetch;
         f.outcap = kOutCap;
-        f.nq = nq;
         const bool fast = (kcap == 32) && filter_fast_smem(f.S / kWarps) + 2048 <= (size_t)ix->max_smem;
         const int fw = filter_warps(fast);
         const int nblocks = (f.S + fw - 1) / fw;
         if (nblocks > kTableCap) return fail(VSB_ERANGE, "too many filter blocks (%d)", nblocks);
-        for (int g = 0; g < nq; ++g) {
-            FilterQuery &q = f.q[g];
-            Slot *slot = slots[g];
-            q.lists = wk->q[g].d_lists;
-            q.tlocal = wk->q[g].d_tlocal;
-            q.logs = wk->q[g].d_logs;
-            q.counts = wk->q[g].d_counts;
-            q.out = head_survivors(slot->d_head);
-            q.out_tail = slot->d_tail;
-            q.table = head_table(slot->d_head);
-            q.hdr = slot->d_head;
-            q.ctrl = slot->d_ctrl;
-            q.seqno = ++slot->seq;
-            q.xslot = (int)(slot - ix->slot);
-            q.xseq = push ? exchange_next_seq(ix, q.xslot) : 0u;
-        }
+        f.lists = wk->d_lists;
+        f.tlocal = wk->d_tlocal;
+        f.logs = wk->d_logs;
+        f.counts = wk->d_counts;
+        f.out = head_survivors(slot->d_head);
+        f.out_tail = slot->d_tail;
+        f.table = head_table(slot->d_head);
+        f.hdr = slot->d_head;
+        f.ctrl = slot->d_ctrl;
+        f.seqno = ++slot->seq;
+        f.xseq = push ? exchange_next_seq(ix, (int)(slot - ix->slot)) : 0u;
         f.bounds = balance ? wk->d_bounds : nullptr;
         f.cta_time = wk->d_cta_time;
         f.total_tiles = total_tiles;
         if (pev) CU(cudaEventRecord(pev[2], ix->fstream));
-        const dim3 grid((unsigned)nblocks, (unsigned)nq);
         if (fast) {
             const size_t fsm = filter_fast_smem(f.S / kWarps);
             CU((cudaError_t)set_smem_limit((const void *)filter_kernel<true>, fsm));
-            filter_kernel<true><<<grid, fw * 32, fsm, ix->fstream>>>(f);
+            filter_kernel<true><<<nblocks, fw * 32, fsm, ix->fstream>>>(f);
         } else {
             const size_t fsm = sizeof(float) * ((size_t)2 * kFilterWarps * kcap + (size_t)f.S + 32);
             CU((cudaError_t)set_smem_limit((const void *)filter_kernel<false>, fsm));
-            filter_kernel<false><<<grid, fw * 32, fsm, ix->fstream>>>(f);
+            filter_kernel<false><<<nblocks, fw * 32, fsm, ix->fstream>>>(f);
         }
         CU(cudaGetLastError());
         ++g_launches;
         if (pev) CU(cudaEventRecord(pev[3], ix->fstream));
         CU(cudaEventRecord(wk->drained, ix->fstream));
         wk->in_use = true;
-        if (fetch) {   // the heads of consecutive slots are contiguous: one copy when the group's slots are
-            bool contiguous = true;
-            for (int g = 1; g < nq; ++g) contiguous = contiguous && slots[g] == slots[g - 1] + 1;
-            if (contiguous) CU(cudaMemcpyAsync(slots[0]->h_head, slots[0]->d_head, kHeadBytes * (size_t)nq, cudaMemcpyDeviceToHost, ix->fstream));
-            else
-                for (int g = 0; g < nq; ++g) CU(cudaMemcpyAsync(slots[g]->h_head, slots[g]->d_head, kHeadBytes, cudaMemcpyDeviceToHost, ix->fstream));
-        }
-        for (int g = 0; g < nq; ++g) CU(cudaEventRecord(slots[g]->done, ix->fstream));
+        if (fetch) CU(cudaMemcpyAsync(slot->h_head, slot->d_head, kHeadBytes, cudaMemcpyDeviceToHost, ix->fstream));
+        CU(cudaEventRecord(slot->done, ix->fstream));
     }
     return VSB_OK;
-}
-
-int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *slot, float *d_dist_all, bool fetch, cudaStream_t ss) {
-    return launch_scan_group(ix, metric, &d_query, 1, k, slot ? &slot : nullptr, d_dist_all, fetch, ss);
 }
 
 // single-query scans alternate between two streams (option scan_streams, see g_opt_scan_streams)
@@ -734,7 +700,7 @@ int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *
     }
     return stream_windows(ix, 2,
         [&](long long, const uint8_t *vec, long long rows, int s) {
-            return launch_scan_group(ix, metric, &d_query, 1, 0, nullptr, ix->d_dist_all + (size_t)s * ix->win_rows, false, ix->stream, false, vec, rows);
+            return launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all + (size_t)s * ix->win_rows, false, ix->stream, false, vec, rows);
         },
         [&](long long, long long r0, long long rows, int s) {
             // distances of window w sit in half s of d_dist_all; the copy is ordered behind that window's scan on the same stream
@@ -750,8 +716,7 @@ int streamed_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k
     const int depth = 4;                                  // result slots 0..3 rotate over the windows
     return stream_windows(ix, depth,
         [&](long long, const uint8_t *vec, long long rows, int s) {
-            Slot *slot = &ix->slot[s];
-            return launch_scan_group(ix, metric, &d_query, 1, k, &slot, nullptr, true, ix->stream, false, vec, rows);
+            return launch_scan(ix, metric, d_query, k, &ix->slot[s], nullptr, true, ix->stream, false, vec, rows);
         },
         [&](long long, long long r0, long long, int s) {
             bool ovf = false;
@@ -815,8 +780,8 @@ int check_index(const vsb_index *ix) {
     return VSB_OK;
 }
 
-// scan + filter launches for a group of independent queries (query j at queries + j * query_stride; slots first_slot ..).
-// push: the heads also travel to the exchange targets (peer memory), see exchange.inc
+// one scan + filter launch per query of a group of independent queries (query j at queries + j * query_stride; slots
+// first_slot ..).  push: the heads are labelled for the exchange targets (peer memory), see exchange.inc
 int submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device, int k, int fetch,
                  int first_slot, bool push) {
     if (check_index(ix)) return VSB_EINVAL;
@@ -827,28 +792,19 @@ int submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_s
     if (rc) return rc;
     rc = ensure_workspace(ix, k);
     if (rc) return rc;
-    const bool fuse = (double)ix->n * ix->pitch < (double)g_opt_fuse_mb * 1048576.0;
-    const int per_launch = fuse ? kMaxGroup : 1;          // small shards: one scan launch per kMaxGroup queries
-    for (int g0 = 0; g0 < nq; g0 += per_launch) {
-        const int m = std::min(per_launch, nq - g0);
-        const uint8_t *dq[kMaxGroup];
-        Slot *sl[kMaxGroup];
+    for (int j = 0; j < nq; ++j) {
+        Slot *slot = &ix->slot[first_slot + j];
+        const uint8_t *q = (const uint8_t *)queries + (size_t)j * (size_t)query_stride;
         cudaStream_t ss = next_scan_stream(ix);
-        for (int j = 0; j < m; ++j) {
-            Slot *slot = &ix->slot[first_slot + g0 + j];
-            const uint8_t *q = (const uint8_t *)queries + (size_t)(g0 + j) * (size_t)query_stride;
-            if (!query_on_device) {
-                if (slot->seq > 0) CU(cudaEventSynchronize(slot->done));   // the slot's pinned staging buffer is free again
-                rc = stage_query(ix, slot, q, ss);
-                if (rc) return rc;
-                q = slot->d_query;
-            }
-            dq[j] = q;
-            sl[j] = slot;
+        if (!query_on_device) {
+            if (slot->seq > 0) CU(cudaEventSynchronize(slot->done));   // the slot's pinned staging buffer is free again
+            rc = stage_query(ix, slot, q, ss);
+            if (rc) return rc;
+            q = slot->d_query;
         }
-        rc = launch_scan_group(ix, metric, dq, m, k, sl, nullptr, fetch != 0, ss, push);
+        rc = launch_scan(ix, metric, q, k, slot, nullptr, fetch != 0, ss, push);
         if (rc) return rc;
-        ix->last_slot = first_slot + g0 + m - 1;
+        ix->last_slot = first_slot + j;
         ix->last_metric = metric;
     }
     return VSB_OK;
@@ -895,14 +851,11 @@ int vsb_set_option(const char *name, int value) {
     else if (!strcmp(name, "no_batch")) p = &g_opt_no_batch;
     else if (!strcmp(name, "epi_chunk")) p = &g_opt_epi_chunk;
     else if (!strcmp(name, "balance")) p = &g_opt_balance;
-    else if (!strcmp(name, "fuse_mb")) p = &g_opt_fuse_mb;
     else if (!strcmp(name, "batch_m0")) p = &g_opt_batch_m0;
     else if (!strcmp(name, "batch_growth")) p = &g_opt_batch_growth;
-    else if (!strcmp(name, "merge_stream")) p = &g_opt_merge_stream;
     else if (!strcmp(name, "batch_debug")) p = &g_opt_batch_debug;
     else if (!strcmp(name, "scan_streams")) p = &g_opt_scan_streams;
     else if (!strcmp(name, "xwait_ms")) p = &g_opt_xwait_ms;
-    else if (!strcmp(name, "push_mode")) p = &g_opt_push_mode;
     else if (!strcmp(name, "f32_batch")) p = &g_opt_f32_batch;
     if (!p) return fail(VSB_EINVAL, "unknown option %s", name);
     if (value < 0) return fail(VSB_EINVAL, "option %s: values are non-negative", name);   // so that a negative return is always an error
@@ -1330,14 +1283,13 @@ int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double 
     for (size_t i = 0; i < ix->prof_kind.size(); ++i) {
         float ms = 0;
         CU(cudaEventElapsedTime(&ms, ix->prof_ev[4 * i], ix->prof_ev[4 * i + 1]));
-        a += ms; na += ix->prof_nq[i];          // a launch that scans G queries counts as G scans
+        a += ms; ++na;
         if (ix->prof_kind[i] == 2) {
             CU(cudaEventElapsedTime(&ms, ix->prof_ev[4 * i + 2], ix->prof_ev[4 * i + 3]));
-            b += ms; nb += ix->prof_nq[i];
+            b += ms; ++nb;
         }
     }
     ix->prof_kind.clear();
-    ix->prof_nq.clear();
     ix->prof_used = 0;
     if (scan_ms) *scan_ms = a;
     if (scan_launches) *scan_launches = na;
@@ -1348,29 +1300,10 @@ int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double 
 
 int vsb_scan_submit(vsb_index *ix, int metric, const void *query, int query_on_device, int k, int fetch, int want_slot) {
     if (check_index(ix)) return VSB_EINVAL;
-    if (!query || k <= 0 || k > kMaxK) return fail(VSB_EINVAL, "bad scan arguments (k must be 1..%d)", kMaxK);
-    CU(cudaSetDevice(ix->device));
-    int rc = ensure_slots(ix);
-    if (rc) return rc;
-    rc = ensure_workspace(ix, k);
-    if (rc) return rc;
     if (want_slot >= kSlots) return fail(VSB_EINVAL, "slot %d out of range (have %d)", want_slot, kSlots);
     const int si = want_slot >= 0 ? want_slot : (ix->last_slot + 1) % kSlots;
-    Slot *slot = &ix->slot[si];
-    const uint8_t *dq = (const uint8_t *)query;
-    cudaStream_t ss = next_scan_stream(ix);
-    if (!query_on_device) {
-        // the slot's pinned staging buffer is free once the slot's previous query has completed on the device
-        if (slot->seq > 0) CU(cudaEventSynchronize(slot->done));
-        rc = stage_query(ix, slot, query, ss);
-        if (rc) return rc;
-        dq = slot->d_query;
-    }
-    rc = launch_scan(ix, metric, dq, k, slot, nullptr, fetch != 0, ss);
-    if (rc) return rc;
-    ix->last_slot = si;
-    ix->last_metric = metric;
-    return si;   // slot id (>= 0) for vsb_collect / vsb_result_block
+    const int rc = submit_group(ix, metric, query, 0, 1, query_on_device, k, fetch, si, false);
+    return rc ? rc : si;   // slot id (>= 0) for vsb_collect / vsb_result_block
 }
 
 int vsb_scan_submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device, int k,

@@ -33,18 +33,7 @@ constexpr int kBarrierBytes = 1024;   // reserved at the start of dynamic smem f
 enum { T_F32 = 1, T_F16 = 2, T_BF16 = 3, T_U8 = 4, T_I8 = 5 };
 enum { MC_L2 = 0, MC_COS = 1, MC_DOT = 2, MC_L1 = 3 };  // L2 and SQUARED_L2 share a kernel (root flag)
 
-constexpr int kMaxGroup = 8;          // independent queries one launch can scan back to back
-
-struct ScanQuery {        // per-query pointers of a launch
-    const uint8_t *query; // device, pitch bytes, zero padded
-    float *lists;         // k <= 32: [CTAs][32] the k smallest distances of each CTA's rows, sorted ascending, +INF padded;
-                          // k > 32:  [streams][kcap] k smallest distances of each stream (unsorted)
-    float *tlocal;        // k <= 32: [streams] k-th smallest distance over the EARLIER streams of the same CTA (+INF if < k rows)
-    uint2 *logs;          // [streams][logcap] (dist bits, local row)
-    int *counts;          // [streams] log entries written (may exceed logcap => overflow)
-    int *ctrl;            // ctrl[1] = overflow flag
-    float *dist_all;      // optional [n]
-};
+constexpr int kMaxGroup = 8;          // queries of one exchange group (vsb_exchange_submit): heads waited for and pushed together
 
 struct ScanParams {
     const uint8_t *vec;   // [n][pitch]
@@ -58,8 +47,14 @@ struct ScanParams {
     int k;                // 0 => no top-k (dist_all only)
     int kcap;             // k rounded up to 32
     int logcap;
-    int nq;               // queries scanned by this launch (1..kMaxGroup)
-    ScanQuery q[kMaxGroup];
+    const uint8_t *query; // device, pitch bytes, zero padded
+    float *lists;         // k <= 32: [CTAs][32] the k smallest distances of each CTA's rows, sorted ascending, +INF padded;
+                          // k > 32:  [streams][kcap] k smallest distances of each stream (unsorted)
+    float *tlocal;        // k <= 32: [streams] k-th smallest distance over the EARLIER streams of the same CTA (+INF if < k rows)
+    uint2 *logs;          // [streams][logcap] (dist bits, local row)
+    int *counts;          // [streams] log entries written (may exceed logcap => overflow)
+    int *ctrl;            // ctrl[1] = overflow flag
+    float *dist_all;      // optional [n]
     // adaptive row partition (optional): bounds[c] .. bounds[c+1] are the warp-tiles of CTA c (contiguous, ascending, any
     // sizes: the exactness argument only needs streams to be contiguous row ranges in scan order).  Each CTA reports the
     // cycles it took; filter_kernel turns speeds into the partition of the query after next (SMs do not all pull from
@@ -428,35 +423,30 @@ struct SortedList {
 };
 
 // ------------------------------------------------------------------ the scan kernel
-// One launch scans the shard for prm.nq independent queries back to back (nq = 1: the plain single-query call; nq > 1: a
-// group submitted together by the sharded launcher).  Every CTA keeps its row range and simply starts the next query when
-// its 8 streams are done: no kernel boundary, no launch gap, and the TMA ring runs across the query boundary (the first
-// tiles of query g+1 are already in flight while the last tiles of query g are consumed).  Each query still has its own
-// k-lists, logs, counters and control words: results are exactly those of nq separate launches.
+// One launch scans the shard for one query.
 template <int VT, int MC, bool DIRECT>
 __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem);                    // [kWarps][kMaxStages]
-    uint8_t *qs = smem + kBarrierBytes;                                      // [2][pitch] query of the current / next scan
-    const int list_bytes = kWarps * prm.kcap * 4;
-    float *lists_s = reinterpret_cast<float *>(qs + 2 * prm.pitch);          // [2][kWarps][kcap]
-    uint8_t *ring = qs + ((2 * prm.pitch + 2 * list_bytes + 127) & ~127);    // [kWarps][nsw][wtile_bytes]
+    uint8_t *qs = smem + kBarrierBytes;                                      // [pitch] the query
+    float *lists_s = reinterpret_cast<float *>(qs + prm.pitch);              // [kWarps][kcap]
+    uint8_t *ring = qs + ((prm.pitch + kWarps * prm.kcap * 4 + 127) & ~127); // [kWarps][nsw][wtile_bytes]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int P = 1 << prm.log2P, rpw = 32 >> prm.log2P;
     const int nsw = prm.nsw;
     const long long clk0 = clock64();
 
-    // ---- prologue: barriers, first query
+    // ---- prologue: barriers, query
     if (tid == 0) {
         for (int i = 0; i < kWarps * kMaxStages; ++i) mbar_init(&bars[i], 1);
         fence_barrier_init();
     }
     for (int i = tid; i < prm.nc; i += kThreads)
-        reinterpret_cast<uint4 *>(qs)[i] = reinterpret_cast<const uint4 *>(prm.q[0].query)[i];
+        reinterpret_cast<uint4 *>(qs)[i] = reinterpret_cast<const uint4 *>(prm.query)[i];
     __syncthreads();
 
-    // ---- this warp's stream: a contiguous range of warp-tiles (rpw rows each), the same for every query of the launch
+    // ---- this warp's stream: a contiguous range of warp-tiles (rpw rows each)
     const long long sidx = (long long)blockIdx.x * kWarps + warp;
     const long long T = (prm.n + rpw - 1) / rpw;
     long long c0, c1;                                                        // this CTA's warp-tiles
@@ -469,25 +459,20 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
     uint8_t *myring = ring + (size_t)warp * nsw * prm.wtile_bytes;
     const uint64_t pol = policy_evict_first();
 
-    // The warp consumes nq * ntiles tiles in all (its stream once per query); the ring simply keeps running across query
-    // boundaries: the tile fetched into the stage just freed is always the one nsw positions ahead, which near the end of
-    // a query is one of the first tiles of the next query.
-    const unsigned total = (unsigned)prm.nq * (unsigned)ntiles;             // tiles this warp consumes in this launch
-    unsigned fetched = 0;                                                    // tiles issued so far (lane 0)
-    int pf_it = 0;                                                           // stream tile index of the next fetch
-    auto issue = [&](int s) {  // lane 0 only: next tile of the sequence into stage s
+    // the tile fetched into the stage just freed is always the one nsw positions ahead
+    int pf_it = 0;                                                           // stream tile index of the next fetch (lane 0)
+    auto issue = [&](int s) {  // lane 0 only: next tile of the stream into stage s
         const long long row0 = (t0 + pf_it) * rpw;
         long long rows = prm.n - row0;
         if (rows > rpw) rows = rpw;
         const uint32_t bytes = (uint32_t)rows * (uint32_t)prm.pitch;
         mbar_expect_tx(&mybars[s], bytes);
         bulk_g2s(myring + (size_t)s * prm.wtile_bytes, prm.vec + (size_t)row0 * prm.pitch, bytes, &mybars[s], pol);
-        ++fetched;
-        if (++pf_it == ntiles) pf_it = 0;
+        ++pf_it;
     };
     if constexpr (!DIRECT) {
         if (lane == 0)
-            for (int s = 0; s < nsw && fetched < total; ++s) issue(s);
+            for (int s = 0; s < nsw && pf_it < ntiles; ++s) issue(s);
     }
     int stage = 0;                                                           // ring position of the next tile to consume
     uint32_t parity = 0;
@@ -500,153 +485,142 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
     const uint8_t *fix_row = nullptr;
     int fix_stage = 0;
 
-    for (int g = 0; g < prm.nq; ++g) {
-        const ScanQuery &Q = prm.q[g];
-        const uint8_t *qbuf = qs + (size_t)(g & 1) * prm.pitch;
-        float *mylist = lists_s + ((size_t)(g & 1) * kWarps + warp) * prm.kcap;
+    float *mylist = lists_s + (size_t)warp * prm.kcap;
 
-        // query norm (every warp computes it the same way: lane-strided chunks, butterfly sum)
-        QueryNorm qn;
-        {
-            float f = 0.0f;
-            int iq = 0;
-            for (int c = lane; c < prm.nc; c += 32) {
-                const uint4 q = reinterpret_cast<const uint4 *>(qbuf)[c];
-                if constexpr (VT == T_U8) {
-                    iq = (int)__dp4a(q.x, q.x, (uint32_t)iq); iq = (int)__dp4a(q.y, q.y, (uint32_t)iq);
-                    iq = (int)__dp4a(q.z, q.z, (uint32_t)iq); iq = (int)__dp4a(q.w, q.w, (uint32_t)iq);
-                } else if constexpr (VT == T_I8) {
-                    iq = __dp4a((int)q.x, (int)q.x, iq); iq = __dp4a((int)q.y, (int)q.y, iq);
-                    iq = __dp4a((int)q.z, (int)q.z, iq); iq = __dp4a((int)q.w, (int)q.w, iq);
-                } else {
-                    float x[8];
-                    unpack8<VT>(q, x);
-                    constexpr int NE = (VT == T_F32) ? 4 : 8;
+    // query norm (every warp computes it the same way: lane-strided chunks, butterfly sum)
+    QueryNorm qn;
+    {
+        float f = 0.0f;
+        int iq = 0;
+        for (int c = lane; c < prm.nc; c += 32) {
+            const uint4 q = reinterpret_cast<const uint4 *>(qs)[c];
+            if constexpr (VT == T_U8) {
+                iq = (int)__dp4a(q.x, q.x, (uint32_t)iq); iq = (int)__dp4a(q.y, q.y, (uint32_t)iq);
+                iq = (int)__dp4a(q.z, q.z, (uint32_t)iq); iq = (int)__dp4a(q.w, q.w, (uint32_t)iq);
+            } else if constexpr (VT == T_I8) {
+                iq = __dp4a((int)q.x, (int)q.x, iq); iq = __dp4a((int)q.y, (int)q.y, iq);
+                iq = __dp4a((int)q.z, (int)q.z, iq); iq = __dp4a((int)q.w, (int)q.w, iq);
+            } else {
+                float x[8];
+                unpack8<VT>(q, x);
+                constexpr int NE = (VT == T_F32) ? 4 : 8;
 #pragma unroll
-                    for (int j = 0; j < NE; ++j) f = fmaf(x[j], x[j], f);
-                }
-            }
-            for (int off = 16; off >= 1; off >>= 1) {
-                f += __shfl_xor_sync(0xFFFFFFFFu, f, off);
-                iq += __shfl_xor_sync(0xFFFFFFFFu, iq, off);
-            }
-            qn.f = f; qn.i = iq;
-        }
-        for (int j = lane; j < prm.kcap; j += 32) mylist[j] = (j < prm.k) ? INFINITY : -INFINITY;
-        __syncwarp();
-
-        float thr = INFINITY;
-        int pos = 0, logged = 0;
-        uint2 *mylog = Q.logs + (size_t)sidx * prm.logcap;
-
-        for (int it = 0; it < ntiles; ++it) {
-            const long long row0 = (t0 + it) * rpw;
-            const bool valid = (row0 + r) < prm.n;
-            Accum A = {0.f, 0.f, 0.f, 0, 0};
-            if constexpr (!DIRECT) {
-                const int s = stage;
-                mbar_wait(&mybars[s], parity);
-                if (++stage == nsw) { stage = 0; parity ^= 1u; }
-                const uint8_t *rowp = myring + (size_t)s * prm.wtile_bytes + (size_t)r * prm.pitch;
-                if (valid) {
-#pragma unroll 4
-                    for (int i = 0; i < cnt; ++i) {
-                        int ii = i0 + i;
-                        if (ii >= cnt) ii -= cnt;
-                        const int c = p + (ii << prm.log2P);
-                        const uint4 rv = *reinterpret_cast<const uint4 *>(rowp + (size_t)c * 16);
-                        const uint4 qv = *reinterpret_cast<const uint4 *>(qbuf + (size_t)c * 16);
-                        accum16<VT, MC>(A, rv, qv);
-                    }
-                }
-                __syncwarp();
-                if constexpr (!kFix16) {
-                    if (lane == 0 && fetched < total) issue(s);               // may already belong to the next query
-                } else {
-                    fix_row = rowp;                                           // the stage stays valid until the fix-up below has run
-                    fix_stage = s;
-                }
-            } else {
-                const uint8_t *rowp = prm.vec + (size_t)(row0 + r) * prm.pitch;
-                if (valid) {
-#pragma unroll 4
-                    for (int i = 0; i < cnt; ++i) {
-                        const int c = p + (i << prm.log2P);
-                        const uint4 rv = ldg_stream(reinterpret_cast<const uint4 *>(rowp) + c);
-                        const uint4 qv = *reinterpret_cast<const uint4 *>(qbuf + (size_t)c * 16);
-                        accum16<VT, MC>(A, rv, qv);
-                    }
-                }
-            }
-            accum_reduce(A, P);
-            float d = finalize<VT, MC>(A, qn, prm.root);
-            if constexpr (kFix16) {
-                if (valid && p == 0 && row_needs_exact<VT, MC>(A, qn)) {
-                    if constexpr (DIRECT) fix_row = prm.vec + (size_t)(row0 + r) * prm.pitch;
-                    d = special_row_distance<VT, MC>(fix_row, qbuf, prm.pitch / 2, prm.root);
-                }
-                if constexpr (!DIRECT) {
-                    __syncwarp();
-                    if (lane == 0 && fetched < total) issue(fix_stage);
-                }
-            }
-            if (Q.dist_all != nullptr && valid && p == 0) Q.dist_all[row0 + r] = d;
-            if (topk) {
-                // rows are visited in scan order (lane order); strict '<' like the reference (:2102, :2145)
-                unsigned m = __ballot_sync(0xFFFFFFFFu, valid && p == 0 && d < thr);
-                while (m) {
-                    const int src = __ffs(m) - 1;
-                    m &= m - 1;
-                    const float dv = __shfl_sync(0xFFFFFFFFu, d, src);
-                    if (dv < thr) {
-                        if (lane == 0) {
-                            if (logged < prm.logcap) mylog[logged] = make_uint2(__float_as_uint(dv), (uint32_t)(row0 + (src >> prm.log2P)));
-                            mylist[pos] = dv;
-                        }
-                        ++logged;
-                        __syncwarp();
-                        list_argmax(mylist, prm.kcap, lane, thr, pos);
-                    }
-                }
+                for (int j = 0; j < NE; ++j) f = fmaf(x[j], x[j], f);
             }
         }
-        if (topk) {
+        for (int off = 16; off >= 1; off >>= 1) {
+            f += __shfl_xor_sync(0xFFFFFFFFu, f, off);
+            iq += __shfl_xor_sync(0xFFFFFFFFu, iq, off);
+        }
+        qn.f = f; qn.i = iq;
+    }
+    for (int j = lane; j < prm.kcap; j += 32) mylist[j] = (j < prm.k) ? INFINITY : -INFINITY;
+    __syncwarp();
+
+    float thr = INFINITY;
+    int pos = 0, logged = 0;
+    uint2 *mylog = prm.logs + (size_t)sidx * prm.logcap;
+
+    for (int it = 0; it < ntiles; ++it) {
+        const long long row0 = (t0 + it) * rpw;
+        const bool valid = (row0 + r) < prm.n;
+        Accum A = {0.f, 0.f, 0.f, 0, 0};
+        if constexpr (!DIRECT) {
+            const int s = stage;
+            mbar_wait(&mybars[s], parity);
+            if (++stage == nsw) { stage = 0; parity ^= 1u; }
+            const uint8_t *rowp = myring + (size_t)s * prm.wtile_bytes + (size_t)r * prm.pitch;
+            if (valid) {
+#pragma unroll 4
+                for (int i = 0; i < cnt; ++i) {
+                    int ii = i0 + i;
+                    if (ii >= cnt) ii -= cnt;
+                    const int c = p + (ii << prm.log2P);
+                    const uint4 rv = *reinterpret_cast<const uint4 *>(rowp + (size_t)c * 16);
+                    const uint4 qv = *reinterpret_cast<const uint4 *>(qs + (size_t)c * 16);
+                    accum16<VT, MC>(A, rv, qv);
+                }
+            }
             __syncwarp();
-            if (lane == 0) {
-                Q.counts[sidx] = logged;
-                if (logged > prm.logcap) atomicExch(&Q.ctrl[1], 1);
-            }
-            if (prm.kcap == 32) {
-                // k <= 32: the CTA's 8 streams are consecutive in scan order.  Sort each stream's list, then one warp merges
-                // them in stream order, recording the running k-th value BEFORE each stream (its in-CTA prefix bound), and
-                // publishes ONE sorted list per CTA: filter_kernel then walks one list per CTA instead of one per stream.
-                float v = (lane < prm.k) ? mylist[lane] : INFINITY;
-                v = warp_sort_asc(v, lane);
-                mylist[lane] = v;
+            if constexpr (!kFix16) {
+                if (lane == 0 && pf_it < ntiles) issue(s);
             } else {
-                float *gl = Q.lists + (size_t)sidx * prm.kcap;
-                for (int j = lane; j < prm.kcap; j += 32) gl[j] = mylist[j];
+                fix_row = rowp;                                           // the stage stays valid until the fix-up below has run
+                fix_stage = s;
+            }
+        } else {
+            const uint8_t *rowp = prm.vec + (size_t)(row0 + r) * prm.pitch;
+            if (valid) {
+#pragma unroll 4
+                for (int i = 0; i < cnt; ++i) {
+                    const int c = p + (i << prm.log2P);
+                    const uint4 rv = ldg_stream(reinterpret_cast<const uint4 *>(rowp) + c);
+                    const uint4 qv = *reinterpret_cast<const uint4 *>(qs + (size_t)c * 16);
+                    accum16<VT, MC>(A, rv, qv);
+                }
             }
         }
-        if (g + 1 < prm.nq) {
-            // stage the next query into the other buffer: nobody reads that one any more (all warps left query g-1 at its barrier)
-            uint4 *dst = reinterpret_cast<uint4 *>(qs + (size_t)((g + 1) & 1) * prm.pitch);
-            const uint4 *src = reinterpret_cast<const uint4 *>(prm.q[g + 1].query);
-            for (int i = tid; i < prm.nc; i += kThreads) dst[i] = src[i];
-        }
-        if (g + 1 < prm.nq || (topk && prm.kcap == 32)) __syncthreads();     // query g is complete in this CTA; next query staged
-        if (g + 1 == prm.nq && tid == 0 && prm.cta_time != nullptr)
-            prm.cta_time[blockIdx.x] = (unsigned)min((long long)0xFFFFFFFFll, (clock64() - clk0) >> 6);   // units of 64 cycles
-        if (topk && prm.kcap == 32 && warp == 0) {
-            const float *ls = lists_s + (size_t)(g & 1) * kWarps * prm.kcap;
-            SortedList Lm;
-            Lm.init(lane, prm.k);
-            for (int w = 0; w < kWarps; ++w) {
-                if (lane == 0) Q.tlocal[(size_t)blockIdx.x * kWarps + w] = Lm.thr;
-                Lm.offer_sorted(lane, ls[w * 32 + lane]);
+        accum_reduce(A, P);
+        float d = finalize<VT, MC>(A, qn, prm.root);
+        if constexpr (kFix16) {
+            if (valid && p == 0 && row_needs_exact<VT, MC>(A, qn)) {
+                if constexpr (DIRECT) fix_row = prm.vec + (size_t)(row0 + r) * prm.pitch;
+                d = special_row_distance<VT, MC>(fix_row, qs, prm.pitch / 2, prm.root);
             }
-            Q.lists[(size_t)blockIdx.x * 32 + lane] = Lm.v;
+            if constexpr (!DIRECT) {
+                __syncwarp();
+                if (lane == 0 && pf_it < ntiles) issue(fix_stage);
+            }
         }
+        if (prm.dist_all != nullptr && valid && p == 0) prm.dist_all[row0 + r] = d;
+        if (topk) {
+            // rows are visited in scan order (lane order); strict '<' like the reference (:2102, :2145)
+            unsigned m = __ballot_sync(0xFFFFFFFFu, valid && p == 0 && d < thr);
+            while (m) {
+                const int src = __ffs(m) - 1;
+                m &= m - 1;
+                const float dv = __shfl_sync(0xFFFFFFFFu, d, src);
+                if (dv < thr) {
+                    if (lane == 0) {
+                        if (logged < prm.logcap) mylog[logged] = make_uint2(__float_as_uint(dv), (uint32_t)(row0 + (src >> prm.log2P)));
+                        mylist[pos] = dv;
+                    }
+                    ++logged;
+                    __syncwarp();
+                    list_argmax(mylist, prm.kcap, lane, thr, pos);
+                }
+            }
+        }
+    }
+    if (topk) {
+        __syncwarp();
+        if (lane == 0) {
+            prm.counts[sidx] = logged;
+            if (logged > prm.logcap) atomicExch(&prm.ctrl[1], 1);
+        }
+        if (prm.kcap == 32) {
+            // k <= 32: the CTA's 8 streams are consecutive in scan order.  Sort each stream's list, then one warp merges
+            // them in stream order, recording the running k-th value BEFORE each stream (its in-CTA prefix bound), and
+            // publishes ONE sorted list per CTA: filter_kernel then walks one list per CTA instead of one per stream.
+            float v = (lane < prm.k) ? mylist[lane] : INFINITY;
+            v = warp_sort_asc(v, lane);
+            mylist[lane] = v;
+        } else {
+            float *gl = prm.lists + (size_t)sidx * prm.kcap;
+            for (int j = lane; j < prm.kcap; j += 32) gl[j] = mylist[j];
+        }
+    }
+    if (topk && prm.kcap == 32) __syncthreads();                             // every stream's sorted list is in lists_s
+    if (tid == 0 && prm.cta_time != nullptr)
+        prm.cta_time[blockIdx.x] = (unsigned)min((long long)0xFFFFFFFFll, (clock64() - clk0) >> 6);   // units of 64 cycles
+    if (topk && prm.kcap == 32 && warp == 0) {
+        SortedList Lm;
+        Lm.init(lane, prm.k);
+        for (int w = 0; w < kWarps; ++w) {
+            if (lane == 0) prm.tlocal[(size_t)blockIdx.x * kWarps + w] = Lm.thr;
+            Lm.offer_sorted(lane, lists_s[w * 32 + lane]);
+        }
+        prm.lists[(size_t)blockIdx.x * 32 + lane] = Lm.v;
     }
 }
 
@@ -674,7 +648,7 @@ struct ResultHead {
     int headcap;        // survivors stored in the head itself
     int pad[9];
 };
-static_assert(sizeof(ResultHead) == 64, "the header is 8 uint2 words (push_one_head)");
+static_assert(sizeof(ResultHead) == 64, "the header is 8 uint2 words (push_heads_kernel)");
 static_assert(offsetof(ResultHead, total) == 0 && offsetof(ResultHead, flags) == 4 && offsetof(ResultHead, seq) == 8 &&
                   offsetof(ResultHead, nblocks) == 12 && offsetof(ResultHead, xseq) == 16 && offsetof(ResultHead, src) == 20 &&
                   offsetof(ResultHead, headcap) == 24,
@@ -686,26 +660,10 @@ inline const int2 *head_table(const ResultHead *h) { return reinterpret_cast<con
 inline uint2 *head_survivors(ResultHead *h) { return reinterpret_cast<uint2 *>(reinterpret_cast<uint8_t *>(h) + kResHdrBytes); }
 inline const uint2 *head_survivors(const ResultHead *h) { return reinterpret_cast<const uint2 *>(reinterpret_cast<const uint8_t *>(h) + kResHdrBytes); }
 
-struct FilterQuery {    // per-query pointers of a (group) launch: blockIdx.y selects the query
-    const float *lists; // k <= 32: [S / kWarps][32] sorted CTA lists; else [S][kcap] stream lists
-    const float *tlocal;// k <= 32: [S] in-CTA prefix bound of each stream (from scan_kernel)
-    const uint2 *logs;  // [S][logcap]
-    const int *counts;  // [S]
-    uint2 *out;         // survivors (dist bits, local row), grouped by block in stream order: the first headcap of them
-    uint2 *out_tail;    //   go to out (inside the slot's head, the part that travels), the rest to out_tail
-    int2 *table;        // [gridDim.x] (base, count) of each block's survivors in out
-    ResultHead *hdr;
-    int *ctrl;          // device: [0] cursor, [1] overflow from scan_kernel, [2] blocks done
-    int seqno;
-    int xslot;          // push: slot row of the targets' gather buffers
-    unsigned xseq;      // push: exchange sequence number published with the head (ResultHead::xseq) and raised on the flags
-};
-
-// NVLink peer-memory all-gather: push_heads_kernel after a group's filters (default), or the filter block that completes a
-// query's result head (option push_mode = 0), copies the used part of the head (header, block table, survivors) straight into
-// the gather buffer of every target GPU — peer memory mapped through cudaIpc (one process per GPU) or
-// cudaDeviceEnablePeerAccess (one process, several GPUs) — and then raises that target's arrival flag with a system-scope
-// release store.  No NCCL kernel, no host synchronisation: the receiving side waits on the flags with exchange_wait_kernel on
+// NVLink peer-memory all-gather: push_heads_kernel, after a group's filters, copies the used part of each head (header, block
+// table, survivors) straight into the gather buffer of every target GPU — peer memory mapped through cudaIpc (one process per
+// GPU) or cudaDeviceEnablePeerAccess (one process, several GPUs) — and then raises that target's arrival flag with a
+// system-scope release store.  No NCCL kernel, no host synchronisation: the receiving side waits on the flags with exchange_wait_kernel on
 // ITS stream and copies the gathered heads to the host.
 constexpr int kMaxPeers = 16;
 struct PushParams {
@@ -752,36 +710,10 @@ __global__ void exchange_wait_kernel(const WaitParams wp) {
     }
 }
 
-// the push itself: one block stores the used part of one finished head (header, block table, survivors; the survivors beyond
-// headcap from the slot's tail area) into row (xslot, src) of every target and raises the targets' flags.  All threads of the
-// block call it; the caller guarantees that the head is complete and visible (filter_kernel: last block; push_heads_kernel:
-// stream order after the filters).
-__device__ __forceinline__ void push_one_head(const PushParams &pp, const ResultHead *hdr, const uint2 *out, const uint2 *out_tail, int xslot,
-                                              unsigned xseq, int headcap) {
-    const int total = max(__ldcg(&hdr->total), 0), nblocks = __ldcg(&hdr->nblocks);
-    const int nhead = (int)(sizeof(ResultHead) / sizeof(uint2)) + nblocks;   // uint2 words of header + block table
-    const int nsurv = min(total, headcap);
-    const int ntail = min(max(total - headcap, 0), pp.tailcap);
-    const uint2 *src_head = reinterpret_cast<const uint2 *>(hdr);
-    const size_t row = (size_t)xslot * pp.world + pp.src;
-    for (int t = 0; t < pp.ntargets; ++t) {
-        uint8_t *dst = pp.gather[t] + row * kHeadBytes;
-        uint2 *dh = reinterpret_cast<uint2 *>(dst);
-        uint2 *ds = reinterpret_cast<uint2 *>(dst + kResHdrBytes);
-        for (int i = (int)threadIdx.x; i < nhead; i += (int)blockDim.x) dh[i] = __ldcg(src_head + i);
-        for (int i = (int)threadIdx.x; i < nsurv; i += (int)blockDim.x) ds[i] = __ldcg(out + i);
-        if (ntail > 0) {
-            uint2 *dt = pp.tails[t] + row * (size_t)pp.tailcap;
-            for (int i = (int)threadIdx.x; i < ntail; i += (int)blockDim.x) dt[i] = __ldcg(out_tail + i);
-        }
-    }
-    __threadfence_system();
-    __syncthreads();
-    if ((int)threadIdx.x < pp.ntargets) st_release_sys(pp.flags[threadIdx.x] + row, xseq);
-}
-
-// option push_mode = 1: the heads of a finished group are pushed by their own small kernel on the exchange stream instead of by
-// the filter's last block (the filter stream then never waits for NVLink acknowledgements)
+// The heads of a finished group are pushed by their own small kernel on the exchange stream, so the filter stream never waits
+// for NVLink acknowledgements.  Block j stores the used part of query j's head (header, block table, survivors; the survivors
+// beyond headcap from the slot's tail area) into row (xslot, src) of every target and raises the targets' flags.  The heads
+// are complete and visible: the kernel runs in stream order after the filters.
 struct PushGroupParams {
     PushParams push;
     int nq, headcap;
@@ -793,18 +725,49 @@ struct PushGroupParams {
 };
 __global__ void push_heads_kernel(const PushGroupParams gp) {
     const int j = blockIdx.x;
-    if (j < gp.nq) push_one_head(gp.push, gp.hdr[j], gp.out[j], gp.out_tail[j], gp.xslot[j], gp.xseq[j], gp.headcap);
+    if (j >= gp.nq) return;
+    const PushParams &pp = gp.push;
+    const ResultHead *hdr = gp.hdr[j];
+    const int total = max(__ldcg(&hdr->total), 0), nblocks = __ldcg(&hdr->nblocks);
+    const int nhead = (int)(sizeof(ResultHead) / sizeof(uint2)) + nblocks;   // uint2 words of header + block table
+    const int nsurv = min(total, gp.headcap);
+    const int ntail = min(max(total - gp.headcap, 0), pp.tailcap);
+    const uint2 *src_head = reinterpret_cast<const uint2 *>(hdr);
+    const size_t row = (size_t)gp.xslot[j] * pp.world + pp.src;
+    for (int t = 0; t < pp.ntargets; ++t) {
+        uint8_t *dst = pp.gather[t] + row * kHeadBytes;
+        uint2 *dh = reinterpret_cast<uint2 *>(dst);
+        uint2 *ds = reinterpret_cast<uint2 *>(dst + kResHdrBytes);
+        for (int i = (int)threadIdx.x; i < nhead; i += (int)blockDim.x) dh[i] = __ldcg(src_head + i);
+        for (int i = (int)threadIdx.x; i < nsurv; i += (int)blockDim.x) ds[i] = __ldcg(gp.out[j] + i);
+        if (ntail > 0) {
+            uint2 *dt = pp.tails[t] + row * (size_t)pp.tailcap;
+            for (int i = (int)threadIdx.x; i < ntail; i += (int)blockDim.x) dt[i] = __ldcg(gp.out_tail[j] + i);
+        }
+    }
+    __threadfence_system();
+    __syncthreads();
+    if ((int)threadIdx.x < pp.ntargets) st_release_sys(pp.flags[threadIdx.x] + row, gp.xseq[j]);
 }
 
 struct FilterParams {
-    PushParams push;
+    const float *lists; // k <= 32: [S / kWarps][32] sorted CTA lists; else [S][kcap] stream lists
+    const float *tlocal;// k <= 32: [S] in-CTA prefix bound of each stream (from scan_kernel)
+    const uint2 *logs;  // [S][logcap]
+    const int *counts;  // [S]
+    uint2 *out;         // survivors (dist bits, local row), grouped by block in stream order: the first headcap of them
+    uint2 *out_tail;    //   go to out (inside the slot's head, the part that travels), the rest to out_tail
+    int2 *table;        // [gridDim.x] (base, count) of each block's survivors in out
+    ResultHead *hdr;
+    int *ctrl;          // device: [0] cursor, [1] overflow from scan_kernel, [2] blocks done
+    int seqno;
+    int src;            // this shard's index inside a gather row (ResultHead::src)
+    unsigned xseq;      // exchange sequence number published with the head (ResultHead::xseq)
     int S;              // streams
     int k, kcap;
     int logcap;
     int headcap;
     int outcap;         // total capacity (head + tail)
-    int nq;             // queries (gridDim.y)
-    FilterQuery q[kMaxGroup];
     // adaptive partition (k <= 32 path): the last block turns the scan's per-CTA cycles into new tile bounds, in place
     long long *bounds;          // [ncta + 1] or nullptr
     const unsigned *cta_time;   // [ncta]
@@ -829,7 +792,6 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
     constexpr int FW = filter_warps(FAST);
     static_assert(FW >= kSegments, "the segment walks use the first kSegments warps");
     extern __shared__ __align__(16) uint8_t fsm[];
-    const FilterQuery &fq = fp.q[blockIdx.y];
     const int k = fp.k, kcap = fp.kcap;
     const int ncta = fp.S / kWarps;                                         // scan CTAs (FAST: each published one sorted list)
     // generic: [32][kcap] segment lists | [32][kcap] scratch | [S] in-segment prefix bound | [32] segment bounds
@@ -849,8 +811,8 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
     const int s = blockIdx.x * FW + warp;
     int n_log = 0;
     uint2 ereg[kLogRegs];
-    const uint2 *lg = fq.logs + (size_t)s * fp.logcap;
-    if (s < fp.S) n_log = min(fq.counts[s], fp.logcap);
+    const uint2 *lg = fp.logs + (size_t)s * fp.logcap;
+    if (s < fp.S) n_log = min(fp.counts[s], fp.logcap);
 #pragma unroll
     for (int i = 0; i < kLogRegs; ++i) {
         const int j = i * 32 + lane;
@@ -860,7 +822,7 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
     if constexpr (FAST) {
         const int GC = (ncta + kSegments - 1) / kSegments;                  // CTAs per segment
         {   // all CTA lists (ncta x 32 floats, ~19 KB) -> shared memory in one coalesced pass
-            const float4 *src = reinterpret_cast<const float4 *>(fq.lists);
+            const float4 *src = reinterpret_cast<const float4 *>(fp.lists);
             float4 *dst = reinterpret_cast<float4 *>(slists);
             const int tot4 = ncta * 8;
             for (int i = (int)threadIdx.x; i < tot4; i += FW * 32) dst[i] = __ldg(src + i);
@@ -895,7 +857,7 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
             const int s0 = warp * G, s1 = min(fp.S, s0 + G);
             for (int st = s0; st < s1; ++st) {
                 if (lane == 0) tlocal[st] = thr;
-                const float *src = fq.lists + (size_t)st * kcap;
+                const float *src = fp.lists + (size_t)st * kcap;
                 for (int base = 0; base < k; base += 32) {
                     const int j = base + lane;
                     const float v = (j < k) ? src[j] : INFINITY;
@@ -948,7 +910,7 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
     if (s < fp.S) {
         if constexpr (FAST) {
             const int c = s / kWarps, GC = (ncta + kSegments - 1) / kSegments;
-            T = fminf(fminf(__ldg(fq.tlocal + s), tlocal[c]), tseg[c / GC]);
+            T = fminf(fminf(__ldg(fp.tlocal + s), tlocal[c]), tseg[c / GC]);
         } else {
             T = fminf(tlocal[s], tseg[s / G]);
         }
@@ -966,9 +928,9 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
     if (threadIdx.x == 0) {
         int tot = 0;
         for (int w = 0; w < FW; ++w) { woff[w] = tot; tot += wcount[w]; }
-        const int base = atomicAdd(&fq.ctrl[0], tot);
+        const int base = atomicAdd(&fp.ctrl[0], tot);
         blk_base = base;
-        fq.table[blockIdx.x] = make_int2(base, tot);
+        fp.table[blockIdx.x] = make_int2(base, tot);
     }
     __syncthreads();
     int wr = blk_base + woff[warp];
@@ -977,7 +939,7 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
         const bool keep = __uint_as_float(ereg[i].x) < T;
         const unsigned m = __ballot_sync(0xFFFFFFFFu, keep);
         const int off = wr + __popc(m & ((1u << lane) - 1u));
-        if (keep && off < fp.outcap) *(off < fp.headcap ? fq.out + off : fq.out_tail + (off - fp.headcap)) = ereg[i];
+        if (keep && off < fp.outcap) *(off < fp.headcap ? fp.out + off : fp.out_tail + (off - fp.headcap)) = ereg[i];
         wr += __popc(m);
     }
     for (int base = kLogRegs * 32; base < n_log; base += 32) {
@@ -987,12 +949,12 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
         if (j < n_log) { e = lg[j]; keep = __uint_as_float(e.x) < T; }
         const unsigned m = __ballot_sync(0xFFFFFFFFu, keep);
         const int off = wr + __popc(m & ((1u << lane) - 1u));
-        if (keep && off < fp.outcap) *(off < fp.headcap ? fq.out + off : fq.out_tail + (off - fp.headcap)) = e;
+        if (keep && off < fp.outcap) *(off < fp.headcap ? fp.out + off : fp.out_tail + (off - fp.headcap)) = e;
         wr += __popc(m);
     }
     if constexpr (FAST) {
         // ---- adaptive partition: share of CTA c for the query after next  ∝  its measured speed (tiles per cycle), damped
-        if (fp.bounds != nullptr && blockIdx.x == gridDim.x - 1 && blockIdx.y == gridDim.y - 1 && fp.total_tiles >= 64ll * ncta && ncta <= 1024) {
+        if (fp.bounds != nullptr && blockIdx.x == gridDim.x - 1 && fp.total_tiles >= 64ll * ncta && ncta <= 1024) {
             __shared__ float spd[1024];
             __shared__ int bad;
             if (threadIdx.x == 0) bad = 0;
@@ -1026,33 +988,22 @@ __global__ void __launch_bounds__(filter_warps(FAST) * 32, 1) filter_kernel(cons
     }
     // last block publishes the header and re-arms the control words for the next query.  The host only reads the
     // mapped buffers after the stream has drained, so device-scope ordering between blocks is all that is needed.
-    __shared__ int is_last;
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) {
-        const int done = atomicAdd(&fq.ctrl[2], 1);
-        const int last = (done == (int)gridDim.x - 1);
-        if (last) {
+        const int done = atomicAdd(&fp.ctrl[2], 1);
+        if (done == (int)gridDim.x - 1) {
             __threadfence();
-            const int total = atomicAdd(&fq.ctrl[0], 0);
-            const int ovf = atomicAdd(&fq.ctrl[1], 0);
-            fq.hdr->total = total;
-            fq.hdr->flags = (ovf != 0 || total > fp.outcap) ? kHeadOverflow : 0;
-            fq.hdr->seq = fq.seqno;
-            fq.hdr->nblocks = (int)gridDim.x;
-            fq.hdr->xseq = (int)fq.xseq;
-            fq.hdr->src = fp.push.src;
-            fq.hdr->headcap = fp.headcap;
-            fq.ctrl[0] = 0; fq.ctrl[1] = 0; fq.ctrl[2] = 0;
-        }
-        is_last = last;
-    }
-    if (fp.push.ntargets > 0) {                                   // uniform across the grid
-        __syncthreads();
-        if (is_last) {
-            // the other blocks' survivors are visible: each fenced before its ctrl[2] increment, thread 0 fenced after
-            // observing the last one; read them through L2 (ld.cg), store them to peer memory over NVLink
-            push_one_head(fp.push, fq.hdr, fq.out, fq.out_tail, fq.xslot, fq.xseq, fp.headcap);
+            const int total = atomicAdd(&fp.ctrl[0], 0);
+            const int ovf = atomicAdd(&fp.ctrl[1], 0);
+            fp.hdr->total = total;
+            fp.hdr->flags = (ovf != 0 || total > fp.outcap) ? kHeadOverflow : 0;
+            fp.hdr->seq = fp.seqno;
+            fp.hdr->nblocks = (int)gridDim.x;
+            fp.hdr->xseq = (int)fp.xseq;
+            fp.hdr->src = fp.src;
+            fp.hdr->headcap = fp.headcap;
+            fp.ctrl[0] = 0; fp.ctrl[1] = 0; fp.ctrl[2] = 0;
         }
     }
 }

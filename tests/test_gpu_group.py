@@ -42,15 +42,6 @@ def _group(vtype, x, ngpus, rowids=None, chunk=7919):
 
 @pytest.mark.parametrize("ngpus", [2, 3, 8])
 def test_group_int8_bit_exact(oracle, ngpus):
-    import sqlite_vector_b200 as vs
-    old_pm = vs.load_engine().set_option("push_mode", 1 if ngpus == 3 else 0)     # one of the three also through the separate push kernel
-    try:
-        _group_int8_bit_exact(oracle, ngpus)
-    finally:
-        vs.load_engine().set_option("push_mode", old_pm)
-
-
-def _group_int8_bit_exact(oracle, ngpus):
     rng = np.random.Generator(np.random.PCG64(100 + ngpus))
     n, dim = 50_000, 64
     x = rng.integers(-5, 6, (n, dim)).astype(np.int8)        # narrow value range: ties at the k-th place
@@ -210,39 +201,34 @@ qd = torch.zeros((nq, pitch), dtype=torch.uint8, device=device)
 qd[:, :dim] = torch.from_numpy(q.view(np.uint8)).to(device)
 torch.cuda.synchronize()
 exch = shard.PeerExchange(ix, eng, world, rank, bounds, group=8)
-for fuse in (0, 4096):
-    eng.set_option("fuse_mb", fuse)
-    for on_device in (True, False):
-        for metric in (api.L2, api.DOT):
-            results, pending = [], []
-            for g0 in range(0, nq, exch.group):
-                m = min(exch.group, nq - g0)
-                t = exch.submit_strided(metric, qd[g0].data_ptr(), pitch, m, k, True) if on_device else exch.submit_strided(metric, q[g0:g0 + m], q.strides[0], m, k, False)
-                pending.append(t)
-                if len(pending) == exch.max_in_flight:
-                    results += exch.finish(pending.pop(0))
-            while pending:
+for on_device in (True, False):
+    for metric in (api.L2, api.DOT):
+        results, pending = [], []
+        for g0 in range(0, nq, exch.group):
+            m = min(exch.group, nq - g0)
+            t = exch.submit_strided(metric, qd[g0].data_ptr(), pitch, m, k, True) if on_device else exch.submit_strided(metric, q[g0:g0 + m], q.strides[0], m, k, False)
+            pending.append(t)
+            if len(pending) == exch.max_in_flight:
                 results += exch.finish(pending.pop(0))
-            assert len(results) == nq
-            for b in range(nq):
-                want_ids, want_d = orc.scan_dense(metric, po.I8, q[b], x, rowids, k)
-                assert np.array_equal(results[b][0], want_ids) and np.array_equal(results[b][1], want_d), (rank, fuse, on_device, metric, b)
-eng.set_option("fuse_mb", 0)
+        while pending:
+            results += exch.finish(pending.pop(0))
+        assert len(results) == nq
+        for b in range(nq):
+            want_ids, want_d = orc.scan_dense(metric, po.I8, q[b], x, rowids, k)
+            assert np.array_equal(results[b][0], want_ids) and np.array_equal(results[b][1], want_d), (rank, on_device, metric, b)
 r1 = exch.query(api.L1, q[3], 7, on_device=False)
 want_ids, want_d = orc.scan_dense(po.L1, po.I8, q[3], x, rowids, 7)
 assert np.array_equal(r1[0], want_ids) and np.array_equal(r1[1], want_d)
-# k = 256: more than 1024 survivors per shard -> the tails travel too; and the separate push kernel (push_mode = 1)
-for pm in (1, 0):
-    eng.set_option("push_mode", pm)
-    for kk in (256, 20):
-        for b in (0, 7):
-            rr = exch.query(api.L2, q[b], kk, on_device=False)
-            want_ids, want_d = orc.scan_dense(po.L2, po.I8, q[b], x, rowids, kk)
-            assert np.array_equal(rr[0], want_ids) and np.array_equal(rr[1], want_d), (rank, "push_mode", pm, kk, b)
-    t = exch.submit_strided(api.DOT, q[8:16], q.strides[0], 8, 20, False)
-    for j, rr in enumerate(exch.finish(t)):
-        want_ids, want_d = orc.scan_dense(po.DOT, po.I8, q[8 + j], x, rowids, 20)
-        assert np.array_equal(rr[0], want_ids) and np.array_equal(rr[1], want_d), (rank, "push_mode group", pm, j)
+# k = 256: more than 1024 survivors per shard -> the tails travel too; and a group of 8
+for kk in (256, 20):
+    for b in (0, 7):
+        rr = exch.query(api.L2, q[b], kk, on_device=False)
+        want_ids, want_d = orc.scan_dense(po.L2, po.I8, q[b], x, rowids, kk)
+        assert np.array_equal(rr[0], want_ids) and np.array_equal(rr[1], want_d), (rank, "tail", kk, b)
+t = exch.submit_strided(api.DOT, q[8:16], q.strides[0], 8, 20, False)
+for j, rr in enumerate(exch.finish(t)):
+    want_ids, want_d = orc.scan_dense(po.DOT, po.I8, q[8 + j], x, rowids, 20)
+    assert np.array_equal(rr[0], want_ids) and np.array_equal(rr[1], want_d), (rank, "group", j)
 # ---- batched queries: entry logs pushed over peer memory, device-side wait, GPU merge; two batches in flight
 qb = rng.integers(-6, 7, (70, dim)).astype(np.int8)
 for metric, kk in ((api.L2, 20), (api.COSINE, 100), (api.DOT, 7)):
@@ -252,22 +238,19 @@ for metric, kk in ((api.L2, 20), (api.COSINE, 100), (api.DOT, 7)):
     for b in range(70):
         want_ids, want_d = orc.scan_dense(metric, po.I8, qb[b], x, rowids, kk)
         assert np.array_equal(res[b][0], want_ids) and np.array_equal(res[b][1], want_d), (rank, "batch", metric, b)
-# a longer pipeline (the buffers are reused): merge on its own stream (default) and everything on the engine stream
+# a longer pipeline (the buffers are reused, the merge of batch j overlaps the levels of batch j + 1)
 qp = rng.integers(-6, 7, (7, 24, dim)).astype(np.int8)
 want_p = [[orc.scan_dense(po.L2, po.I8, qp[j, b], x, rowids, 10) for b in range(24)] for j in range(7)]
-for ms in (1, 0):
-    eng.set_option("merge_stream", ms)
-    got, pend = [], None
-    for j in range(7):
-        t = exch.batch_submit(api.L2, qp[j], 10)
-        if pend is not None:
-            got.append(exch.batch_finish(pend))
-        pend = t
-    got.append(exch.batch_finish(pend))
-    for j in range(7):
-        for b in range(24):
-            assert np.array_equal(got[j][b][0], want_p[j][b][0]) and np.array_equal(got[j][b][1], want_p[j][b][1]), (rank, "pipeline", ms, j, b)
-eng.set_option("merge_stream", 1)
+got, pend = [], None
+for j in range(7):
+    t = exch.batch_submit(api.L2, qp[j], 10)
+    if pend is not None:
+        got.append(exch.batch_finish(pend))
+    pend = t
+got.append(exch.batch_finish(pend))
+for j in range(7):
+    for b in range(24):
+        assert np.array_equal(got[j][b][0], want_p[j][b][0]) and np.array_equal(got[j][b][1], want_p[j][b][1]), (rank, "pipeline", j, b)
 # a shard-local capacity overflow (descending distances: every row enters the slots) must reach EVERY rank as ERANGE
 xo = np.zeros((n, 16), dtype=np.int8)
 xo[:, 0] = np.clip((n - 1 - np.arange(n)) // 1600, 0, 124).astype(np.int8)

@@ -43,7 +43,6 @@ qd = torch.zeros((nq, pitch), dtype=torch.uint8, device=device)
 qd[:, :dim] = torch.from_numpy(q.view(np.uint8)).to(device)
 torch.cuda.synchronize()
 for group in (1, 3, 8):
-    eng.set_option("fuse_mb", 4096 if group == 8 else 0)     # groups of 8 also as ONE fused scan launch
     exch = shard.DeviceExchange(ix, eng, world, bounds, device, group=group)
     for on_device in (True, False):
         results, pending = [], None
@@ -64,8 +63,6 @@ for group in (1, 3, 8):
         for b in range(nq):
             want_ids, want_d = orc.scan_dense(po.L2, po.I8, q[b], x, rowids, k)
             assert np.array_equal(results[b][0], want_ids) and np.array_equal(results[b][1], want_d), (rank, group, on_device, b)
-
-eng.set_option("fuse_mb", 0)
 
 # ---- batched queries: tensor-core levels per shard, all-gather of the entry logs, GPU merge
 for metric in (api.L2, api.COSINE, api.DOT):

@@ -224,16 +224,14 @@ def test_multi_shard_candidates_replay(eng, oracle):
 
 @pytest.mark.parametrize("vtype,dim,n", [(po.I8, 384, 150_000), (po.U8, 100, 40_000), (po.F32, 64, 30_000), (po.BF16, 1536, 9_000), (po.I8, 20000, 700)])
 def test_group_launch_equals_single_queries(eng, oracle, vtype, dim, n):
-    """vsb_scan_submit_group: ONE scan launch for a group of independent queries (the ring runs across query boundaries,
-    double-buffered query / k-list staging) must give exactly what the one-query-per-launch path gives, host queries and
-    device-side staging alike; the last case is the no-staging (DIRECT) kernel."""
+    """vsb_scan_submit_group (one scan launch per query, a full group and a partial one) must give exactly what single
+    queries give, host queries and device-side staging alike; the last case is the no-staging (DIRECT) kernel."""
     import sqlite_vector_b200 as vs
     rng = np.random.Generator(np.random.PCG64(2024 + dim))
     x = po.convert(rng.standard_normal((n, dim), dtype=np.float32), vtype)
     nq = 13
     q = po.convert(rng.standard_normal((nq, dim), dtype=np.float32), vtype)
     ix = make_index(vtype, x)
-    old_fuse = eng.set_option("fuse_mb", 4096)          # the option is off by default: here the group IS fused (8 queries per launch)
     for metric, k in [(po.L2, 20), (po.COS, 7), (po.DOT, 32), (po.L1, 40)]:
         want = ix.scan_topk(metric, q[0], k)            # warms the workspace for this k
         want = [ix.scan_topk(metric, q[b], k)[0] for b in range(nq)]
@@ -243,7 +241,6 @@ def test_group_launch_equals_single_queries(eng, oracle, vtype, dim, n):
             got += [ix.collect(first + j, k) for j in range(m)]
         for b in range(nq):
             assert np.array_equal(got[b][0], want[b][0]) and np.array_equal(got[b][1], want[b][1]), (vtype, metric, k, b)
-    eng.set_option("fuse_mb", old_fuse)
     ix.close()
 
 

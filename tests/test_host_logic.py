@@ -48,6 +48,23 @@ def test_no_cpu_fallback():
         vs.Index(vs.api.I8, 16, 10)
 
 
+def test_set_option_names_match_header():
+    """vsb_set_option accepts exactly the names its header comment lists; the retired group-launch, filter-push and
+    merge-stream options are refused."""
+    import sqlite_vector_b200 as vs
+    eng = vs.load_engine()
+    hdr = open(os.path.join(ROOT, "include", "vsb200.h")).read()
+    listed = re.search(r"tuning knobs for experiments: name in \{([^}]*)\}", hdr)
+    names = re.findall(r'"(\w+)"', listed.group(1))
+    assert len(names) >= 10
+    for name in names:
+        old = eng.set_option(name, 0)
+        assert old >= 0, (name, old, eng.lib.vsb_last_error())
+        assert eng.set_option(name, old) == 0, name
+    for name in ("fuse_mb", "push_mode", "merge_stream"):
+        assert eng.set_option(name, 0) == vs.api.EINVAL, name
+
+
 def test_product_never_imports_oracle():
     for dp, _, files in os.walk(os.path.join(ROOT, "sqlite_vector_b200")):
         for f in files:

@@ -10,7 +10,7 @@
 #   tc_variants   experimental epilogue variants of tc_scan_kernel (timing + correctness)
 #   fp_scan       single-query scan timing for f32 / f16 / bf16 (10M x 384)        ncu_fp   ncu --set full of the f32 scan
 #   sqlbench      tools/sql_bench.py at n = 1M for both extensions
-#   shard8        launch variants (scan streams x fused groups) on a 1/8 shard (1.25M x 384 int8)
+#   shard8        one or two scan streams on a 1/8 shard (1.25M x 384 int8)
 #   stream        f3: single-query scan of a streamed (pinned host -> two device windows) 10M x 384 int8 index
 #   sanitizer     compute-sanitizer memcheck + racecheck over small scans / batches
 set -u
@@ -53,7 +53,7 @@ for step in "$@"; do
       timeout 300 python tools/quick_bench.py --n 10000000 --dim 384 --vtype 2 --metric 4 --iters 30 2>&1 | tail -1 | tee -a ${O}_fp_scan.txt ;;
     ncu_fp)     timeout 600 $NCU --set full --import-source on -k regex:scan_kernel -s 8 -c 1 -f -o ${O}_scan_f32_full python tools/quick_bench.py --n 10000000 --dim 384 --vtype 1 --metric 1 --iters 10 > /dev/null 2>&1; export_rep ${O}_scan_f32_full ;;
     sqlbench)   timeout 900 python tools/sql_bench.py --n 1000000 --dim 384 --queries 50 --which both 2>&1 | cut -c1-900 | tee ${O}_sql_bench.jsonl ;;
-    shard8)     timeout 300 python tools/quick_group.py 2>&1 | tail -4 | tee ${O}_shard8.txt ;;
+    shard8)     timeout 300 python tools/quick_group.py 2>&1 | tail -2 | tee ${O}_shard8.txt ;;
     stream)     timeout 600 python tools/quick_stream.py 2>&1 | tail -1 | tee ${O}_stream.json ;;
     sanitizer)
       for tool in memcheck racecheck; do

@@ -236,6 +236,9 @@ VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */
 /* kernel launch counter (all kernels launched by this library since load) */
 VSB_API int64_t vsb_kernel_launches(void);
+/* diagnostics: CUDA allocations, events, streams and IPC mappings the library holds right now, over every index, group and
+ * quantizer of the process; freeing an object returns the count to what it was before the object was created */
+VSB_API int64_t vsb_debug_live_handles(void);
 /* with option "time_kernels"=N (N >= 1) every N-th query's kernels are bracketed by CUDA events on their streams; this returns
  * (and resets) the summed device time and launch count of the scan kernel and of the filter kernel. */
 VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double *filter_ms, int *filter_launches);

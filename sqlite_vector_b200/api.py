@@ -88,6 +88,7 @@ _SIGNATURES = {
     "vsb_index_stream": (_vp, [_vp]),
     "vsb_index_stat": (_i64, [_vp, C.c_char_p]),
     "vsb_kernel_launches": (_i64, []),
+    "vsb_debug_live_handles": (_i64, []),
     "vsb_set_option": (_i, [C.c_char_p, _i]),
     "vsb_profile_read": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vsb_debug_read": (_i, [_vp, C.c_char_p, _vp, _i64]),
@@ -132,6 +133,9 @@ class Engine:
 
     def kernel_launches(self) -> int:
         return int(self.lib.vsb_kernel_launches())
+
+    def debug_live_handles(self) -> int:
+        return int(self.lib.vsb_debug_live_handles())
 
     def set_option(self, name: str, value: int) -> int:
         return self.lib.vsb_set_option(name.encode(), int(value))

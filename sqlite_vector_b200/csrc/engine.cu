@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -27,6 +28,7 @@
 #include "scan_kernels.cuh"
 #include "batch_kernels.cuh"
 #include "quant_kernels.cuh"
+#include "owners.cuh"
 
 using namespace vsb;
 
@@ -113,14 +115,14 @@ constexpr int kSlots = 32;               // result slots: queries in flight (the
 // Scan workspace of one query (per-stream k-lists / CTA lists, in-CTA bounds, candidate logs): written by scan_kernel, read
 // by filter_kernel.  The Works rotate so that the filter of launch i (filter stream) overlaps the scan of launch i+1.
 struct Work {
-    float *d_lists = nullptr, *d_tlocal = nullptr;
-    uint2 *d_logs = nullptr;
-    int *d_counts = nullptr;
-    long long *d_bounds = nullptr;   // [CTAs + 1] adaptive tile partition used by the NEXT scan on this workspace
-    unsigned *d_cta_time = nullptr;  // [CTAs] cycles each scan CTA took (written by scan_kernel, read by filter_kernel)
+    DeviceBuf<float> d_lists, d_tlocal;
+    DeviceBuf<uint2> d_logs;
+    DeviceBuf<int> d_counts;
+    DeviceBuf<long long> d_bounds;   // [CTAs + 1] adaptive tile partition used by the NEXT scan on this workspace
+    DeviceBuf<unsigned> d_cta_time;  // [CTAs] cycles each scan CTA took (written by scan_kernel, read by filter_kernel)
     long long bounds_tiles = -1;     // total tiles the bounds were laid out for (-1: not initialised)
-    cudaEvent_t scanned = nullptr;   // scan stream: the scan that filled this workspace has finished
-    cudaEvent_t drained = nullptr;   // filter stream: the filters that read this workspace have finished
+    Event scanned;                   // scan stream: the scan that filled this workspace has finished
+    Event drained;                   // filter stream: the filters that read this workspace have finished
     bool in_use = false;
 };
 constexpr int kWorks = 4;
@@ -133,50 +135,61 @@ constexpr int kWorks = 4;
 struct Slot {
     ResultHead *d_head = nullptr, *h_head = nullptr; // this slot's head inside vsb_index::d_heads / h_heads
     uint2 *h_tail = nullptr, *d_tail = nullptr;      // survivors kFirstFetch.. (inside vsb_index::d_tails / h_tails)
-    uint8_t *h_query = nullptr, *d_query = nullptr;  // pinned staging + device copy of the query
-    int *d_ctrl = nullptr;
-    cudaEvent_t done = nullptr;   // recorded after the result block of this slot has been copied to the host
+    uint8_t *h_query = nullptr, *d_query = nullptr;  // pinned staging + device copy of the query (inside vsb_index::h_queries / d_queries)
+    int *d_ctrl = nullptr;                           // inside vsb_index::d_ctrl
+    Event done;   // recorded after the result block of this slot has been copied to the host
     int seq = 0;
 };
 
+struct BatchWs;   // batch_host.inc
+
 }  // namespace
 
+struct Exchange;    // exchange.inc
+
+// Destroyed only with its streams drained and its device current (vsb_index_free); see owners.cuh
 struct vsb_index {
+    Stream stream;    // staging, scans and the batch path
+    Stream fstream;   // filter + result copy of a query
+    Stream stream2;   // second scan stream (option scan_streams = 2): single-query scans alternate between the two
+    Stream xstream;   // exchange: flag wait + copy of the gathered heads to the host
+    Stream cstream;   // streamed index: window copies
     int device = 0, vtype = 0, dim = 0, esize = 0, pitch = 0;
     long long cap = 0, n = 0, first_seq = 0;
-    uint8_t *d_vec = nullptr;
+    DeviceBuf<uint8_t> d_vec;
     bool implicit_ids = true;
     std::vector<int64_t> h_rowids;
-    cudaStream_t stream = nullptr;
-    uint8_t *stage[2] = {nullptr, nullptr};
-    cudaEvent_t stage_ev[2] = {nullptr, nullptr};
+    HostBuf<uint8_t> stage[2];
+    Event stage_ev[2];
     int stage_next = 0;
     int num_sms = 0, max_smem = 0;
-    cudaStream_t fstream = nullptr;   // filter + result copy of a query; `stream` carries staging, scans and the batch path
     // streamed mode (corpus larger than the device budget, SURVEY §8 f3): the column lives in pinned host memory and passes
     // through two device windows of win_rows rows; every window is scanned like a shard while the next one is copied
     bool streamed = false;
-    uint8_t *h_arena = nullptr;       // [cap][pitch] pinned
-    uint8_t *d_win[2] = {nullptr, nullptr};
+    HostBuf<uint8_t> h_arena;         // [cap][pitch] pinned
+    DeviceBuf<uint8_t> d_win[2];
     long long win_rows = 0;
-    cudaStream_t cstream = nullptr;   // window copies
-    cudaEvent_t win_copied[2] = {nullptr, nullptr}, win_scanned[2] = {nullptr, nullptr};
+    Event win_copied[2], win_scanned[2];
     long long st_stream_bytes = 0, st_stream_us = 0;
-    cudaStream_t stream2 = nullptr;   // second scan stream (option scan_streams = 2): single-query scans alternate between the two
-    cudaStream_t xstream = nullptr;   // exchange: flag wait + copy of the gathered heads to the host
     int snext = 0;
-    struct Exchange *xch = nullptr;   // peer-memory exchange (multi-GPU), see exchange.inc
+    std::unique_ptr<Exchange> xch;    // peer-memory exchange (multi-GPU), see exchange.inc
     // scan workspaces
     int ws_kcap = 0, ws_logcap = 0, ws_streams = 0, ws_next = 0;
     Work work[kWorks];
     Slot slot[kSlots];
-    uint8_t *d_heads = nullptr, *h_heads = nullptr;   // kSlots x kHeadBytes
-    uint8_t *d_tails = nullptr, *h_tails = nullptr;   // kSlots x (kOutCap - kFirstFetch) x uint2
+    // the allocations behind the result slots (a Slot holds views into them)
+    DeviceBuf<uint8_t> d_heads;       // kSlots x kHeadBytes
+    HostBuf<uint8_t> h_heads;
+    DeviceBuf<uint8_t> d_tails;       // kSlots x (kOutCap - kFirstFetch) x uint2
+    HostBuf<uint8_t> h_tails;
+    HostBuf<uint8_t> h_queries;       // kSlots x pitch
+    DeviceBuf<uint8_t> d_queries;
+    DeviceBuf<int> d_ctrl;            // kSlots x 4
     bool slots_ready = false;
-    float *d_dist_all = nullptr;
+    DeviceBuf<float> d_dist_all;
     int last_slot = -1, last_metric = 0;
     // optional per-kernel event timing (vsb_profile_read)
-    std::vector<cudaEvent_t> prof_ev;   // quadruples: before scan, after scan (scan stream), before filter, after filter (filter stream)
+    std::vector<Event> prof_ev;         // quadruples: before scan, after scan (scan stream), before filter, after filter (filter stream)
     std::vector<int> prof_kind;         // 1 = scan only, 2 = scan + filter
     size_t prof_used = 0;
     unsigned prof_tick = 0;
@@ -184,7 +197,7 @@ struct vsb_index {
     long long st_queries = 0, st_survivors = 0, st_fallbacks = 0, st_last_survivors = 0;
     long long st_batches = 0, st_batch_cands = 0, st_batch_kept = 0, st_tc_us = 0, st_tc_rows = 0, st_batch_us = 0;
     int last_log2p = -1, last_nsw = -1, last_direct = -1;   // plan of the most recent scan launch (vsb_index_stat "plan_*")
-    void *batch = nullptr;   // BatchWs (tensor-core batch path workspace)
+    std::unique_ptr<BatchWs> batch;   // tensor-core batch path workspace
 };
 
 namespace {
@@ -261,58 +274,40 @@ Plan make_plan(const vsb_index *ix, int kcap) {
     return pl;
 }
 
-void free_slots(vsb_index *ix) {
-    if (ix->slot[0].h_query) cudaFreeHost(ix->slot[0].h_query);     // slot 0 holds the base of the shared allocations
-    if (ix->slot[0].d_query) cudaFree(ix->slot[0].d_query);
-    if (ix->slot[0].d_ctrl) cudaFree(ix->slot[0].d_ctrl);
-    for (int i = 0; i < kSlots; ++i) {
-        Slot &s = ix->slot[i];
-        if (s.done) cudaEventDestroy(s.done);
-        s = Slot();
-    }
-    if (ix->h_heads) cudaFreeHost(ix->h_heads);
-    if (ix->d_heads) cudaFree(ix->d_heads);
-    if (ix->h_tails) cudaFreeHost(ix->h_tails);
-    if (ix->d_tails) cudaFree(ix->d_tails);
-    ix->h_heads = nullptr; ix->d_heads = nullptr; ix->h_tails = nullptr; ix->d_tails = nullptr;
-    ix->slots_ready = false;
-}
-
-int ensure_slots_alloc(vsb_index *ix) {
-    const size_t tail_bytes = sizeof(uint2) * (size_t)(kOutCap - kFirstFetch);
-    CU(cudaMalloc((void **)&ix->d_heads, kHeadBytes * kSlots));
-    CU(cudaMemset(ix->d_heads, 0, kHeadBytes * kSlots));
-    CU(cudaHostAlloc((void **)&ix->h_heads, kHeadBytes * kSlots, cudaHostAllocDefault));
-    memset(ix->h_heads, 0, kHeadBytes * kSlots);
-    CU(cudaMalloc((void **)&ix->d_tails, tail_bytes * kSlots));
-    CU(cudaHostAlloc((void **)&ix->h_tails, tail_bytes * kSlots, cudaHostAllocDefault));
-    uint8_t *hq = nullptr, *dq = nullptr;                      // query staging of all slots: one pinned + one device allocation
-    int *dc = nullptr;
-    CU(cudaHostAlloc((void **)&hq, (size_t)ix->pitch * kSlots, cudaHostAllocDefault));
-    ix->slot[0].h_query = hq;
-    CU(cudaMalloc((void **)&dq, (size_t)ix->pitch * kSlots));
-    ix->slot[0].d_query = dq;
-    CU(cudaMalloc((void **)&dc, sizeof(int) * 4 * kSlots));
-    ix->slot[0].d_ctrl = dc;
-    CU(cudaMemset(dc, 0, sizeof(int) * 4 * kSlots));
-    for (int i = 0; i < kSlots; ++i) {
-        Slot &s = ix->slot[i];
-        s.d_head = (ResultHead *)(ix->d_heads + kHeadBytes * i);
-        s.h_head = (ResultHead *)(ix->h_heads + kHeadBytes * i);
-        s.d_tail = (uint2 *)(ix->d_tails + tail_bytes * i);
-        s.h_tail = (uint2 *)(ix->h_tails + tail_bytes * i);
-        s.h_query = hq + (size_t)ix->pitch * i;
-        s.d_query = dq + (size_t)ix->pitch * i;
-        s.d_ctrl = dc + 4 * i;
-        CU(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-    }
-    return VSB_OK;
-}
-
+// the result slots, built on first need
 int ensure_slots(vsb_index *ix) {
     if (ix->slots_ready) return VSB_OK;
-    const int rc = ensure_slots_alloc(ix);
-    if (rc != VSB_OK) { free_slots(ix); return rc; }   // a half-built slot set must not be reused (g_err keeps the CUDA message)
+    const size_t tail_bytes = sizeof(uint2) * (size_t)(kOutCap - kFirstFetch);
+    DeviceBuf<uint8_t> d_heads, d_tails, d_queries;
+    HostBuf<uint8_t> h_heads, h_tails, h_queries;
+    DeviceBuf<int> d_ctrl;
+    Event done[kSlots];
+    CU(d_heads.alloc(kHeadBytes * kSlots));
+    CU(cudaMemset(d_heads, 0, kHeadBytes * kSlots));
+    CU(h_heads.alloc(kHeadBytes * kSlots));
+    memset(h_heads, 0, kHeadBytes * kSlots);
+    CU(d_tails.alloc(tail_bytes * kSlots));
+    CU(h_tails.alloc(tail_bytes * kSlots));
+    CU(h_queries.alloc((size_t)ix->pitch * kSlots));        // query staging of all slots: one pinned + one device allocation
+    CU(d_queries.alloc((size_t)ix->pitch * kSlots));
+    CU(d_ctrl.alloc(sizeof(int) * 4 * kSlots));
+    CU(cudaMemset(d_ctrl, 0, sizeof(int) * 4 * kSlots));
+    for (Event &e : done) CU(e.create(cudaEventDisableTiming));
+    for (int i = 0; i < kSlots; ++i) {
+        Slot &s = ix->slot[i];
+        s.d_head = (ResultHead *)(d_heads + kHeadBytes * i);
+        s.h_head = (ResultHead *)(h_heads + kHeadBytes * i);
+        s.d_tail = (uint2 *)(d_tails + tail_bytes * i);
+        s.h_tail = (uint2 *)(h_tails + tail_bytes * i);
+        s.h_query = h_queries + (size_t)ix->pitch * i;
+        s.d_query = d_queries + (size_t)ix->pitch * i;
+        s.d_ctrl = d_ctrl + 4 * i;
+        s.done = std::move(done[i]);
+    }
+    ix->d_heads = std::move(d_heads); ix->h_heads = std::move(h_heads);
+    ix->d_tails = std::move(d_tails); ix->h_tails = std::move(h_tails);
+    ix->h_queries = std::move(h_queries); ix->d_queries = std::move(d_queries);
+    ix->d_ctrl = std::move(d_ctrl);
     ix->slots_ready = true;
     return VSB_OK;
 }
@@ -325,18 +320,6 @@ int drain(vsb_index *ix) {
     return VSB_OK;
 }
 
-// the device buffers of a workspace (its events stay)
-void free_work(Work &w) {
-    cudaFree(w.d_lists);
-    cudaFree(w.d_logs);
-    cudaFree(w.d_counts);
-    cudaFree(w.d_tlocal);
-    cudaFree(w.d_bounds);
-    cudaFree(w.d_cta_time);
-    w.d_lists = nullptr; w.d_tlocal = nullptr; w.d_logs = nullptr; w.d_counts = nullptr;
-    w.d_bounds = nullptr; w.d_cta_time = nullptr;
-}
-
 int ensure_workspace(vsb_index *ix, int k) {
     const int kcap = (k + 31) & ~31;
     const int logcap = std::max(256, 12 * k);
@@ -344,20 +327,22 @@ int ensure_workspace(vsb_index *ix, int k) {
     if (ix->ws_kcap >= kcap && ix->ws_logcap >= logcap && ix->ws_streams == streams) return VSB_OK;
     const int rc = drain(ix);       // queries in flight still use the old workspaces
     if (rc) return rc;
-    ix->ws_kcap = 0;
+    Work fresh[kWorks];
     for (int i = 0; i < kWorks; ++i) {
-        Work &w = ix->work[i];
-        free_work(w);
-        CU(cudaMalloc((void **)&w.d_lists, sizeof(float) * (size_t)streams * kcap));
-        CU(cudaMalloc((void **)&w.d_logs, sizeof(uint2) * (size_t)streams * logcap));
-        CU(cudaMalloc((void **)&w.d_counts, sizeof(int) * (size_t)streams));
-        CU(cudaMalloc((void **)&w.d_tlocal, sizeof(float) * (size_t)streams));
-        w.bounds_tiles = -1;
-        w.in_use = false;
-        CU(cudaMalloc((void **)&w.d_bounds, sizeof(long long) * (size_t)(ix->num_sms + 1)));
-        CU(cudaMalloc((void **)&w.d_cta_time, sizeof(unsigned) * (size_t)ix->num_sms));
-        if (!w.scanned) CU(cudaEventCreateWithFlags(&w.scanned, cudaEventDisableTiming));
-        if (!w.drained) CU(cudaEventCreateWithFlags(&w.drained, cudaEventDisableTiming));
+        Work &w = fresh[i], &old = ix->work[i];
+        CU(w.d_lists.alloc(sizeof(float) * (size_t)streams * kcap));
+        CU(w.d_logs.alloc(sizeof(uint2) * (size_t)streams * logcap));
+        CU(w.d_counts.alloc(sizeof(int) * (size_t)streams));
+        CU(w.d_tlocal.alloc(sizeof(float) * (size_t)streams));
+        CU(w.d_bounds.alloc(sizeof(long long) * (size_t)(ix->num_sms + 1)));
+        CU(w.d_cta_time.alloc(sizeof(unsigned) * (size_t)ix->num_sms));
+        if (!old.scanned) CU(old.scanned.create(cudaEventDisableTiming));
+        if (!old.drained) CU(old.drained.create(cudaEventDisableTiming));
+    }
+    for (int i = 0; i < kWorks; ++i) {   // the events stay across regrowth
+        fresh[i].scanned = std::move(ix->work[i].scanned);
+        fresh[i].drained = std::move(ix->work[i].drained);
+        ix->work[i] = std::move(fresh[i]);
     }
     ix->ws_kcap = kcap; ix->ws_logcap = logcap; ix->ws_streams = streams;
     return VSB_OK;
@@ -365,7 +350,6 @@ int ensure_workspace(vsb_index *ix, int k) {
 
 unsigned exchange_next_seq(vsb_index *ix, int slot);
 int merge_blocks_strided(const uint8_t *blocks, int world, size_t stride, const int64_t *first_seq, int k, int64_t *out_rowids, double *out_dist);
-void exchange_free(vsb_index *ix);
 int exchange_fill_push(vsb_index *ix, PushParams *pp);
 
 // launches the scan kernel for one query (device pointer, pitch bytes) on ss and, when k > 0, the filter on ix->fstream;
@@ -426,21 +410,21 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
     p.kcap = kcap;
     p.logcap = ix->ws_logcap;
     p.query = d_query;
-    p.lists = wk ? wk->d_lists : nullptr;
-    p.tlocal = wk ? wk->d_tlocal : nullptr;
-    p.logs = wk ? wk->d_logs : nullptr;
-    p.counts = wk ? wk->d_counts : nullptr;
+    p.lists = wk ? wk->d_lists.get() : nullptr;
+    p.tlocal = wk ? wk->d_tlocal.get() : nullptr;
+    p.logs = wk ? wk->d_logs.get() : nullptr;
+    p.counts = wk ? wk->d_counts.get() : nullptr;
     p.ctrl = slot ? slot->d_ctrl : nullptr;
     p.dist_all = d_dist_all;
-    p.bounds = balance ? wk->d_bounds : nullptr;
-    p.cta_time = balance ? wk->d_cta_time : nullptr;
-    cudaEvent_t *pev = nullptr;
+    p.bounds = balance ? wk->d_bounds.get() : nullptr;
+    p.cta_time = balance ? wk->d_cta_time.get() : nullptr;
+    Event *pev = nullptr;
     if (g_opt_time_kernels > 0 && (ix->prof_tick++ % g_opt_time_kernels) == 0) {   // time_kernels = N: every N-th launch
         if (ix->prof_used + 4 > ix->prof_ev.size()) {
             for (int i = 0; i < 4; ++i) {
-                cudaEvent_t e;
-                CU(cudaEventCreate(&e));
-                ix->prof_ev.push_back(e);
+                Event e;
+                CU(e.create(cudaEventDefault));
+                ix->prof_ev.push_back(std::move(e));
             }
         }
         pev = &ix->prof_ev[ix->prof_used];
@@ -484,7 +468,7 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
         f.ctrl = slot->d_ctrl;
         f.seqno = ++slot->seq;
         f.xseq = push ? exchange_next_seq(ix, (int)(slot - ix->slot)) : 0u;
-        f.bounds = balance ? wk->d_bounds : nullptr;
+        f.bounds = balance ? wk->d_bounds.get() : nullptr;
         f.cta_time = wk->d_cta_time;
         f.total_tiles = total_tiles;
         if (pev) CU(cudaEventRecord(pev[2], ix->fstream));
@@ -640,7 +624,7 @@ int scan_all_into(vsb_index *ix, int metric, const uint8_t *d_query, std::vector
         return streamed_scan_all(ix, metric, d_query, dist.data());
     }
     if (!ix->d_dist_all) {
-        CU(cudaMalloc((void **)&ix->d_dist_all, sizeof(float) * (size_t)std::max<long long>(ix->cap, 1)));
+        CU(ix->d_dist_all.alloc(sizeof(float) * (size_t)std::max<long long>(ix->cap, 1)));
         ix->dev_bytes += sizeof(float) * (size_t)ix->cap;
     }
     int rc = launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all, true, ix->stream);
@@ -695,7 +679,7 @@ int stream_windows(vsb_index *ix, int depth, Launch launch, Visit visit) {
 // all distances of a streamed index (stream modules, k > 256, overflow fallback)
 int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *out_dist) {
     if (!ix->d_dist_all) {
-        CU(cudaMalloc((void **)&ix->d_dist_all, sizeof(float) * 2 * (size_t)ix->win_rows));
+        CU(ix->d_dist_all.alloc(sizeof(float) * 2 * (size_t)ix->win_rows));
         ix->dev_bytes += sizeof(float) * 2 * (size_t)ix->win_rows;
     }
     return stream_windows(ix, 2,
@@ -842,6 +826,8 @@ const char *vsb_backend_name(void) {
 
 int64_t vsb_kernel_launches(void) { return g_launches.load(); }
 
+int64_t vsb_debug_live_handles(void) { return g_live_handles.load(); }
+
 int vsb_set_option(const char *name, int value) {
     int *p = nullptr;
     if (!strcmp(name, "stage_bytes")) p = &g_opt_stage_bytes;
@@ -892,57 +878,53 @@ static int index_create(vsb_index **out, int device, int vtype, int dim, int64_t
     CU(cudaGetDeviceProperties(&pr, device));
     if (pr.major != 9 || pr.minor != 0)   // sm_90a code (wgmma, TMA) runs on compute capability 9.0 only
         return fail(VSB_ENODEV, "device %s (cc %d.%d): this build holds sm_90a (H100) code only", pr.name, pr.major, pr.minor);
-    vsb_index *ix = new (std::nothrow) vsb_index();
+    std::unique_ptr<vsb_index> ix(new (std::nothrow) vsb_index());
     if (!ix) return fail(VSB_ENOMEM, "out of host memory");
     ix->device = device; ix->vtype = vtype; ix->dim = dim; ix->esize = es;
     ix->pitch = (dim * es + 15) & ~15;
     ix->cap = capacity_rows; ix->first_seq = first_seq;
     ix->num_sms = pr.multiProcessorCount;
     ix->max_smem = (int)pr.sharedMemPerBlockOptin;
-    cudaError_t e = cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ix->stream2, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ix->fstream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ix->xstream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) {
-        if (ix->stream) cudaStreamDestroy(ix->stream);
-        if (ix->stream2) cudaStreamDestroy(ix->stream2);
-        if (ix->fstream) cudaStreamDestroy(ix->fstream);
-        delete ix;
-        return fail(VSB_ECUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
-    }
+    cudaError_t e = ix->stream.create();
+    if (e == cudaSuccess) e = ix->stream2.create();
+    if (e == cudaSuccess) e = ix->fstream.create();
+    if (e == cudaSuccess) e = ix->xstream.create();
+    if (e != cudaSuccess) return fail(VSB_ECUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
     size_t bytes = (size_t)std::max<long long>(capacity_rows, 1) * ix->pitch + 1024;
     if (window_rows > 0) {
         // streamed: the column stays in pinned host memory, two windows on the device
         ix->streamed = true;
         ix->win_rows = std::min<long long>(std::max<long long>(window_rows, 32), std::max<long long>(capacity_rows, 32));
-        e = cudaHostAlloc((void **)&ix->h_arena, bytes, cudaHostAllocDefault);
+        e = ix->h_arena.alloc(bytes);
         const size_t wb = (size_t)ix->win_rows * ix->pitch + 1024;
         for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-            e = cudaMalloc((void **)&ix->d_win[b], wb);
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ix->win_copied[b], cudaEventDisableTiming);
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ix->win_scanned[b], cudaEventDisableTiming);
+            e = ix->d_win[b].alloc(wb);
+            if (e == cudaSuccess) e = ix->win_copied[b].create(cudaEventDisableTiming);
+            if (e == cudaSuccess) e = ix->win_scanned[b].create(cudaEventDisableTiming);
         }
-        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ix->cstream, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = ix->cstream.create();
         bytes = 2 * wb;
     } else {
-        e = cudaMalloc((void **)&ix->d_vec, bytes);
+        e = ix->d_vec.alloc(bytes);
     }
     if (e != cudaSuccess) {
         cudaGetLastError();
-        const std::string why = cudaGetErrorString(e);
-        vsb_index_free(ix);
-        return fail(VSB_ENOMEM, "allocating %zu bytes for the %s column failed: %s", bytes, window_rows > 0 ? "streamed" : "resident", why.c_str());
+        return fail(VSB_ENOMEM, "allocating %zu bytes for the %s column failed: %s", bytes, window_rows > 0 ? "streamed" : "resident", cudaGetErrorString(e));
     }
     ix->dev_bytes = bytes;
-    *out = ix;
+    *out = ix.release();
     return VSB_OK;
 }
 
 static int stage_acquire(vsb_index *ix, int *which) {
     const int b = ix->stage_next;
     if (!ix->stage[b]) {
-        CU(cudaHostAlloc((void **)&ix->stage[b], kStageBuf, cudaHostAllocDefault));
-        CU(cudaEventCreateWithFlags(&ix->stage_ev[b], cudaEventDisableTiming));
+        HostBuf<uint8_t> buf;
+        Event ev;
+        CU(buf.alloc(kStageBuf));
+        CU(ev.create(cudaEventDisableTiming));
+        ix->stage[b] = std::move(buf);
+        ix->stage_ev[b] = std::move(ev);
     } else {
         CU(cudaEventSynchronize(ix->stage_ev[b]));  // previous copy out of this buffer finished
     }
@@ -1053,8 +1035,8 @@ int vsb_index_finalize(vsb_index *ix) {
     CU(cudaSetDevice(ix->device));
     CU(cudaStreamSynchronize(ix->stream));
     for (int b = 0; b < 2; ++b) {  // the staging buffers are only needed while loading
-        if (ix->stage[b]) { cudaFreeHost(ix->stage[b]); ix->stage[b] = nullptr; }
-        if (ix->stage_ev[b]) { cudaEventDestroy(ix->stage_ev[b]); ix->stage_ev[b] = nullptr; }
+        ix->stage[b].reset();
+        ix->stage_ev[b].reset();
     }
     return VSB_OK;
 }
@@ -1090,34 +1072,8 @@ void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullpt
 void vsb_index_free(vsb_index *ix) {
     if (!ix) return;
     cudaSetDevice(ix->device);
-    drain(ix);                      // the streams exist: index_create deletes an index whose streams it could not create
+    drain(ix);
     cudaStreamSynchronize(ix->xstream);
-    exchange_free(ix);
-    for (int b = 0; b < 2; ++b) {
-        if (ix->stage[b]) cudaFreeHost(ix->stage[b]);
-        if (ix->stage_ev[b]) cudaEventDestroy(ix->stage_ev[b]);
-    }
-    free_slots(ix);
-    for (Work &w : ix->work) {
-        free_work(w);
-        if (w.scanned) cudaEventDestroy(w.scanned);
-        if (w.drained) cudaEventDestroy(w.drained);
-    }
-    if (ix->d_dist_all) cudaFree(ix->d_dist_all);
-    if (ix->d_vec) cudaFree(ix->d_vec);
-    if (ix->h_arena) cudaFreeHost(ix->h_arena);
-    for (int b = 0; b < 2; ++b) {
-        if (ix->d_win[b]) cudaFree(ix->d_win[b]);
-        if (ix->win_copied[b]) cudaEventDestroy(ix->win_copied[b]);
-        if (ix->win_scanned[b]) cudaEventDestroy(ix->win_scanned[b]);
-    }
-    if (ix->cstream) cudaStreamDestroy(ix->cstream);
-    for (cudaEvent_t e : ix->prof_ev) cudaEventDestroy(e);
-    batch_free(ix);
-    if (ix->fstream) cudaStreamDestroy(ix->fstream);
-    if (ix->xstream) cudaStreamDestroy(ix->xstream);
-    if (ix->stream2) cudaStreamDestroy(ix->stream2);
-    if (ix->stream) cudaStreamDestroy(ix->stream);
     delete ix;
 }
 
@@ -1354,11 +1310,10 @@ int vsb_batch_shard_scan(vsb_index *ix, int metric, const void *queries, int nq,
     int rc = batch_levels(ix, metric, queries, nq, k, true);
     if (rc) return rc;
     CU(cudaStreamSynchronize(ix->stream));
-    rc = batch_check(ix, (BatchWs *)ix->batch);
+    rc = batch_check(ix, ix->batch.get());
     if (rc) return rc;
     ix->st_batch_us += std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t0).count();
-    BatchWs *w = (BatchWs *)ix->batch;
-    *d_block = w->d_acc;
+    *d_block = ix->batch->d_acc;
     *bytes = (int64_t)acc_block_bytes(nq, acc_cap_of(k));
     return VSB_OK;
 }

@@ -65,8 +65,12 @@ VSB_API int vsb_index_create(vsb_index **out, int device, int vtype, int dim, in
  * re-reads the chunks from the shadow table for every query): the column is kept in PINNED HOST memory and streamed through two
  * device windows of window_rows rows each — the copy of window w+1 (cudaMemcpyAsync on its own stream) overlaps the scan of
  * window w; every window is scanned like a shard and the survivors are replayed in scan order, so results are those of a
- * resident index.  vsb_scan_topk / vsb_scan_all / vsb_scan_candidates work; the asynchronous, exchange and tensor-core batch entry
- * points need a resident index.  Counters: vsb_index_stat "stream_bytes" / "stream_us". */
+ * resident index.  vsb_scan_topk / vsb_scan_all / vsb_scan_candidates work.  A batch that the tensor-core path takes (see
+ * vsb_scan_topk) runs its levels window by window, one pass of the column per batch, with the results of the resident batch path;
+ * this needs windows of at least 128 rows (smaller windows: one pass per query), and vsb_batch_shard_scan works the same way.
+ * fp DOT batches add one more pass, once per column version, for the largest row norm.  The asynchronous entry points
+ * (vsb_scan_submit / vsb_collect) and the exchange need a resident index.  Counters: vsb_index_stat "stream_bytes" / "stream_us"
+ * (a batch: device time from its first window copy to its last level). */
 VSB_API int vsb_index_create_streamed(vsb_index **out, int device, int vtype, int dim, int64_t capacity_rows, int64_t first_seq,
                                       int64_t window_rows);
 VSB_API int vsb_index_is_streamed(const vsb_index *ix);

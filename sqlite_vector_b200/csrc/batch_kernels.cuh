@@ -552,7 +552,7 @@ __global__ void all_pairs_kernel(uint2 *cand, unsigned *count, long long m0, int
 }
 
 struct RefineParams {
-    const uint8_t *vec;      // [n][pitch]
+    const uint8_t *vec;      // [n][pitch] the rows the candidates index (streamed index: the window buffer)
     const uint8_t *queries;  // [nq][pitch] zero padded
     int pitch, root;
     const uint2 *cand;
@@ -563,6 +563,7 @@ struct RefineParams {
     unsigned *bcount;        // [nq] entries appended this level (may exceed bucket_cap => overflow, seen by replay_kernel)
     unsigned bucket_cap;
     unsigned *stats;         // [0] += candidates refined, [2] |= 1 when the candidate log overflowed
+    unsigned row_base;       // added to a candidate's row in the bucket: the shard row of vec's first row (window start, else 0)
 };
 
 constexpr unsigned kBucketCap = 2048;   // kept candidates per query and level (replay_kernel sorts them in shared memory)
@@ -634,7 +635,7 @@ __global__ void refine_kernel(const RefineParams rp) {
         const bool keep = live && sub == 0 && d < rp.U[cq.y];
         if (keep) {
             const unsigned w = atomicAdd(&rp.bcount[cq.y], 1u);
-            if (w < rp.bucket_cap) rp.bucket[(size_t)cq.y * rp.bucket_cap + w] = make_uint2(cq.x, __float_as_uint(d));
+            if (w < rp.bucket_cap) rp.bucket[(size_t)cq.y * rp.bucket_cap + w] = make_uint2(cq.x + rp.row_base, __float_as_uint(d));
         }
     }
 }

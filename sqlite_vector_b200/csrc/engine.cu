@@ -646,8 +646,10 @@ int stage_query(vsb_index *ix, Slot *slot, const void *query, cudaStream_t ss) {
 // ---- streamed index: the window loop.  Window w (rows [w * win_rows, ...)) is copied into d_win[w & 1] on the copy stream
 // while window w-1 is being scanned; a window is scanned exactly like a shard (scan + filter into a result slot), its survivors
 // carry window-local rows.  visit(w, first_row, rows, slot) is called in window order once the slot's head is on the host.
+// host_clock: add the loop's host time to stream_us, which measures the stream only when the visits wait for the windows (the
+// batch path waits for nothing here and times its windows with events, batch_account)
 template <class Launch, class Visit>
-int stream_windows(vsb_index *ix, int depth, Launch launch, Visit visit) {
+int stream_windows(vsb_index *ix, int depth, Launch launch, Visit visit, bool host_clock = true) {
     const long long W = (ix->n + ix->win_rows - 1) / ix->win_rows;
     const auto t0 = std::chrono::steady_clock::now();
     long long next_visit = 0;
@@ -672,7 +674,7 @@ int stream_windows(vsb_index *ix, int depth, Launch launch, Visit visit) {
         const int rc = visit(next_visit, next_visit * ix->win_rows, std::min(ix->win_rows, ix->n - next_visit * ix->win_rows), (int)(next_visit % depth));
         if (rc) return rc;
     }
-    ix->st_stream_us += std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t0).count();
+    if (host_clock) ix->st_stream_us += std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t0).count();
     return VSB_OK;
 }
 

@@ -103,6 +103,20 @@ VSB_API void vsb_index_free(vsb_index *ix);
 VSB_API int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k, int64_t *out_rowids,
                           double *out_dist, int *out_counts, int *max_index);
 
+/* ---- filtered top-k: the k nearest among a given set of rows (no counterpart in the reference) ------------------------------
+ * allow: HOST bitmap over the index's scan-order rows, row i eligible when bit i & 31 of word i >> 5 is set; nbits must equal
+ * vsb_index_rows(ix) (else VSB_EINVAL).  The result is exactly what vsb_scan_topk returns for a column holding only the eligible
+ * rows, in this column's scan order: the same max_index carry, exchange sort and INF trim (fewer than k eligible rows give fewer
+ * than k results, none give zero rows), bit-exact for int8/uint8.  With every row eligible it equals vsb_scan_topk bit for bit.
+ * Otherwise the contract is vsb_scan_topk's: the same batch conditions and fallbacks.  The bitmap is copied to the device once per
+ * call.  A filtered scan still reads the whole column. */
+VSB_API int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *queries, int nq, int k, const uint32_t *allow, int64_t nbits,
+                                   int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
+/* rowids -> eligibility bitmap of ix (out_bits: (vsb_index_rows + 31) / 32 words, overwritten).  Rowids not in the column are
+ * ignored, duplicates are harmless.  Returns the number of eligible rows, or < 0.  Explicit rowids use a rowid -> row table built
+ * on first use and rebuilt after an append. */
+VSB_API int64_t vsb_index_rowid_bitmap(vsb_index *ix, const int64_t *rowids, int64_t n, uint32_t *out_bits);
+
 /* every row's distance for one query, in scan order (what the *_stream modules compute one row per
  * xNext, src/sqlite-vector.c:1901-1998).  out_dist has vsb_index_rows() floats; out_rowids may be NULL. */
 VSB_API int vsb_scan_all(vsb_index *ix, int metric, const void *query, float *out_dist, int64_t *out_rowids);
@@ -210,6 +224,10 @@ VSB_API int vsb_group_finalize(vsb_group *g);
 VSB_API int vsb_group_scan_topk(vsb_group *g, int metric, const void *queries, int nq, int k, int64_t *out_rowids, double *out_dist,
                                 int *out_counts, int *max_index);
 VSB_API int vsb_group_scan_all(vsb_group *g, int metric, const void *query, float *out_dist, int64_t *out_rowids);
+/* vsb_scan_topk_filtered / vsb_index_rowid_bitmap over the group's global scan order (nbits = vsb_group_rows) */
+VSB_API int vsb_group_scan_topk_filtered(vsb_group *g, int metric, const void *queries, int nq, int k, const uint32_t *allow, int64_t nbits,
+                                         int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
+VSB_API int64_t vsb_group_rowid_bitmap(vsb_group *g, const int64_t *rowids, int64_t n, uint32_t *out_bits);
 VSB_API int vsb_group_gpus(const vsb_group *g);
 VSB_API int64_t vsb_group_rows(const vsb_group *g);
 VSB_API vsb_index *vsb_group_shard(vsb_group *g, int shard); /* borrowed; for statistics */

@@ -48,6 +48,8 @@ _SIGNATURES = {
     "vsb_index_device_bytes": (_i64, [_vp]),
     "vsb_index_free": (None, [_vp]),
     "vsb_scan_topk": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "vsb_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "vsb_index_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
     "vsb_scan_all": (_i, [_vp, _i, _vp, _vp, _vp]),
     "vsb_scan_candidates": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _vp]),
     "vsb_replay_topk": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
@@ -74,6 +76,8 @@ _SIGNATURES = {
     "vsb_group_finalize": (_i, [_vp]),
     "vsb_group_scan_topk": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "vsb_group_scan_all": (_i, [_vp, _i, _vp, _vp, _vp]),
+    "vsb_group_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "vsb_group_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
     "vsb_group_gpus": (_i, [_vp]),
     "vsb_group_rows": (_i64, [_vp]),
     "vsb_group_shard": (_vp, [_vp, _i]),
@@ -169,6 +173,50 @@ class Engine:
         return ids[:cnt].copy(), dist[:cnt].copy(), mi.value
 
 
+def row_bitmap(mask) -> np.ndarray:
+    """boolean mask over scan-order rows -> the row bitmap of the filtered scans (uint32 words, row i: bit i & 31 of word i >> 5)"""
+    b = np.packbits(np.ascontiguousarray(mask, dtype=bool), bitorder="little")
+    return np.concatenate([b, np.zeros((-len(b)) % 4, np.uint8)]).view("<u4").copy()
+
+
+def _allow_words(allow, rows: int) -> np.ndarray:
+    """a bitmap of the filtered scans from a boolean mask of `rows` rows or from uint32 words"""
+    a = np.asarray(allow)
+    if a.dtype == bool:
+        if a.shape != (rows,):
+            raise ValueError(f"the mask has {a.shape} entries, the column {rows} rows")
+        return row_bitmap(a)
+    w = np.ascontiguousarray(a, dtype=np.uint32)
+    if w.size < (rows + 31) // 32:
+        raise ValueError(f"the bitmap has {w.size} words, {rows} rows need {(rows + 31) // 32}")
+    return w
+
+
+def _topk(eng: "Engine", call, queries: np.ndarray, k: int, max_index: int | None, as_arrays: bool):
+    """the output handling of the scan_topk entry points: call(queries, nq, ids, dist, counts, max_index pointer) -> rc"""
+    q = np.ascontiguousarray(queries)
+    q2 = q.reshape(-1, q.shape[-1]) if q.ndim > 1 else q.reshape(1, -1)
+    nq = q2.shape[0]
+    ids = np.zeros((nq, max(k, 1)), dtype=np.int64)
+    dist = np.zeros((nq, max(k, 1)), dtype=np.float64)
+    counts = np.zeros(nq, dtype=np.int32)
+    mi = C.c_int(0 if max_index is None else max_index)
+    eng.check(call(_ptr(q2), nq, _ptr(ids), _ptr(dist), _ptr(counts), C.byref(mi) if max_index is not None else None))
+    if as_arrays:
+        return ((ids, dist, counts), mi.value) if max_index is not None else (ids, dist, counts)
+    out = [(ids[b, :counts[b]].copy(), dist[b, :counts[b]].copy()) for b in range(nq)]
+    return (out, mi.value) if max_index is not None else out
+
+
+def _rowid_bitmap(eng: "Engine", fn, h, rows: int, rowids) -> tuple[np.ndarray, int]:
+    rid = np.ascontiguousarray(rowids, dtype=np.int64).reshape(-1)
+    bits = np.zeros(max((rows + 31) // 32, 1), dtype=np.uint32)
+    n = fn(h, _ptr(rid), rid.size, _ptr(bits))
+    if n < 0:
+        eng.check(int(n))
+    return bits, int(n)
+
+
 _ENGINE = None
 
 
@@ -230,21 +278,21 @@ class Index:
     def scan_topk(self, metric: int, queries: np.ndarray, k: int, max_index: int | None = None, as_arrays: bool = False):
         """top-k of one query or a batch.  Returns one (rowids, distances) pair per query, or with as_arrays the C-ABI's own
         output (rowids[nq, k], distances[nq, k], counts[nq]) without the per-query Python objects."""
-        q = np.ascontiguousarray(queries)
-        q2 = q.reshape(-1, q.shape[-1]) if q.ndim > 1 else q.reshape(1, -1)
-        nq = q2.shape[0]
-        ids = np.zeros((nq, max(k, 1)), dtype=np.int64)
-        dist = np.zeros((nq, max(k, 1)), dtype=np.float64)
-        counts = np.zeros(nq, dtype=np.int32)
-        mi = C.c_int(0 if max_index is None else max_index)
-        self.eng.check(self.eng.lib.vsb_scan_topk(self.h, metric, _ptr(q2), nq, k, _ptr(ids), _ptr(dist), _ptr(counts),
-                                                 C.byref(mi) if max_index is not None else None))
-        if as_arrays:
-            return ((ids, dist, counts), mi.value) if max_index is not None else (ids, dist, counts)
-        out = [(ids[b, :counts[b]].copy(), dist[b, :counts[b]].copy()) for b in range(nq)]
-        if max_index is not None:
-            return out, mi.value
-        return out
+        lib = self.eng.lib
+        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_scan_topk(self.h, metric, q, nq, k, ids, dist, counts, mi),
+                     queries, k, max_index, as_arrays)
+
+    def scan_topk_filtered(self, metric: int, queries: np.ndarray, k: int, allow, max_index: int | None = None, as_arrays: bool = False):
+        """scan_topk among the eligible rows only (vsb_scan_topk_filtered): `allow` is a boolean mask over the scan-order rows or
+        a uint32 row bitmap (row_bitmap, rowid_bitmap)"""
+        bits, lib = _allow_words(allow, self.rows), self.eng.lib
+        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
+                                                                                               ids, dist, counts, mi),
+                     queries, k, max_index, as_arrays)
+
+    def rowid_bitmap(self, rowids) -> tuple[np.ndarray, int]:
+        """(row bitmap of the rows whose rowid is in `rowids`, number of such rows) (vsb_index_rowid_bitmap)"""
+        return _rowid_bitmap(self.eng, self.eng.lib.vsb_index_rowid_bitmap, self.h, self.rows, rowids)
 
     def scan_all(self, metric: int, query: np.ndarray, want_rowids: bool = False):
         n = self.rows
@@ -500,17 +548,20 @@ class Group:
         self.eng.check(self.eng.lib.vsb_group_finalize(self.h))
 
     def scan_topk(self, metric: int, queries: np.ndarray, k: int, max_index: int | None = None):
-        q = np.ascontiguousarray(queries)
-        q2 = q.reshape(-1, q.shape[-1]) if q.ndim > 1 else q.reshape(1, -1)
-        nq = q2.shape[0]
-        ids = np.zeros((nq, max(k, 1)), dtype=np.int64)
-        dist = np.zeros((nq, max(k, 1)), dtype=np.float64)
-        counts = np.zeros(nq, dtype=np.int32)
-        mi = C.c_int(0 if max_index is None else max_index)
-        self.eng.check(self.eng.lib.vsb_group_scan_topk(self.h, metric, _ptr(q2), nq, k, _ptr(ids), _ptr(dist), _ptr(counts),
-                                                       C.byref(mi) if max_index is not None else None))
-        out = [(ids[b, :counts[b]].copy(), dist[b, :counts[b]].copy()) for b in range(nq)]
-        return (out, mi.value) if max_index is not None else out
+        lib = self.eng.lib
+        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_group_scan_topk(self.h, metric, q, nq, k, ids, dist, counts, mi),
+                     queries, k, max_index, False)
+
+    def scan_topk_filtered(self, metric: int, queries: np.ndarray, k: int, allow, max_index: int | None = None):
+        """Index.scan_topk_filtered over the group's global scan order (vsb_group_scan_topk_filtered)"""
+        bits, lib = _allow_words(allow, self.rows), self.eng.lib
+        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_group_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
+                                                                                                     ids, dist, counts, mi),
+                     queries, k, max_index, False)
+
+    def rowid_bitmap(self, rowids) -> tuple[np.ndarray, int]:
+        """Index.rowid_bitmap over the group's global scan order (vsb_group_rowid_bitmap)"""
+        return _rowid_bitmap(self.eng, self.eng.lib.vsb_group_rowid_bitmap, self.h, self.rows, rowids)
 
     def scan_all(self, metric: int, query: np.ndarray, want_rowids: bool = False):
         n = self.rows

@@ -47,6 +47,9 @@ struct TcParams {
     unsigned *cand_count;
     unsigned cand_cap;
     uint32_t *scores;       // MC_TC_SCORES only: [r1 - r0][nq] int32 / float bits
+    // row filter: a row whose bit allow_base + row is clear is never a hit (ScanParams::allow); nullptr: every row is eligible
+    const uint32_t *allow;
+    long long allow_base;
 };
 
 // ------------------------------------------------------------------ PTX wrappers (TMA / wgmma)
@@ -256,7 +259,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
         uint32_t nbits[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {                                          // issued before the MMAs: the load latency hides behind them
-            rowvalid[h] = row[h] >= prm.r0 && row[h] < prm.r1;
+            // an ineligible row is never a hit: the bound U comes from eligible rows only, so one that scores better (a copy of
+            // the query) would otherwise flood the candidate log
+            rowvalid[h] = row[h] >= prm.r0 && row[h] < prm.r1 && row_allowed(prm.allow, prm.allow_base + row[h]);
             nbits[h] = rowvalid[h] ? reinterpret_cast<const uint32_t *>(prm.norms)[row[h]] : 0u;
         }
         int prev = -1;
@@ -465,7 +470,7 @@ __global__ void __launch_bounds__(kL1Threads, 1) l1_batch_kernel(const __grid_co
 #pragma unroll
         for (int i = 0; i < R; ++i) {
             row[i] = mt * kTcM + lane + 32 * i;
-            rowvalid[i] = row[i] >= prm.r0 && row[i] < prm.r1;
+            rowvalid[i] = row[i] >= prm.r0 && row[i] < prm.r1 && row_allowed(prm.allow, prm.allow_base + row[i]);
         }
         const int qbase = ng * N + q0;
         if (prm.mc == MC_TC_SCORES) {
@@ -543,12 +548,25 @@ __global__ void row_norm_kernel(const uint8_t *vec, long long n, int pitch, void
 }
 
 // ------------------------------------------------------------------ exact refinement
-// level 0: every (row, query) pair of the first m0 rows is a candidate
-__global__ void all_pairs_kernel(uint2 *cand, unsigned *count, long long m0, int nq) {
-    const long long total = m0 * nq;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
-        cand[i] = make_uint2((uint32_t)(i % m0), (uint32_t)(i / m0));
-    if (blockIdx.x == 0 && threadIdx.x == 0) *count = (unsigned)total;
+// level 0: every (row, query) pair of the first m0 rows is a candidate.  With a row filter (allow != nullptr) only the eligible
+// rows' pairs are, appended one warp per row (the caller has checked their number against the log; *count starts at 0)
+__global__ void all_pairs_kernel(uint2 *cand, unsigned *count, long long m0, int nq, const uint32_t *allow, long long allow_base) {
+    if (allow == nullptr) {
+        const long long total = m0 * nq;
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
+            cand[i] = make_uint2((uint32_t)(i % m0), (uint32_t)(i / m0));
+        if (blockIdx.x == 0 && threadIdx.x == 0) *count = (unsigned)total;
+        return;
+    }
+    const int lane = threadIdx.x & 31;
+    const long long nwarps = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < m0; row += nwarps) {
+        if (!row_allowed(allow, allow_base + row)) continue;                  // warp-uniform
+        unsigned base = 0;
+        if (lane == 0) base = atomicAdd(count, (unsigned)nq);
+        base = __shfl_sync(0xFFFFFFFFu, base, 0);
+        for (int q = lane; q < nq; q += 32) cand[base + q] = make_uint2((uint32_t)row, (uint32_t)q);
+    }
 }
 
 struct RefineParams {

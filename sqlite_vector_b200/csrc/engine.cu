@@ -198,6 +198,15 @@ struct vsb_index {
     long long st_batches = 0, st_batch_cands = 0, st_batch_kept = 0, st_tc_us = 0, st_tc_rows = 0, st_batch_us = 0;
     int last_log2p = -1, last_nsw = -1, last_direct = -1;   // plan of the most recent scan launch (vsb_index_stat "plan_*")
     std::unique_ptr<BatchWs> batch;   // tensor-core batch path workspace
+    // row filter of the filtered scan in progress (vsb_scan_topk_filtered, FilterScope): bitmaps over this shard's rows (row i:
+    // bit i & 31 of word i >> 5) on the host and in d_allow; both null outside such a call, when every row is eligible
+    const uint32_t *flt_h = nullptr, *flt_d = nullptr;
+    DeviceBuf<uint32_t> d_allow;      // rows / 32 words + 1: a warp's read past the last row stays inside
+    size_t allow_words = 0;
+    // rowid -> row lookup of explicit rowids (vsb_index_rowid_bitmap): (rowid, row) sorted, built for rowid_rows rows on first
+    // need; an append changes n and so rebuilds it
+    std::vector<std::pair<int64_t, long long>> rowid_sorted;
+    long long rowid_rows = -1;
 };
 
 namespace {
@@ -358,8 +367,9 @@ int exchange_fill_push(vsb_index *ix, PushParams *pp);
 // ss: the scan stream of this launch (next_scan_stream); push: the head is labelled for the exchange (shard index and
 // exchange sequence number); push_heads_kernel moves it (exchange_push)
 // view_vec / view_n: scan these rows instead of the resident column (the windows of a streamed index)
+// view_r0: the shard row of view_vec's first row (the row filter is indexed by shard rows)
 int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *slot, float *d_dist_all, bool fetch, cudaStream_t ss,
-                bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1) {
+                bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1, long long view_r0 = 0) {
     const uint8_t *scan_vec = view_vec ? view_vec : ix->d_vec;
     const long long scan_n = view_vec ? view_n : ix->n;
     if (!scan_vec) return fail(VSB_EINVAL, "this entry point needs a resident (not streamed) index");
@@ -418,6 +428,8 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
     p.dist_all = d_dist_all;
     p.bounds = balance ? wk->d_bounds.get() : nullptr;
     p.cta_time = balance ? wk->d_cta_time.get() : nullptr;
+    p.allow = ix->flt_d;
+    p.allow_base = view_r0;
     Event *pev = nullptr;
     if (g_opt_time_kernels > 0 && (ix->prof_tick++ % g_opt_time_kernels) == 0) {   // time_kernels = N: every N-th launch
         if (ix->prof_used + 4 > ix->prof_ev.size()) {
@@ -701,8 +713,8 @@ int streamed_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k
     *overflow = false;
     const int depth = 4;                                  // result slots 0..3 rotate over the windows
     return stream_windows(ix, depth,
-        [&](long long, const uint8_t *vec, long long rows, int s) {
-            return launch_scan(ix, metric, d_query, k, &ix->slot[s], nullptr, true, ix->stream, false, vec, rows);
+        [&](long long w, const uint8_t *vec, long long rows, int s) {
+            return launch_scan(ix, metric, d_query, k, &ix->slot[s], nullptr, true, ix->stream, false, vec, rows, w * ix->win_rows);
         },
         [&](long long, long long r0, long long, int s) {
             bool ovf = false;
@@ -713,19 +725,83 @@ int streamed_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k
         });
 }
 
-// the all-distances fallback (k > kMaxK, candidate overflow): every row is a candidate, in scan order
+inline bool row_eligible(const uint32_t *bits, long long row) { return ((bits[row >> 5] >> (row & 31)) & 1u) != 0u; }
+
+// eligible rows among [a, b) of a row bitmap
+long long count_bits(const uint32_t *bits, long long a, long long b) {
+    long long c = 0;
+    for (; a < b && (a & 31); ++a) c += row_eligible(bits, a);
+    for (; a + 32 <= b; a += 32) c += __builtin_popcount(bits[a >> 5]);
+    for (; a < b; ++a) c += row_eligible(bits, a);
+    return c;
+}
+
+// the all-distances fallback (k > kMaxK, candidate overflow): every (eligible) row is a candidate, in scan order
 int all_candidates(vsb_index *ix, int metric, const uint8_t *d_query, std::vector<uint2> &cands) {
     ix->st_fallbacks++;
     std::vector<float> dist;
     const int rc = scan_all_into(ix, metric, d_query, dist);
     if (rc) return rc;
-    cands.resize((size_t)ix->n);
+    cands.clear();
+    cands.reserve((size_t)ix->n);
     for (long long i = 0; i < ix->n; ++i) {
+        if (ix->flt_h && !row_eligible(ix->flt_h, i)) continue;
         uint32_t bits;
         memcpy(&bits, &dist[(size_t)i], 4);
-        cands[(size_t)i] = make_uint2(bits, (uint32_t)i);
+        cands.push_back(make_uint2(bits, (uint32_t)i));
     }
     return VSB_OK;
+}
+
+// Sets the row filter of one filtered call on ix (host bitmap `bits` over ix->n rows, uploaded once into ix->d_allow); the
+// scope's destructor clears it, so that every other entry point sees an unfiltered index
+struct FilterScope {
+    vsb_index *ix = nullptr;
+    FilterScope() = default;
+    FilterScope(const FilterScope &) = delete;
+    FilterScope &operator=(const FilterScope &) = delete;
+    ~FilterScope() {
+        if (ix) { ix->flt_h = nullptr; ix->flt_d = nullptr; }
+    }
+};
+
+int filter_begin(vsb_index *ix, const uint32_t *bits, FilterScope *scope) {
+    CU(cudaSetDevice(ix->device));
+    const size_t words = (size_t)((ix->n + 31) / 32) + 1;
+    if (words > ix->allow_words) {        // filtered calls are synchronous: no launch still reads the old buffer
+        DeviceBuf<uint32_t> d;
+        CU(d.alloc(4 * words));
+        ix->dev_bytes += 4 * (words - ix->allow_words);
+        ix->d_allow = std::move(d);
+        ix->allow_words = words;
+    }
+    if (words > 1) CU(cudaMemcpyAsync(ix->d_allow, bits, 4 * (words - 1), cudaMemcpyHostToDevice, ix->stream));
+    CU(cudaMemsetAsync(ix->d_allow + (words - 1), 0, 4, ix->stream));
+    CU(cudaStreamSynchronize(ix->stream));   // the scans of a group may run on the second scan stream
+    ix->flt_h = bits;
+    ix->flt_d = ix->d_allow;
+    scope->ix = ix;
+    return VSB_OK;
+}
+
+// calls mark(row) for every row of ix whose rowid is in rowids[0, n); rowids not in the column are skipped
+template <class Mark>
+void rows_of_rowids(vsb_index *ix, const int64_t *rowids, int64_t n, Mark mark) {
+    if (ix->implicit_ids) {                                   // rowid = first_seq + row + 1
+        for (int64_t i = 0; i < n; ++i)
+            if (rowids[i] > ix->first_seq && rowids[i] - ix->first_seq <= ix->n) mark((long long)(rowids[i] - ix->first_seq - 1));
+        return;
+    }
+    if (ix->rowid_rows != ix->n) {
+        ix->rowid_sorted.resize((size_t)ix->n);
+        for (long long r = 0; r < ix->n; ++r) ix->rowid_sorted[(size_t)r] = {ix->h_rowids[(size_t)r], r};
+        std::sort(ix->rowid_sorted.begin(), ix->rowid_sorted.end());
+        ix->rowid_rows = ix->n;
+    }
+    const auto &s = ix->rowid_sorted;
+    for (int64_t i = 0; i < n; ++i)
+        for (auto it = std::lower_bound(s.begin(), s.end(), std::make_pair(rowids[i], (long long)INT64_MIN)); it != s.end() && it->first == rowids[i]; ++it)
+            mark(it->second);
 }
 
 // stages one host query on ix->stream into the slot of the synchronous calls (streamed: slots 0..3 rotate over the windows,
@@ -1110,6 +1186,25 @@ int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k,
     }
     cur.finish();
     return VSB_OK;
+}
+
+int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *queries, int nq, int k, const uint32_t *allow, int64_t nbits,
+                           int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index) {
+    if (check_index(ix)) return VSB_EINVAL;
+    if (nbits != ix->n) return fail(VSB_EINVAL, "the row bitmap has %lld bits, the index %lld rows", (long long)nbits, ix->n);
+    if (!allow && nbits > 0) return fail(VSB_EINVAL, "the row bitmap is null");
+    FilterScope scope;
+    const int rc = filter_begin(ix, allow, &scope);
+    if (rc) return rc;
+    return vsb_scan_topk(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts, max_index);
+}
+
+int64_t vsb_index_rowid_bitmap(vsb_index *ix, const int64_t *rowids, int64_t n, uint32_t *out_bits) {
+    if (check_index(ix)) return VSB_EINVAL;
+    if (n < 0 || (!rowids && n > 0) || !out_bits) return fail(VSB_EINVAL, "bad rowid bitmap arguments");
+    memset(out_bits, 0, sizeof(uint32_t) * (size_t)((ix->n + 31) / 32));
+    rows_of_rowids(ix, rowids, n, [&](long long row) { out_bits[row >> 5] |= 1u << (row & 31); });
+    return count_bits(out_bits, 0, ix->n);
 }
 
 int vsb_scan_all(vsb_index *ix, int metric, const void *query, float *out_dist, int64_t *out_rowids) {

@@ -61,7 +61,16 @@ struct ScanParams {
     // HBM at the same rate, and with equal shares the slowest one sets the kernel time).
     const long long *bounds;   // [gridDim.x + 1] or nullptr (equal shares)
     unsigned *cta_time;        // [gridDim.x] or nullptr
+    // row filter (vsb_scan_topk_filtered): row r of vec is eligible when bit allow_base + r of the shard bitmap `allow` is set;
+    // nullptr: every row is.  An ineligible row never enters a k-list or a log (dist_all is written for every row)
+    const uint32_t *allow;
+    long long allow_base;      // shard row of vec's first row (a window of a streamed index), else 0
 };
+
+// bit `row` of a row bitmap (bit row & 31 of word row >> 5); nullptr: every row is eligible
+__device__ __forceinline__ bool row_allowed(const uint32_t *allow, long long row) {
+    return allow == nullptr || ((__ldg(allow + (row >> 5)) >> (row & 31)) & 1u) != 0u;
+}
 
 // ------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -575,7 +584,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
         if (prm.dist_all != nullptr && valid && p == 0) prm.dist_all[row0 + r] = d;
         if (topk) {
             // rows are visited in scan order (lane order); strict '<' like the reference (:2102, :2145)
-            unsigned m = __ballot_sync(0xFFFFFFFFu, valid && p == 0 && d < thr);
+            unsigned m = __ballot_sync(0xFFFFFFFFu, valid && p == 0 && d < thr && row_allowed(prm.allow, prm.allow_base + row0 + r));
             while (m) {
                 const int src = __ffs(m) - 1;
                 m &= m - 1;

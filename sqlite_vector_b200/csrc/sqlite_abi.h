@@ -128,6 +128,12 @@ typedef struct sqlite3_api_routines {
 extern const sqlite3_api_routines *vsq_api;
 #define VSQ_CALL(name, type) ((type)vsq_api->slot[VSQ_##name])
 
+/* sqlite3_aggregate_context (vector_rowid_set) is the struct's first member; the slot table above is pinned by
+ * tests/golden/sqlite3_api_slots.json, this one by tests/golden/sqlite3_api_slot_aggregate.json (tests/test_filtered_host.py),
+ * both taken from the same sqlite3ext.h */
+#define VSQ_SLOT_AGGREGATE_CONTEXT 0
+#define sqlite3_aggregate_context ((void *(*)(sqlite3_context *, int))vsq_api->slot[VSQ_SLOT_AGGREGATE_CONTEXT])
+
 #define sqlite3_bind_blob VSQ_CALL(bind_blob, int (*)(sqlite3_stmt *, int, const void *, int, sqlite3_destructor_type))
 #define sqlite3_bind_double VSQ_CALL(bind_double, int (*)(sqlite3_stmt *, int, double))
 #define sqlite3_bind_int VSQ_CALL(bind_int, int (*)(sqlite3_stmt *, int, int))

@@ -6,6 +6,8 @@
  *           vector_quantize_preload, vector_quantize_cleanup, vector_as_{f32,f16,bf16,i8,u8} (1|2 args)
  *   table-valued: vector_full_scan, vector_quantize_scan (tbl, col, vector, k),
  *                 vector_full_scan_stream, vector_quantize_scan_stream (tbl, col, vector)
+ * additions: vector_*_scan_batch (tbl, col, vectors, k); vector_*_scan_filtered (tbl, col, vector, k, rowids),
+ *            vector_*_scan_batch_filtered (tbl, col, vectors, k, rowids) and the aggregate vector_rowid_set(x) that builds rowids
  * Column state, option parsing, JSON vectors, quantization build and the shadow-table chunk format are host
  * C and behave like the reference (citations at each function).  What differs is where a scan runs:
  *   vector_quantize_preload  -> chunks are staged through pinned memory into HBM (vsb_group_append_quant_chunk), row-sharded
@@ -65,6 +67,7 @@ typedef struct {
     sqlite3_vtab base;
     sqlite3 *db;
     vcontext *ctx;
+    int filtered;                  /* the *_filtered modules: one more hidden column (rowids) before the visible ones */
 } scan_vtab;
 
 typedef struct {
@@ -1115,44 +1118,51 @@ static int stage_full_column(scan_vtab *vt, vcolumn *v) {
 }
 
 /* ------------------------------------------------------------------------------------------------ virtual tables */
-static int vt_connect(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) { /* :1828-1842 */
-    (void)argc; (void)argv; (void)err;
-    int rc = sqlite3_declare_vtab(db, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, id, distance);");
+static int connect_vtab(sqlite3 *db, void *aux, const char *schema, int filtered, sqlite3_vtab **out) {
+    int rc = sqlite3_declare_vtab(db, schema);
     if (rc != SQLITE_OK) return rc;
     scan_vtab *vt = (scan_vtab *)sqlite3_malloc((int)sizeof *vt);
     if (!vt) return SQLITE_NOMEM;
     memset(vt, 0, sizeof *vt);
     vt->db = db;
     vt->ctx = (vcontext *)aux;
+    vt->filtered = filtered;
     *out = &vt->base;
     return SQLITE_OK;
 }
+static int vt_connect(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) { /* :1828-1842 */
+    (void)argc; (void)argv; (void)err;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, id, distance);", 0, out);
+}
+static int vt_connect_filtered(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
+    (void)argc; (void)argv; (void)err;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, rowids hidden, id, distance);", 1, out);
+}
 static int vt_disconnect(sqlite3_vtab *p) { sqlite3_free(p); return SQLITE_OK; }
 
-static void map_constraints(sqlite3_index_info *ii) { /* hidden column N -> argv[N] (:1856-1878) */
+static void map_constraints(sqlite3_vtab *t, sqlite3_index_info *ii) { /* hidden column N -> argv[N] (:1856-1878) */
+    const int last_hidden = COL_MEMIDX + ((scan_vtab *)t)->filtered;
     for (int i = 0; i < ii->nConstraint; ++i) {
         const struct sqlite3_index_constraint *c = &ii->aConstraint[i];
         if (!c->usable || c->op != SQLITE_INDEX_CONSTRAINT_EQ) continue;
-        if (c->iColumn >= COL_TBL && c->iColumn <= COL_MEMIDX) {
+        if (c->iColumn >= COL_TBL && c->iColumn <= last_hidden) {
             ii->aConstraintUsage[i].argvIndex = c->iColumn + 1;
             ii->aConstraintUsage[i].omit = 1;
         }
     }
 }
 static int vt_best_index(sqlite3_vtab *t, sqlite3_index_info *ii) { /* :1850-1880 */
-    (void)t;
     ii->estimatedCost = 1.0;
     ii->estimatedRows = 100;
     ii->orderByConsumed = 1;
     ii->idxNum = 1;
-    map_constraints(ii);
+    map_constraints(t, ii);
     return SQLITE_OK;
 }
 static int vt_best_index_stream(sqlite3_vtab *t, sqlite3_index_info *ii) { /* :2245-2275 */
-    (void)t;
     ii->estimatedCost = 1e8;
     ii->estimatedRows = 100000;
-    map_constraints(ii);
+    map_constraints(t, ii);
     return SQLITE_OK;
 }
 static int vt_open(sqlite3_vtab *t, sqlite3_vtab_cursor **out) {
@@ -1184,6 +1194,7 @@ static sqlite3_int64 cur_id(const scan_cursor *c) {
 }
 static int vt_column(sqlite3_vtab_cursor *cur, sqlite3_context *ctx, int col) { /* :2006-2014 */
     scan_cursor *c = (scan_cursor *)cur;
+    col -= ((scan_vtab *)cur->pVtab)->filtered;
     if (col == COL_ID) sqlite3_result_int64(ctx, cur_id(c));
     else if (col == COL_DISTANCE) sqlite3_result_double(ctx, c->streaming ? (c->spos < 0 ? 0.0 : (double)c->sdist[c->spos]) : c->dist[c->row_index]);
     return SQLITE_OK;
@@ -1230,18 +1241,46 @@ static int resident_index(scan_vtab *vt, vcolumn *v, const char *tbl, const char
     return SQLITE_OK;
 }
 
-/* common xFilter (vCursorFilterCommon, :1723-1826) */
+/* ------------------------------------------------------------------------------------------------ filtered scans
+ * vector_*_scan_filtered(tbl, col, vector, k, rowids) / vector_*_scan_batch_filtered(tbl, col, vectors, k, rowids): the k nearest
+ * among the rows whose rowid is in `rowids`, a BLOB of little-endian int64 (vector_rowid_set builds it).  No counterpart in the
+ * reference; the results are those of the unfiltered function over a table holding only those rows (vsb_group_scan_topk_filtered). */
+static int check_rowids_arg(scan_vtab *vt, const char *fname, sqlite3_value *arg) {
+    const int t = sqlite3_value_type(arg);
+    if (t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument 5 must be of type BLOB (got %s).", fname, sql_type_name(t));
+    if (sqlite3_value_bytes(arg) % 8 != 0)
+        return vtab_error(&vt->base, "%s: rowids has %d bytes, expected a multiple of 8 (int64 rowids).", fname, sqlite3_value_bytes(arg));
+    return SQLITE_OK;
+}
+
+/* the rows of the resident column ix whose rowid is in the (checked) rowids BLOB, as the row bitmap of the scan (sqlite3_free it) */
+static int rowids_bitmap(scan_vtab *vt, const char *fname, sqlite3_value *arg, vsb_group *ix, uint32_t **out) {
+    const sqlite3_int64 n = sqlite3_value_bytes(arg) / 8, rows = vsb_group_rows(ix);
+    int64_t *ids = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(int64_t));
+    uint32_t *bits = (uint32_t *)sqlite3_malloc64((sqlite3_uint64)((rows + 31) / 32 + 1) * sizeof(uint32_t));
+    int rc = (ids && bits) ? SQLITE_OK : SQLITE_NOMEM;
+    if (rc == SQLITE_OK && n > 0) memcpy(ids, sqlite3_value_blob(arg), (size_t)n * sizeof(int64_t));   /* little-endian host */
+    if (rc == SQLITE_OK && vsb_group_rowid_bitmap(ix, ids, n, bits) < 0) rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
+    sqlite3_free(ids);
+    if (rc != SQLITE_OK) { sqlite3_free(bits); return rc; }
+    *out = bits;
+    return SQLITE_OK;
+}
+
+/* common xFilter (vCursorFilterCommon, :1723-1826); filtered: the *_filtered twin, whose 5th argument is the rowid set */
 static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized, int streaming) {
     scan_cursor *c = (scan_cursor *)cur;
     scan_vtab *vt = (scan_vtab *)cur->pVtab;
+    const int filtered = vt->filtered;
     c->streaming = streaming;
-    const int nargs = streaming ? 3 : 4;
+    const int nargs = streaming ? 3 : 4 + filtered;
     if (argc != nargs) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, nargs, argc);
     for (int i = 0; i < argc; ++i) {
         int t = sqlite3_value_type(argv[i]);
         if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 4) { int rc = check_rowids_arg(vt, fname, argv[4]); if (rc != SQLITE_OK) return rc; }
     }
     const char *tbl = (const char *)sqlite3_value_text(argv[0]);
     const char *col = (const char *)sqlite3_value_text(argv[1]);
@@ -1265,6 +1304,7 @@ static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **arg
     int rc = SQLITE_OK;
     vsb_group *ix = 0;
     uint8_t *qq = 0;
+    uint32_t *allow = 0;
     rc = resident_index(vt, v, tbl, col, fname, quantized, &ix);
     if (rc != SQLITE_OK) goto out;
     if (quantized) {
@@ -1298,8 +1338,15 @@ static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **arg
         }
         c->row_index = 0;
         c->row_count = 0;
-        int count = 0;
-        if (vsb_group_scan_topk(ix, v->metric, query, 1, k, (int64_t *)c->ids, c->dist, &count, &c->max_index) != VSB_OK) {
+        int count = 0, src;
+        if (filtered) {
+            rc = rowids_bitmap(vt, fname, argv[4], ix, &allow);
+            if (rc != SQLITE_OK) goto out;
+            src = vsb_group_scan_topk_filtered(ix, v->metric, query, 1, k, allow, vsb_group_rows(ix), (int64_t *)c->ids, c->dist, &count, &c->max_index);
+        } else {
+            src = vsb_group_scan_topk(ix, v->metric, query, 1, k, (int64_t *)c->ids, c->dist, &count, &c->max_index);
+        }
+        if (src != VSB_OK) {
             rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
             goto out;
         }
@@ -1308,6 +1355,7 @@ static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **arg
 out:
     sqlite3_free(owned);
     sqlite3_free(qq);
+    sqlite3_free(allow);
     return rc;
 }
 static int vt_filter_full(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan", 0, 0); }
@@ -1326,15 +1374,11 @@ enum { BCOL_QUERY = 4, BCOL_ID = 5, BCOL_DISTANCE = 6 };
 
 static int vt_connect_batch(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
     (void)argc; (void)argv; (void)err;
-    int rc = sqlite3_declare_vtab(db, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, query, id, distance);");
-    if (rc != SQLITE_OK) return rc;
-    scan_vtab *vt = (scan_vtab *)sqlite3_malloc((int)sizeof *vt);
-    if (!vt) return SQLITE_NOMEM;
-    memset(vt, 0, sizeof *vt);
-    vt->db = db;
-    vt->ctx = (vcontext *)aux;
-    *out = &vt->base;
-    return SQLITE_OK;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, query, id, distance);", 0, out);
+}
+static int vt_connect_batch_filtered(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
+    (void)argc; (void)argv; (void)err;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, rowids hidden, query, id, distance);", 1, out);
 }
 static void batch_skip_empty(scan_cursor *c) {
     while (c->bq < c->bnq && c->bj >= c->bcounts[c->bq]) { ++c->bq; c->bj = 0; }
@@ -1352,6 +1396,7 @@ static int vt_eof_batch(sqlite3_vtab_cursor *cur) {
 static int vt_column_batch(sqlite3_vtab_cursor *cur, sqlite3_context *ctx, int col) {
     scan_cursor *c = (scan_cursor *)cur;
     const size_t at = (size_t)c->bq * (size_t)c->bk + (size_t)c->bj;
+    col -= ((scan_vtab *)cur->pVtab)->filtered;
     if (col == BCOL_QUERY) sqlite3_result_int(ctx, c->bq);
     else if (col == BCOL_ID) sqlite3_result_int64(ctx, c->ids[at]);
     else if (col == BCOL_DISTANCE) sqlite3_result_double(ctx, c->dist[at]);
@@ -1365,14 +1410,16 @@ static int vt_rowid_batch(sqlite3_vtab_cursor *cur, sqlite3_int64 *out) {
 static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized) {
     scan_cursor *c = (scan_cursor *)cur;
     scan_vtab *vt = (scan_vtab *)cur->pVtab;
+    const int filtered = vt->filtered;
     c->batch = 1;
     c->bnq = 0; c->bq = 0; c->bj = 0;
-    if (argc != 4) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, 4, argc);
+    if (argc != 4 + filtered) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, 4 + filtered, argc);
     for (int i = 0; i < argc; ++i) {
         int t = sqlite3_value_type(argv[i]);
         if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 4) { int rc = check_rowids_arg(vt, fname, argv[4]); if (rc != SQLITE_OK) return rc; }
     }
     const char *tbl = (const char *)sqlite3_value_text(argv[0]);
     const char *col = (const char *)sqlite3_value_text(argv[1]);
@@ -1393,6 +1440,7 @@ static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv
     }
     int rc = SQLITE_OK;
     uint8_t *qq = 0;
+    uint32_t *allow = 0;
     vsb_group *ix = 0;
     if (bytes <= 0 || bytes % need != 0) {
         rc = vtab_error(&vt->base, "%s: input has %d bytes, expected a positive multiple of %d (dimension %d).", fname, bytes, need, v->dim);
@@ -1417,7 +1465,15 @@ static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv
         c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)k * sizeof(double));
         c->bcounts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
         if (!c->ids || !c->dist || !c->bcounts) { rc = SQLITE_NOMEM; goto out; }
-        if (vsb_group_scan_topk(ix, v->metric, queries, nq, k, (int64_t *)c->ids, c->dist, c->bcounts, 0) != VSB_OK) {
+        int src;
+        if (filtered) {
+            rc = rowids_bitmap(vt, fname, argv[4], ix, &allow);
+            if (rc != SQLITE_OK) goto out;
+            src = vsb_group_scan_topk_filtered(ix, v->metric, queries, nq, k, allow, vsb_group_rows(ix), (int64_t *)c->ids, c->dist, c->bcounts, 0);
+        } else {
+            src = vsb_group_scan_topk(ix, v->metric, queries, nq, k, (int64_t *)c->ids, c->dist, c->bcounts, 0);
+        }
+        if (src != VSB_OK) {
             rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
             goto out;
         }
@@ -1428,6 +1484,7 @@ static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv
 out:
     sqlite3_free(owned);
     sqlite3_free(qq);
+    sqlite3_free(allow);
     return rc;
 }
 static int vt_filter_full_batch(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_full_scan_batch", 0); }
@@ -1436,14 +1493,58 @@ static sqlite3_module mod_full_batch = {0, 0, vt_connect_batch, vt_best_index, v
                                         vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 static sqlite3_module mod_quant_batch = {0, 0, vt_connect_batch, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch, vt_next_batch,
                                          vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+static int vt_filter_full_batch_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_full_scan_batch_filtered", 0); }
+static int vt_filter_quant_batch_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_quantize_scan_batch_filtered", 1); }
+static sqlite3_module mod_full_batch_filtered = {0, 0, vt_connect_batch_filtered, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_full_batch_filtered,
+                                                 vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+static sqlite3_module mod_quant_batch_filtered = {0, 0, vt_connect_batch_filtered, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch_filtered,
+                                                  vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 
-#define SCAN_MODULE(NAME, BEST, FILTER)                                                                                      \
-    static sqlite3_module NAME = {0, 0, vt_connect, BEST, vt_disconnect, 0, vt_open, vt_close, FILTER, vt_next, vt_eof, \
+#define SCAN_MODULE(NAME, CONNECT, BEST, FILTER)                                                                          \
+    static sqlite3_module NAME = {0, 0, CONNECT, BEST, vt_disconnect, 0, vt_open, vt_close, FILTER, vt_next, vt_eof, \
                                   vt_column, vt_rowid, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}
-SCAN_MODULE(mod_full, vt_best_index, vt_filter_full);
-SCAN_MODULE(mod_quant, vt_best_index, vt_filter_quant);
-SCAN_MODULE(mod_full_stream, vt_best_index_stream, vt_filter_full_stream);
-SCAN_MODULE(mod_quant_stream, vt_best_index_stream, vt_filter_quant_stream);
+static int vt_filter_full_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan_filtered", 0, 0); }
+static int vt_filter_quant_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan_filtered", 1, 0); }
+SCAN_MODULE(mod_full, vt_connect, vt_best_index, vt_filter_full);
+SCAN_MODULE(mod_quant, vt_connect, vt_best_index, vt_filter_quant);
+SCAN_MODULE(mod_full_stream, vt_connect, vt_best_index_stream, vt_filter_full_stream);
+SCAN_MODULE(mod_quant_stream, vt_connect, vt_best_index_stream, vt_filter_quant_stream);
+SCAN_MODULE(mod_full_filtered, vt_connect_filtered, vt_best_index, vt_filter_full_filtered);
+SCAN_MODULE(mod_quant_filtered, vt_connect_filtered, vt_best_index, vt_filter_quant_filtered);
+
+/* vector_rowid_set(x): aggregate of the non-NULL x as the rowids BLOB of the *_filtered modules (int64, host byte order =
+ * little-endian), e.g. (SELECT vector_rowid_set(rowid) FROM docs WHERE lang = 'en'); no rows give an empty BLOB */
+typedef struct {
+    int64_t *v;
+    sqlite3_int64 n, cap;
+} rowid_set;
+static void rowid_set_step(sqlite3_context *ctx, int argc, sqlite3_value **argv) {
+    (void)argc;
+    if (sqlite3_value_type(argv[0]) == SQLITE_NULL) return;
+    rowid_set *s = (rowid_set *)sqlite3_aggregate_context(ctx, (int)sizeof *s);
+    if (!s) { sqlite3_result_error_code(ctx, SQLITE_NOMEM); return; }
+    if (s->n == s->cap) {
+        const sqlite3_int64 cap = s->cap ? 2 * s->cap : 1024;
+        int64_t *v = (int64_t *)sqlite3_malloc64((sqlite3_uint64)cap * sizeof(int64_t));
+        if (!v) { sqlite3_result_error_code(ctx, SQLITE_NOMEM); return; }
+        if (s->n) memcpy(v, s->v, (size_t)s->n * sizeof(int64_t));
+        sqlite3_free(s->v);
+        s->v = v;
+        s->cap = cap;
+    }
+    s->v[s->n++] = (int64_t)sqlite3_value_int64(argv[0]);
+}
+static void rowid_set_final(sqlite3_context *ctx) {
+    rowid_set *s = (rowid_set *)sqlite3_aggregate_context(ctx, 0);
+    if (!s || s->n == 0) {
+        sqlite3_result_blob(ctx, "", 0, SQLITE_STATIC);
+    } else if (s->n > INT32_MAX / 8) {
+        fn_error(ctx, SQLITE_ERROR,"vector_rowid_set: %lld rowids do not fit in one BLOB.", (long long)s->n);
+    } else {
+        sqlite3_result_blob(ctx, s->v, (int)(s->n * 8), SQLITE_TRANSIENT);
+    }
+    if (s) sqlite3_free(s->v);
+}
 
 /* ------------------------------------------------------------------------------------------------ entry point */
 __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char **err, const sqlite3_api_routines *api) { /* :2555-2638 */
@@ -1478,5 +1579,11 @@ __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char
     /* additions (not in the reference): batched scans */
     if ((rc = sqlite3_create_module(db, "vector_full_scan_batch", &mod_full_batch, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch", &mod_quant_batch, ctx)) != SQLITE_OK) return rc;
+    /* additions: filtered scans and the aggregate that builds their rowid set */
+    if ((rc = sqlite3_create_module(db, "vector_full_scan_filtered", &mod_full_filtered, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_filtered", &mod_quant_filtered, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_full_scan_batch_filtered", &mod_full_batch_filtered, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch_filtered", &mod_quant_batch_filtered, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_function(db, "vector_rowid_set", 1, SQLITE_UTF8, ctx, 0, rowid_set_step, rowid_set_final)) != SQLITE_OK) return rc;
     return SQLITE_OK;
 }

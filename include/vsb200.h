@@ -117,6 +117,26 @@ VSB_API int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *querie
  * on first use and rebuilt after an append. */
 VSB_API int64_t vsb_index_rowid_bitmap(vsb_index *ix, const int64_t *rowids, int64_t n, uint32_t *out_bits);
 
+/* ---- range search: every row closer than a radius (no counterpart in the reference, whose stream modules answer it as
+ * SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < r ORDER BY distance) --------------------------------------
+ * For query b (nq HOST queries, as for vsb_scan_topk) the result is every row with (double)d < radius[b], d being the distance
+ * vsb_scan_topk reports for that row (after the nearly-zero clamp); strict, so a NaN radius or distance never qualifies and
+ * radius +INF selects every row with a finite (or -INF) distance.  Rows come ordered by ascending distance, equal distances in
+ * scan order; distances are widened to double.  allow (may be NULL: every row) is the row bitmap of vsb_scan_topk_filtered,
+ * nbits = vsb_index_rows.  A single query is one range scan into a list of the index (65536 pairs at first); a larger result is
+ * counted exactly, the list grows to that count and a second pass collects it (vsb_index_stat "range_passes"): nothing is ever
+ * truncated.  nq >= 16 queries under the conditions of vsb_scan_topk's batch path (k aside) run as one batch on the tensor cores
+ * (L1: the CUDA-core batch kernel) with the exact refine: int8 / uint8 results equal nq single calls bit for bit, fp results
+ * agree within the refine's rounding.  A query that keeps more than 16384 rows in a batch is answered alone ("range_query_fallbacks"),
+ * and a batch whose candidate log overflows is answered query by query ("range_batch_fallbacks"; "range_batches" counts the
+ * others).  Streamed indexes scan window by window.  *out receives a result owned by the caller (vsb_range_free); vsb_range_get
+ * borrows query q's arrays from it. */
+typedef struct vsb_range vsb_range;
+VSB_API int vsb_scan_range(vsb_index *ix, int metric, const void *queries, int nq, const double *radius /* [nq] */,
+                           const uint32_t *allow /* NULL: every row */, int64_t nbits, vsb_range **out);
+VSB_API int vsb_range_get(const vsb_range *r, int q, const int64_t **rowids, const double **dist, int64_t *count); /* borrowed until free */
+VSB_API void vsb_range_free(vsb_range *r);
+
 /* every row's distance for one query, in scan order (what the *_stream modules compute one row per
  * xNext, src/sqlite-vector.c:1901-1998).  out_dist has vsb_index_rows() floats; out_rowids may be NULL. */
 VSB_API int vsb_scan_all(vsb_index *ix, int metric, const void *query, float *out_dist, int64_t *out_rowids);
@@ -228,6 +248,10 @@ VSB_API int vsb_group_scan_all(vsb_group *g, int metric, const void *query, floa
 VSB_API int vsb_group_scan_topk_filtered(vsb_group *g, int metric, const void *queries, int nq, int k, const uint32_t *allow, int64_t nbits,
                                          int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
 VSB_API int64_t vsb_group_rowid_bitmap(vsb_group *g, const int64_t *rowids, int64_t n, uint32_t *out_bits);
+/* vsb_scan_range over the group's global scan order (nbits = vsb_group_rows): every shard scans its rows, the shards' lists are
+ * merged by (distance, global scan row) */
+VSB_API int vsb_group_scan_range(vsb_group *g, int metric, const void *queries, int nq, const double *radius, const uint32_t *allow,
+                                 int64_t nbits, vsb_range **out);
 VSB_API int vsb_group_gpus(const vsb_group *g);
 VSB_API int64_t vsb_group_rows(const vsb_group *g);
 VSB_API vsb_index *vsb_group_shard(vsb_group *g, int shard); /* borrowed; for statistics */
@@ -252,7 +276,9 @@ VSB_API void vsb_quantizer_free(vsb_quantizer *qz);
 
 VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row on the device (multiple of 16) */
 /* counters since creation; name in {"queries","survivors","last_survivors","fallbacks","filter_blocks","fetch_bytes","slots","batches","batch_cands","batch_kept","tc_us","tc_rows","batch_us","stream_bytes","stream_us",
- * "sms" (scan CTAs per launch)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * "sms" (scan CTAs per launch), "range_pairs" (rows returned by range queries), "range_passes" (range queries that took a second
+ * pass), "range_host_sorts" (range results too long for the GPU sort, ordered on the host), "range_batches",
+ * "range_batch_fallbacks", "range_query_fallbacks" (see vsb_scan_range)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
  * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */

@@ -50,6 +50,9 @@ _SIGNATURES = {
     "vsb_scan_topk": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "vsb_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vsb_index_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
+    "vsb_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
+    "vsb_range_get": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_i64)]),
+    "vsb_range_free": (None, [_vp]),
     "vsb_scan_all": (_i, [_vp, _i, _vp, _vp, _vp]),
     "vsb_scan_candidates": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _vp]),
     "vsb_replay_topk": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
@@ -78,6 +81,7 @@ _SIGNATURES = {
     "vsb_group_scan_all": (_i, [_vp, _i, _vp, _vp, _vp]),
     "vsb_group_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vsb_group_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
+    "vsb_group_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_group_gpus": (_i, [_vp]),
     "vsb_group_rows": (_i64, [_vp]),
     "vsb_group_shard": (_vp, [_vp, _i]),
@@ -208,6 +212,32 @@ def _topk(eng: "Engine", call, queries: np.ndarray, k: int, max_index: int | Non
     return (out, mi.value) if max_index is not None else out
 
 
+def _range(eng: "Engine", fn, h, rows: int, metric: int, queries: np.ndarray, radius, allow):
+    """the range entry points: fn(handle, metric, queries, nq, radius, allow, nbits, &result) -> rc; one (rowids, distances) pair
+    per query, rows ordered by ascending distance (equal distances in scan order)"""
+    q = np.ascontiguousarray(queries)
+    q2 = q.reshape(-1, q.shape[-1]) if q.ndim > 1 else q.reshape(1, -1)
+    nq = q2.shape[0]
+    r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, dtype=np.float64), (nq,)))
+    bits = None if allow is None else _allow_words(allow, rows)
+    res = _vp()
+    eng.check(fn(h, metric, _ptr(q2), nq, _ptr(r), _ptr(bits), rows if bits is not None else 0, C.byref(res)))
+    out = []
+    try:
+        for b in range(nq):
+            ids, dist, cnt = _vp(), _vp(), _i64()
+            eng.check(eng.lib.vsb_range_get(res, b, C.byref(ids), C.byref(dist), C.byref(cnt)))
+            n = int(cnt.value)
+            if n == 0:
+                out.append((np.zeros(0, np.int64), np.zeros(0, np.float64)))
+                continue
+            out.append((np.ctypeslib.as_array(C.cast(ids, C.POINTER(C.c_int64)), (n,)).copy(),
+                        np.ctypeslib.as_array(C.cast(dist, C.POINTER(C.c_double)), (n,)).copy()))
+    finally:
+        eng.lib.vsb_range_free(res)
+    return out
+
+
 def _rowid_bitmap(eng: "Engine", fn, h, rows: int, rowids) -> tuple[np.ndarray, int]:
     rid = np.ascontiguousarray(rowids, dtype=np.int64).reshape(-1)
     bits = np.zeros(max((rows + 31) // 32, 1), dtype=np.uint32)
@@ -289,6 +319,11 @@ class Index:
         return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
                                                                                                ids, dist, counts, mi),
                      queries, k, max_index, as_arrays)
+
+    def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
+        """every row with distance < radius (vsb_scan_range), for one query or a batch; radius: one value or one per query, allow:
+        None, a boolean mask over the scan-order rows or a uint32 row bitmap.  Returns one (rowids, distances) pair per query"""
+        return _range(self.eng, self.eng.lib.vsb_scan_range, self.h, self.rows, metric, queries, radius, allow)
 
     def rowid_bitmap(self, rowids) -> tuple[np.ndarray, int]:
         """(row bitmap of the rows whose rowid is in `rowids`, number of such rows) (vsb_index_rowid_bitmap)"""
@@ -558,6 +593,10 @@ class Group:
         return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_group_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
                                                                                                      ids, dist, counts, mi),
                      queries, k, max_index, False)
+
+    def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
+        """Index.scan_range over the group's global scan order (vsb_group_scan_range)"""
+        return _range(self.eng, self.eng.lib.vsb_group_scan_range, self.h, self.rows, metric, queries, radius, allow)
 
     def rowid_bitmap(self, rowids) -> tuple[np.ndarray, int]:
         """Index.rowid_bitmap over the group's global scan order (vsb_group_rowid_bitmap)"""

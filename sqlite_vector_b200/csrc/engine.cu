@@ -207,23 +207,41 @@ struct vsb_index {
     // need; an append changes n and so rebuilds it
     std::vector<std::pair<int64_t, long long>> rowid_sorted;
     long long rowid_rows = -1;
+    // range search (vsb_scan_range): the pair list the range scan appends to, its counter, and the counter's host copy; the list
+    // starts at kRangeCap0 pairs and grows to the exact count of a query that needed more
+    DeviceBuf<uint2> d_range;
+    long long range_cap = 0;
+    DeviceBuf<unsigned> d_range_count;
+    HostBuf<unsigned> h_range_count;
+    long long st_range_pairs = 0, st_range_passes = 0, st_range_host_sorts = 0;
+    long long st_range_batches = 0, st_range_batch_fallbacks = 0, st_range_query_fallbacks = 0;
+};
+
+// result of a range call (vsb_scan_range): per query, rowids and distances in result order
+struct vsb_range {
+    std::vector<std::vector<int64_t>> ids;
+    std::vector<std::vector<double>> dist;
 };
 
 namespace {
 
 // ------------------------------------------------------------------ kernel dispatch
 using ScanFn = void (*)(const ScanParams);
-template <int VT, int MC, bool D>
-ScanFn fn_of() { return scan_kernel<VT, MC, D>; }
+template <int VT, int MC, bool D, bool R>
+ScanFn fn_of() {
+    if constexpr (R) return scan_range_kernel<VT, MC, D>;
+    else return scan_kernel<VT, MC, D>;
+}
 
-ScanFn pick_kernel(int vtype, int mc, bool direct) {
+template <bool R>
+ScanFn pick_kernel_of(int vtype, int mc, bool direct) {
 #define ROW(VT)                                                                                                   \
     case VT:                                                                                                      \
         switch (mc) {                                                                                             \
-        case MC_L2: return direct ? fn_of<VT, MC_L2, true>() : fn_of<VT, MC_L2, false>();                         \
-        case MC_COS: return direct ? fn_of<VT, MC_COS, true>() : fn_of<VT, MC_COS, false>();                      \
-        case MC_DOT: return direct ? fn_of<VT, MC_DOT, true>() : fn_of<VT, MC_DOT, false>();                      \
-        case MC_L1: return direct ? fn_of<VT, MC_L1, true>() : fn_of<VT, MC_L1, false>();                         \
+        case MC_L2: return direct ? fn_of<VT, MC_L2, true, R>() : fn_of<VT, MC_L2, false, R>();                   \
+        case MC_COS: return direct ? fn_of<VT, MC_COS, true, R>() : fn_of<VT, MC_COS, false, R>();                \
+        case MC_DOT: return direct ? fn_of<VT, MC_DOT, true, R>() : fn_of<VT, MC_DOT, false, R>();                \
+        case MC_L1: return direct ? fn_of<VT, MC_L1, true, R>() : fn_of<VT, MC_L1, false, R>();                   \
         }                                                                                                         \
         break;
     switch (vtype) {
@@ -231,6 +249,10 @@ ScanFn pick_kernel(int vtype, int mc, bool direct) {
     }
 #undef ROW
     return nullptr;
+}
+// range: the range-mode instantiation (vsb_scan_range)
+ScanFn pick_kernel(int vtype, int mc, bool direct, bool range = false) {
+    return range ? pick_kernel_of<true>(vtype, mc, direct) : pick_kernel_of<false>(vtype, mc, direct);
 }
 
 int metric_class(int metric, int *root) {
@@ -872,6 +894,161 @@ int submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_s
     return VSB_OK;
 }
 
+// ------------------------------------------------------------------ range search (vsb_scan_range, DESIGN §3.10)
+constexpr long long kRangeCap0 = 1 << 16;   // pairs of the first pass of a range query (512 KB); a larger result takes a second pass
+
+// the float threshold of a double radius: the smallest float t with (double)t >= r, so that for every float d, d < t iff
+// (double)d < r (the comparison `distance < r` of SQL over the float widened to double).  NaN: no float qualifies (-INF).
+float range_threshold(double r) {
+    if (r != r) return -INFINITY;
+    float t = (float)r;
+    if ((double)t < r) t = std::nextafter(t, INFINITY);
+    return t;
+}
+
+// the pair list holds at least cap pairs (grown, never shrunk; range calls are synchronous, no launch reads the old list)
+int ensure_range(vsb_index *ix, long long cap) {
+    if (!ix->d_range_count) {
+        DeviceBuf<unsigned> d;
+        HostBuf<unsigned> h;
+        CU(d.alloc(sizeof(unsigned)));
+        CU(h.alloc(sizeof(unsigned)));
+        ix->d_range_count = std::move(d);
+        ix->h_range_count = std::move(h);
+        ix->dev_bytes += sizeof(unsigned);
+    }
+    if (cap <= ix->range_cap) return VSB_OK;
+    DeviceBuf<uint2> d;
+    CU(d.alloc(sizeof(uint2) * (size_t)cap));
+    ix->dev_bytes += sizeof(uint2) * (size_t)(cap - ix->range_cap);
+    ix->d_range = std::move(d);
+    ix->range_cap = cap;
+    return VSB_OK;
+}
+
+// one range-mode scan over rows [0, n) of vec, whose first row is shard row r0, appending to the pair list on ix->stream
+int launch_range(vsb_index *ix, int metric, const uint8_t *d_query, float t, const uint8_t *vec, long long n, long long r0) {
+    int root = 0;
+    const int mc = metric_class(metric, &root);
+    if (mc < 0) return fail(VSB_EINVAL, "unknown distance metric %d", metric);
+    const Plan pl = make_plan(ix, 0);
+    ScanFn fn = pick_kernel(ix->vtype, mc, pl.direct, true);
+    if (!fn) return fail(VSB_EINVAL, "unsupported vector type %d", ix->vtype);
+    CU((cudaError_t)set_smem_limit((const void *)fn, pl.smem));
+    ScanParams p{};
+    p.vec = vec;
+    p.n = n;
+    p.pitch = ix->pitch;
+    p.nc = ix->pitch / 16;
+    p.log2P = pl.log2P;
+    p.wtile_bytes = pl.wtile_bytes;
+    p.nsw = pl.nsw;
+    p.root = root;
+    p.query = d_query;
+    p.allow = ix->flt_d;
+    p.allow_base = r0;
+    p.range_t = t;
+    p.range_pairs = ix->d_range;
+    p.range_count = ix->d_range_count;
+    p.range_cap = ix->range_cap;
+    p.range_row_base = (unsigned)r0;
+    fn<<<ix->num_sms, kThreads, pl.smem, ix->stream>>>(p);
+    CU(cudaGetLastError());
+    ++g_launches;
+    ix->last_log2p = pl.log2P; ix->last_nsw = pl.nsw; ix->last_direct = pl.direct ? 1 : 0;
+    return VSB_OK;
+}
+
+// the float order of distance bits as an unsigned order (fkey of scan_kernels.cuh, on the host)
+inline uint32_t dist_order_key(uint32_t bits) { return (bits & 0x80000000u) ? ~bits : (bits | 0x80000000u); }
+
+// orders `count` pairs (row, distance bits) by (distance, row) on the host: the lists longer than range_sort_kernel takes
+void range_sort_host(uint2 *pairs, size_t count) {
+    std::sort(pairs, pairs + count, [](const uint2 &a, const uint2 &b) {
+        const uint32_t ka = dist_order_key(a.y), kb = dist_order_key(b.y);
+        return ka != kb ? ka < kb : a.x < b.x;
+    });
+}
+
+// one query staged at d_query: every eligible row of ix with distance < r, as (shard row, distance bits) ordered by (distance,
+// row).  The first pass appends into kRangeCap0 pairs; when the counter says more, the list grows to the exact count and the
+// scan runs once more.  A streamed index scans window by window into the same list.
+int range_query(vsb_index *ix, int metric, const uint8_t *d_query, double r, std::vector<uint2> &out) {
+    out.clear();
+    const float t = range_threshold(r);
+    if (ix->n == 0 || t == -INFINITY) return VSB_OK;            // nothing is below -INF (and NaN radii select nothing)
+    int rc = ensure_range(ix, kRangeCap0);
+    if (rc) return rc;
+    unsigned cnt = 0;
+    for (int pass = 0;; ++pass) {
+        CU(cudaMemsetAsync(ix->d_range_count, 0, sizeof(unsigned), ix->stream));
+        if (ix->streamed) {
+            rc = stream_windows(ix, 2,
+                [&](long long w, const uint8_t *vec, long long rows, int) { return launch_range(ix, metric, d_query, t, vec, rows, w * ix->win_rows); },
+                [&](long long, long long, long long, int) { return (int)VSB_OK; });
+        } else {
+            rc = launch_range(ix, metric, d_query, t, ix->d_vec, ix->n, 0);
+        }
+        if (rc) return rc;
+        CU(cudaMemcpyAsync(ix->h_range_count, ix->d_range_count, sizeof(unsigned), cudaMemcpyDeviceToHost, ix->stream));
+        CU(cudaStreamSynchronize(ix->stream));
+        cnt = *ix->h_range_count;
+        if ((long long)cnt <= ix->range_cap) break;
+        if (pass > 0) return fail(VSB_ECUDA, "range scan: %u pairs after growing the list to %lld", cnt, ix->range_cap);
+        ix->st_range_passes++;
+        rc = ensure_range(ix, (long long)cnt);
+        if (rc) return rc;
+    }
+    if (cnt >= 2 && cnt <= (unsigned)kRangeSortCap) {
+        size_t n2 = 2;
+        while (n2 < cnt) n2 <<= 1;
+        const size_t smem = sizeof(unsigned long long) * n2;
+        CU((cudaError_t)set_smem_limit((const void *)range_sort_kernel, smem));
+        RangeSortParams sp{ix->d_range, ix->d_range_count, 0, nullptr, nullptr};
+        range_sort_kernel<<<1, kRangeSortThreads, smem, ix->stream>>>(sp);
+        CU(cudaGetLastError());
+        ++g_launches;
+    }
+    out.resize(cnt);
+    if (cnt > 0) CU(cudaMemcpyAsync(out.data(), ix->d_range, sizeof(uint2) * (size_t)cnt, cudaMemcpyDeviceToHost, ix->stream));
+    CU(cudaStreamSynchronize(ix->stream));
+    if (cnt > (unsigned)kRangeSortCap) {
+        ix->st_range_host_sorts++;
+        range_sort_host(out.data(), out.size());
+    }
+    ix->st_range_pairs += cnt;
+    return VSB_OK;
+}
+
+// checks the arguments of a range call and allocates its result
+int range_begin(int metric, const void *queries, int nq, const double *radius, vsb_range **out) {
+    if (!out) return fail(VSB_EINVAL, "out is null");
+    *out = nullptr;
+    if (nq < 0 || (nq > 0 && (!queries || !radius))) return fail(VSB_EINVAL, "bad range arguments");
+    int root = 0;
+    if (metric_class(metric, &root) < 0) return fail(VSB_EINVAL, "unknown distance metric %d", metric);
+    vsb_range *r = new (std::nothrow) vsb_range();
+    if (!r) return fail(VSB_ENOMEM, "out of host memory");
+    r->ids.resize((size_t)nq);
+    r->dist.resize((size_t)nq);
+    *out = r;
+    return VSB_OK;
+}
+
+// query q's n result rows into r: at(i) -> (rowid, distance bits) of row i in result order
+template <class At>
+void range_put(vsb_range *r, int q, size_t n, At at) {
+    r->ids[(size_t)q].resize(n);
+    r->dist[(size_t)q].resize(n);
+    for (size_t i = 0; i < n; ++i) {
+        const std::pair<int64_t, uint32_t> e = at(i);
+        float d;
+        memcpy(&d, &e.second, 4);
+        r->ids[(size_t)q][i] = e.first;
+        r->dist[(size_t)q][i] = (double)d;
+    }
+}
+
 }  // namespace
 
 #include "batch_host.inc"
@@ -1143,6 +1320,12 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "plan_log2p")) return ix->last_log2p;
     if (!strcmp(name, "plan_nsw")) return ix->last_nsw;
     if (!strcmp(name, "plan_direct")) return ix->last_direct;
+    if (!strcmp(name, "range_pairs")) return ix->st_range_pairs;
+    if (!strcmp(name, "range_passes")) return ix->st_range_passes;
+    if (!strcmp(name, "range_host_sorts")) return ix->st_range_host_sorts;
+    if (!strcmp(name, "range_batches")) return ix->st_range_batches;
+    if (!strcmp(name, "range_batch_fallbacks")) return ix->st_range_batch_fallbacks;
+    if (!strcmp(name, "range_query_fallbacks")) return ix->st_range_query_fallbacks;
     return -1;
 }
 void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullptr; }
@@ -1198,6 +1381,38 @@ int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *queries, int n
     if (rc) return rc;
     return vsb_scan_topk(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts, max_index);
 }
+
+int vsb_scan_range(vsb_index *ix, int metric, const void *queries, int nq, const double *radius, const uint32_t *allow, int64_t nbits,
+                   vsb_range **out) {
+    if (check_index(ix)) return VSB_EINVAL;
+    int rc = range_begin(metric, queries, nq, radius, out);
+    if (rc) return rc;
+    std::unique_ptr<vsb_range> res(*out);
+    *out = nullptr;
+    FilterScope scope;
+    if (allow) {
+        if (nbits != ix->n) return fail(VSB_EINVAL, "the row bitmap has %lld bits, the index %lld rows", (long long)nbits, ix->n);
+        rc = filter_begin(ix, allow, &scope);
+        if (rc) return rc;
+    }
+    std::vector<std::vector<uint2>> all;
+    rc = range_index(ix, metric, queries, nq, radius, all);
+    if (rc) return rc;
+    for (int b = 0; b < nq; ++b)
+        range_put(res.get(), b, all[(size_t)b].size(), [&](size_t i) { return std::make_pair(rowid_of(ix, all[(size_t)b][i].x), all[(size_t)b][i].y); });
+    *out = res.release();
+    return VSB_OK;
+}
+
+int vsb_range_get(const vsb_range *r, int q, const int64_t **rowids, const double **dist, int64_t *count) {
+    if (!r || q < 0 || (size_t)q >= r->ids.size()) return fail(VSB_EINVAL, "bad range result or query %d", q);
+    if (rowids) *rowids = r->ids[(size_t)q].data();
+    if (dist) *dist = r->dist[(size_t)q].data();
+    if (count) *count = (int64_t)r->ids[(size_t)q].size();
+    return VSB_OK;
+}
+
+void vsb_range_free(vsb_range *r) { delete r; }
 
 int64_t vsb_index_rowid_bitmap(vsb_index *ix, const int64_t *rowids, int64_t n, uint32_t *out_bits) {
     if (check_index(ix)) return VSB_EINVAL;

@@ -65,6 +65,14 @@ struct ScanParams {
     // nullptr: every row is.  An ineligible row never enters a k-list or a log (dist_all is written for every row)
     const uint32_t *allow;
     long long allow_base;      // shard row of vec's first row (a window of a streamed index), else 0
+    // range mode (scan_range_kernel, vsb_scan_range): every eligible row with d < range_t is appended to range_pairs
+    // as (row_base + local row, distance bits) at the position one atomicAdd on *range_count reserves for the warp's ballot; the
+    // counter keeps counting past range_cap, so the host sees the exact size of an overflowed list
+    float range_t;
+    uint2 *range_pairs;        // [range_cap]
+    unsigned *range_count;
+    long long range_cap;
+    unsigned range_row_base;   // shard row of vec's first row, added to the rows written (the windows of a streamed index)
 };
 
 // bit `row` of a row bitmap (bit row & 31 of word row >> 5); nullptr: every row is eligible
@@ -432,9 +440,11 @@ struct SortedList {
 };
 
 // ------------------------------------------------------------------ the scan kernel
-// One launch scans the shard for one query.
-template <int VT, int MC, bool DIRECT>
-__global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm) {
+// One launch scans the shard for one query: scan_kernel (top-k, all distances) and scan_range_kernel (range search) share this
+// body.  RANGE: the fixed threshold prm.range_t instead of the k-lists, hits appended to prm.range_pairs (no log, no lists, no
+// filter_kernel afterwards).
+template <int VT, int MC, bool DIRECT, bool RANGE>
+__device__ __forceinline__ void scan_body(const ScanParams &prm) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem);                    // [kWarps][kMaxStages]
     uint8_t *qs = smem + kBarrierBytes;                                      // [pitch] the query
@@ -489,7 +499,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
     const int r = lane >> prm.log2P, p = lane & (P - 1);
     const int cnt = (prm.nc > p) ? (prm.nc - p + P - 1) >> prm.log2P : 0;  // chunks owned by this lane
     const int i0 = cnt ? (r % cnt) : 0;                                       // rotation: conflict-free LDS.128
-    const bool topk = prm.k > 0;
+    const bool topk = !RANGE && prm.k > 0;
     constexpr bool kFix16 = has_special_policy<VT, MC>();   // rows with NaN / Inf are recomputed from the staged tile: see special_row_distance
     const uint8_t *fix_row = nullptr;
     int fix_stage = 0;
@@ -581,6 +591,20 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
                 if (lane == 0 && pf_it < ntiles) issue(fix_stage);
             }
         }
+        if constexpr (RANGE) {
+            // one reservation per ballot; hit lanes write at their rank among the hits (slots are ordered later, range_sort_kernel)
+            const bool hit = valid && p == 0 && d < prm.range_t && row_allowed(prm.allow, prm.allow_base + row0 + r);
+            const unsigned m = __ballot_sync(0xFFFFFFFFu, hit);
+            if (m != 0u) {
+                unsigned base = 0;
+                if (lane == 0) base = atomicAdd(prm.range_count, (unsigned)__popc(m));
+                base = __shfl_sync(0xFFFFFFFFu, base, 0);
+                const unsigned at = base + (unsigned)__popc(m & ((1u << lane) - 1u));
+                if (hit && (long long)at < prm.range_cap)
+                    prm.range_pairs[at] = make_uint2(prm.range_row_base + (unsigned)(row0 + r), __float_as_uint(d));
+            }
+            continue;
+        }
         if (prm.dist_all != nullptr && valid && p == 0) prm.dist_all[row0 + r] = d;
         if (topk) {
             // rows are visited in scan order (lane order); strict '<' like the reference (:2102, :2145)
@@ -630,6 +654,65 @@ __global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm)
             Lm.offer_sorted(lane, lists_s[w * 32 + lane]);
         }
         prm.lists[(size_t)blockIdx.x * 32 + lane] = Lm.v;
+    }
+}
+
+template <int VT, int MC, bool DIRECT>
+__global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm) { scan_body<VT, MC, DIRECT, false>(prm); }
+template <int VT, int MC, bool DIRECT>
+__global__ void __launch_bounds__(kThreads, 1) scan_range_kernel(const ScanParams prm) { scan_body<VT, MC, DIRECT, true>(prm); }
+
+// ------------------------------------------------------------------ range search: result order
+// One block per query orders that query's (row, distance bits) pairs by (distance, row), in place: a bitonic sort of 64-bit keys
+// (fkey(distance) << 32 | row) in shared memory.  fkey preserves the float order, so negative DOT distances and -INF come first;
+// equal distances keep scan order (the row).  A query with more than kRangeSortCap pairs is left as it is (the host orders it
+// or, in a batch, answers the query alone).
+constexpr int kRangeSortCap = 16384;     // 128 KB of keys
+constexpr int kRangeSortThreads = 1024;
+struct RangeSortParams {
+    uint2 *pairs;             // query q: pairs + q * stride, count[q] entries (row, distance bits)
+    const unsigned *count;    // [gridDim.x]
+    long long stride;
+    uint2 *out;               // nullptr: in place; else query q's ordered pairs go to out + out_off[q] (the batch's compaction)
+    const long long *out_off;
+};
+__global__ void __launch_bounds__(kRangeSortThreads, 1) range_sort_kernel(const RangeSortParams sp) {
+    extern __shared__ __align__(16) unsigned long long rkeys[];
+    const unsigned cnt = sp.count[blockIdx.x];
+    if (cnt > (unsigned)kRangeSortCap) return;
+    uint2 *pr = sp.pairs + (size_t)blockIdx.x * (size_t)sp.stride;
+    uint2 *dst = sp.out ? sp.out + sp.out_off[blockIdx.x] : pr;
+    if (cnt < 2u) {
+        if (cnt == 1u && threadIdx.x == 0 && dst != pr) dst[0] = pr[0];
+        return;
+    }
+    const int n = (int)cnt;
+    int n2 = 2;
+    while (n2 < n) n2 <<= 1;
+    for (int i = threadIdx.x; i < n2; i += blockDim.x) {
+        if (i < n) {
+            const uint2 e = pr[i];
+            rkeys[i] = ((unsigned long long)fkey(__uint_as_float(e.y)) << 32) | e.x;
+        } else {
+            rkeys[i] = ~0ull;
+        }
+    }
+    __syncthreads();
+    for (int size = 2; size <= n2; size <<= 1) {
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+            for (int i = threadIdx.x; i < n2; i += blockDim.x) {
+                const int j = i ^ stride;
+                if (j > i) {
+                    const unsigned long long a = rkeys[i], b = rkeys[j];
+                    if ((a > b) == ((i & size) == 0)) { rkeys[i] = b; rkeys[j] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const unsigned long long key = rkeys[i];
+        dst[i] = make_uint2((unsigned)key, __float_as_uint(funkey((uint32_t)(key >> 32))));
     }
 }
 

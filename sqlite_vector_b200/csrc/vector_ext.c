@@ -7,7 +7,8 @@
  *   table-valued: vector_full_scan, vector_quantize_scan (tbl, col, vector, k),
  *                 vector_full_scan_stream, vector_quantize_scan_stream (tbl, col, vector)
  * additions: vector_*_scan_batch (tbl, col, vectors, k); vector_*_scan_filtered (tbl, col, vector, k, rowids),
- *            vector_*_scan_batch_filtered (tbl, col, vectors, k, rowids) and the aggregate vector_rowid_set(x) that builds rowids
+ *            vector_*_scan_batch_filtered (tbl, col, vectors, k, rowids) and the aggregate vector_rowid_set(x) that builds rowids;
+ *            vector_*_scan_range (tbl, col, vector, radius), vector_*_scan_range_filtered (tbl, col, vector, radius, rowids)
  * Column state, option parsing, JSON vectors, quantization build and the shadow-table chunk format are host
  * C and behave like the reference (citations at each function).  What differs is where a scan runs:
  *   vector_quantize_preload  -> chunks are staged through pinned memory into HBM (vsb_group_append_quant_chunk), row-sharded
@@ -1267,19 +1268,51 @@ static int rowids_bitmap(scan_vtab *vt, const char *fname, sqlite3_value *arg, v
     return SQLITE_OK;
 }
 
+/* range scans (additions): vector_*_scan_range(tbl, col, vector, radius) and the *_range_filtered twins (+ rowids): every row with
+ * distance < radius, ordered by distance, equal distances in scan order (vsb_group_scan_range).  The reference answers this only as
+ * SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < radius ORDER BY distance: the same rows, here without a pass
+ * of every row through the VM.  For vector_quantize_scan_range the radius is in the units vector_quantize_scan reports. */
+enum { SCAN_TOPK = 0, SCAN_STREAM = 1, SCAN_RANGE = 2 };
+
+/* the rows of a range scan into the cursor (its id / distance arrays, sized to the result) */
+static int range_rows(scan_vtab *vt, scan_cursor *c, const char *fname, vsb_group *ix, int metric, const void *query, double radius,
+                      const uint32_t *allow) {
+    vsb_range *res = 0;
+    if (vsb_group_scan_range(ix, metric, query, 1, &radius, allow, allow ? vsb_group_rows(ix) : 0, &res) != VSB_OK)
+        return vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
+    const int64_t *ids = 0;
+    const double *dist = 0;
+    int64_t n = 0;
+    vsb_range_get(res, 0, &ids, &dist, &n);
+    sqlite3_free(c->ids); sqlite3_free(c->dist);
+    c->k_alloc = 0;                                                      /* a later top-k call on this cursor allocates its own */
+    c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(sqlite3_int64));
+    c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(double));
+    const int rc = (c->ids && c->dist) ? SQLITE_OK : SQLITE_NOMEM;
+    if (rc == SQLITE_OK && n > 0) {
+        memcpy(c->ids, ids, (size_t)n * sizeof(int64_t));
+        memcpy(c->dist, dist, (size_t)n * sizeof(double));
+    }
+    c->row_count = rc == SQLITE_OK ? (int)n : 0;
+    vsb_range_free(res);
+    return rc;
+}
+
 /* common xFilter (vCursorFilterCommon, :1723-1826); filtered: the *_filtered twin, whose 5th argument is the rowid set */
-static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized, int streaming) {
+static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized, int mode) {
     scan_cursor *c = (scan_cursor *)cur;
     scan_vtab *vt = (scan_vtab *)cur->pVtab;
     const int filtered = vt->filtered;
-    c->streaming = streaming;
-    const int nargs = streaming ? 3 : 4 + filtered;
+    c->streaming = mode == SCAN_STREAM;
+    const int nargs = mode == SCAN_STREAM ? 3 : 4 + filtered;
     if (argc != nargs) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, nargs, argc);
     for (int i = 0; i < argc; ++i) {
         int t = sqlite3_value_type(argv[i]);
         if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 3 && mode == SCAN_RANGE && t != SQLITE_INTEGER && t != SQLITE_FLOAT)
+            return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER or FLOAT (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 3 && mode != SCAN_RANGE && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 4) { int rc = check_rowids_arg(vt, fname, argv[4]); if (rc != SQLITE_OK) return rc; }
     }
     const char *tbl = (const char *)sqlite3_value_text(argv[0]);
@@ -1314,7 +1347,14 @@ static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **arg
         query = qq;
     }
 
-    if (streaming) {
+    if (mode == SCAN_RANGE) {
+        c->row_index = 0;
+        c->row_count = 0;
+        if (filtered && (rc = rowids_bitmap(vt, fname, argv[4], ix, &allow)) != SQLITE_OK) goto out;
+        rc = range_rows(vt, c, fname, ix, v->metric, query, sqlite3_value_double(argv[3]), allow);
+        goto out;
+    }
+    if (mode == SCAN_STREAM) {
         sqlite3_int64 n = vsb_group_rows(ix);
         sqlite3_free(c->sdist); sqlite3_free(c->sids);
         c->sdist = (float *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(float));
@@ -1511,6 +1551,15 @@ SCAN_MODULE(mod_full_stream, vt_connect, vt_best_index_stream, vt_filter_full_st
 SCAN_MODULE(mod_quant_stream, vt_connect, vt_best_index_stream, vt_filter_quant_stream);
 SCAN_MODULE(mod_full_filtered, vt_connect_filtered, vt_best_index, vt_filter_full_filtered);
 SCAN_MODULE(mod_quant_filtered, vt_connect_filtered, vt_best_index, vt_filter_quant_filtered);
+static int vt_filter_full_range(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan_range", 0, SCAN_RANGE); }
+static int vt_filter_quant_range(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan_range", 1, SCAN_RANGE); }
+static int vt_filter_full_range_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan_range_filtered", 0, SCAN_RANGE); }
+static int vt_filter_quant_range_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan_range_filtered", 1, SCAN_RANGE); }
+/* the radius takes the hidden column `k` of the top-k schema (argument 4), the rowids the `rowids` column of the filtered one */
+SCAN_MODULE(mod_full_range, vt_connect, vt_best_index, vt_filter_full_range);
+SCAN_MODULE(mod_quant_range, vt_connect, vt_best_index, vt_filter_quant_range);
+SCAN_MODULE(mod_full_range_filtered, vt_connect_filtered, vt_best_index, vt_filter_full_range_filtered);
+SCAN_MODULE(mod_quant_range_filtered, vt_connect_filtered, vt_best_index, vt_filter_quant_range_filtered);
 
 /* vector_rowid_set(x): aggregate of the non-NULL x as the rowids BLOB of the *_filtered modules (int64, host byte order =
  * little-endian), e.g. (SELECT vector_rowid_set(rowid) FROM docs WHERE lang = 'en'); no rows give an empty BLOB */
@@ -1585,5 +1634,10 @@ __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char
     if ((rc = sqlite3_create_module(db, "vector_full_scan_batch_filtered", &mod_full_batch_filtered, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch_filtered", &mod_quant_batch_filtered, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_function(db, "vector_rowid_set", 1, SQLITE_UTF8, ctx, 0, rowid_set_step, rowid_set_final)) != SQLITE_OK) return rc;
+    /* additions: range scans */
+    if ((rc = sqlite3_create_module(db, "vector_full_scan_range", &mod_full_range, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range", &mod_quant_range, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_full_scan_range_filtered", &mod_full_range_filtered, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range_filtered", &mod_quant_range_filtered, ctx)) != SQLITE_OK) return rc;
     return SQLITE_OK;
 }

@@ -99,7 +99,10 @@ VSB_API void vsb_index_free(vsb_index *ix);
  * nq > 1 has no counterpart in the reference (one vector per xFilter); each query then behaves like a fresh cursor.
  * For nq >= 16 on f16/bf16/int8/uint8 columns with L2/SQUARED_L2/COSINE/DOT the scores are computed on the tensor
  * cores (wgmma), and with L1 on any column type by a CUDA-core batch kernel over the same tiles; either way they are
- * refined exactly and results are the same as nq single calls. */
+ * refined exactly and results are the same as nq single calls.
+ * k > 256 (any nq, one query at a time): the all-distances scan, then on the device the exact k-th distance of every prefix
+ * [0, k 2^j) of the column and the rows below their segment's bound in scan order (DESIGN §3.11); the host replays only those.
+ * Results are the same bits as a replay over every row ("large_k_queries", "large_k_cands", "large_k_regrows"). */
 VSB_API int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k, int64_t *out_rowids,
                           double *out_dist, int *out_counts, int *max_index);
 
@@ -143,12 +146,15 @@ VSB_API int vsb_scan_all(vsb_index *ix, int metric, const void *query, float *ou
 
 /* ---- multi-GPU plumbing: each shard emits a small superset of the rows that can enter the
  * reference's slots; the caller concatenates shards in scan order (e.g. after an NCCL all-gather)
- * and finishes with vsb_replay_topk. -------------------------------------------------------- */
+ * and finishes with vsb_replay_topk.  k <= 256: the scan's survivors, or every row when its candidate log
+ * overflowed; k > 256: the rows below their prefix bound (vsb_scan_topk, DESIGN §3.11), about
+ * k (1 + log2(n / k)) rows for rows in random order, every row for strictly falling distances. ------------ */
 VSB_API int vsb_scan_candidates(vsb_index *ix, int metric, const void *queries, int nq, int k, vsb_candidate *out,
                                 int cap_per_query, int *out_counts);
 /* the reference's slot algorithm over candidates in scan order: init (src/sqlite-vector.c:1808-1813),
  * replace-the-max with first-argmax (:2022-2049, :2145-2152), exchange sort and INF trim (:2051-2069,
- * :1816-1817).  Pure host code.  Returns the number of valid rows. */
+ * :1816-1817).  Pure host code; for k > 256 the first argmax is kept in a tournament tree, O(log k) per
+ * replaced slot, with the same result.  Returns the number of valid rows. */
 VSB_API int vsb_replay_topk(const vsb_candidate *cands, int n, int k, int *max_index, int64_t *out_rowids,
                             double *out_dist);
 
@@ -278,7 +284,9 @@ VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row o
 /* counters since creation; name in {"queries","survivors","last_survivors","fallbacks","filter_blocks","fetch_bytes","slots","batches","batch_cands","batch_kept","tc_us","tc_rows","batch_us","stream_bytes","stream_us",
  * "sms" (scan CTAs per launch), "range_pairs" (rows returned by range queries), "range_passes" (range queries that took a second
  * pass), "range_host_sorts" (range results too long for the GPU sort, ordered on the host), "range_batches",
- * "range_batch_fallbacks", "range_query_fallbacks" (see vsb_scan_range)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * "range_batch_fallbacks", "range_query_fallbacks" (see vsb_scan_range), "large_k_queries" (queries with k > 256),
+ * "large_k_cands" (their candidates replayed on the host), "large_k_regrows" (large-k queries whose candidates outgrew the pair
+ * list, which then grew to the exact count)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
  * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */
@@ -291,7 +299,9 @@ VSB_API int64_t vsb_debug_live_handles(void);
  * (and resets) the summed device time and launch count of the scan kernel and of the filter kernel. */
 VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double *filter_ms, int *filter_launches);
 /* diagnostics: copies an internal device buffer of the most recent single-query scan to `out`; name in {"cta_time" (unsigned
- * cycles per scan CTA), "bounds" (int64 tile boundaries of the adaptive row partition)}.  Returns the bytes copied or < 0. */
+ * cycles per scan CTA), "bounds" (int64 tile boundaries of the adaptive row partition), "topk_bounds" (the most recent k > 256
+ * view, a resident column or one streamed window: int64 segment count S, int64 segment ends[32] (the first S used), float
+ * bounds[32] (segment 0: +INF, segment s: the k-th distance of rows [0, ends[s - 1])))}.  Returns the bytes copied or < 0. */
 VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes);
 /* diagnostics: the counterpart of vsb_debug_read for name "bounds": plants a row partition (int64 tile boundaries, one per scan
  * CTA plus one, non-decreasing from 0 to the tile count of the k <= 32 plan; vsb_index_stat "sms" CTAs) into every scan

@@ -108,7 +108,7 @@ int elem_size(int vtype) {
 
 constexpr size_t kStageBuf = 32u << 20;  // pinned staging buffers for preload (two of them)
 constexpr int kOutCap = 1 << 16;         // survivor capacity per query (mapped pinned)
-constexpr int kMaxK = 256;               // candidate path; larger k uses the all-distances path
+constexpr int kMaxK = 256;               // candidate path; larger k takes the large-k path (large_k_candidates)
 constexpr int kSlots = 32;               // result slots: queries in flight (the sharded exchange moves groups of them; a rank may have at most
                                          // kSlots / 2 queries in flight so that a peer never overwrites a gather row that is still being read)
 
@@ -215,6 +215,14 @@ struct vsb_index {
     HostBuf<unsigned> h_range_count;
     long long st_range_pairs = 0, st_range_passes = 0, st_range_host_sorts = 0;
     long long st_range_batches = 0, st_range_batch_fallbacks = 0, st_range_query_fallbacks = 0;
+    // large k (k > kMaxK, DESIGN §3.11): the prefix select's histograms and state, the compaction's per-block offsets (for
+    // lk_boff_cap blocks) and the pinned copy of the candidates; the candidates themselves go to the range search's pair list
+    DeviceBuf<unsigned> d_lk_hist, d_lk_boff;
+    DeviceBuf<LkState> d_lk_state;
+    long long lk_boff_cap = 0;
+    HostBuf<uint2> h_lk;
+    long long h_lk_cap = 0;
+    long long st_large_k_queries = 0, st_large_k_cands = 0, st_large_k_regrows = 0;
 };
 
 // result of a range call (vsb_scan_range): per query, rowids and distances in result order
@@ -538,17 +546,36 @@ inline int64_t rowid_of(const vsb_index *ix, uint32_t local) {
 }
 
 // ------------------------------------------------------------------ the reference's k-slot algorithm
-struct SlotState {
-    int k, mi;
-    double *dist;
-    int64_t *ids;
-};
 inline int first_max(const double *v, int n) {  // first index of the maximum, strict '>' (:2022-2049)
     int b = 0;
     for (int i = 1; i < n; ++i)
         if (v[i] > v[b]) b = i;
     return b;
 }
+// k > kMaxK: first_max in O(log k) per slot change.  A tournament tree over the slots: node i (children 2i, 2i + 1, leaf j at
+// node m + j) holds the first index of the maximum of its leaves.  A right child wins only when strictly greater, so equal
+// values go to the lower index, as in first_max (the slots never hold NaN).  Leaves past k hold -1 and never win.
+struct MaxTree {
+    int m = 1;
+    std::vector<int> node;
+    static int better(const double *v, int a, int b) { return b < 0 ? a : a < 0 ? b : v[b] > v[a] ? b : a; }
+    void build(const double *v, int k) {
+        while (m < k) m <<= 1;
+        node.assign((size_t)2 * m, -1);
+        for (int j = 0; j < k; ++j) node[(size_t)(m + j)] = j;
+        for (int i = m - 1; i >= 1; --i) node[(size_t)i] = better(v, node[(size_t)(2 * i)], node[(size_t)(2 * i + 1)]);
+    }
+    int update(const double *v, int j) {   // after slot j changed: the new first index of the maximum
+        for (int i = (m + j) >> 1; i >= 1; i >>= 1) node[(size_t)i] = better(v, node[(size_t)(2 * i)], node[(size_t)(2 * i + 1)]);
+        return node[1];
+    }
+};
+struct SlotState {
+    int k, mi;
+    double *dist;
+    int64_t *ids;
+    MaxTree *tree = nullptr;   // k > kMaxK (slots_replay), else first_max
+};
 inline void slots_begin(SlotState &s) {  // :1808-1813 (max_index is carried over, not reset)
     for (int i = 0; i < s.k; ++i) { s.dist[i] = std::numeric_limits<double>::infinity(); s.ids[i] = 0; }
     if (s.mi < 0 || s.mi >= s.k) s.mi = 0;
@@ -557,7 +584,7 @@ inline void slots_offer(SlotState &s, float d, int64_t id) {  // :2102-2106 / :2
     if ((double)d < s.dist[s.mi]) {
         s.dist[s.mi] = (double)d;
         s.ids[s.mi] = id;
-        s.mi = first_max(s.dist, s.k);
+        s.mi = s.tree ? s.tree->update(s.dist, s.mi) : first_max(s.dist, s.k);
     }
 }
 inline int slots_finish(SlotState &s) {  // exchange sort + INF trim (:2051-2069, :1816-1817)
@@ -586,6 +613,11 @@ template <class Feed>
 int slots_replay(int k, int *mi, double *dist, int64_t *ids, Feed feed) {
     SlotState s{k, mi ? *mi : 0, dist, ids};
     slots_begin(s);
+    MaxTree tree;
+    if (k > kMaxK) {
+        tree.build(dist, k);
+        s.tree = &tree;
+    }
     const int rc = feed(s);
     if (rc) return rc;
     if (mi) *mi = s.mi;
@@ -652,16 +684,27 @@ int visit_survivors(vsb_index *ix, Slot *slot, bool *overflow, Visit visit) {
 
 int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *out_dist);
 
+// the all-distances buffer, allocated on first use: capacity floats for a resident index, two window halves for a streamed one
+int ensure_dist_all(vsb_index *ix) {
+    if (ix->d_dist_all) return VSB_OK;
+    if (ix->streamed) {
+        CU(ix->d_dist_all.alloc(sizeof(float) * 2 * (size_t)ix->win_rows));
+        ix->dev_bytes += sizeof(float) * 2 * (size_t)ix->win_rows;
+    } else {
+        CU(ix->d_dist_all.alloc(sizeof(float) * (size_t)std::max<long long>(ix->cap, 1)));
+        ix->dev_bytes += sizeof(float) * (size_t)ix->cap;
+    }
+    return VSB_OK;
+}
+
 int scan_all_into(vsb_index *ix, int metric, const uint8_t *d_query, std::vector<float> &dist) {
     if (ix->streamed) {
         dist.resize((size_t)ix->n);
         return streamed_scan_all(ix, metric, d_query, dist.data());
     }
-    if (!ix->d_dist_all) {
-        CU(ix->d_dist_all.alloc(sizeof(float) * (size_t)std::max<long long>(ix->cap, 1)));
-        ix->dev_bytes += sizeof(float) * (size_t)ix->cap;
-    }
-    int rc = launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all, true, ix->stream);
+    int rc = ensure_dist_all(ix);
+    if (rc) return rc;
+    rc = launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all, true, ix->stream);
     if (rc) return rc;
     dist.resize((size_t)ix->n);
     CU(cudaMemcpyAsync(dist.data(), ix->d_dist_all, sizeof(float) * (size_t)ix->n, cudaMemcpyDeviceToHost, ix->stream));
@@ -712,12 +755,10 @@ int stream_windows(vsb_index *ix, int depth, Launch launch, Visit visit, bool ho
     return VSB_OK;
 }
 
-// all distances of a streamed index (stream modules, k > 256, overflow fallback)
+// all distances of a streamed index (stream modules, overflow fallback)
 int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *out_dist) {
-    if (!ix->d_dist_all) {
-        CU(ix->d_dist_all.alloc(sizeof(float) * 2 * (size_t)ix->win_rows));
-        ix->dev_bytes += sizeof(float) * 2 * (size_t)ix->win_rows;
-    }
+    const int rc = ensure_dist_all(ix);
+    if (rc) return rc;
     return stream_windows(ix, 2,
         [&](long long, const uint8_t *vec, long long rows, int s) {
             return launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all + (size_t)s * ix->win_rows, false, ix->stream, false, vec, rows);
@@ -758,7 +799,7 @@ long long count_bits(const uint32_t *bits, long long a, long long b) {
     return c;
 }
 
-// the all-distances fallback (k > kMaxK, candidate overflow): every (eligible) row is a candidate, in scan order
+// the all-distances fallback (candidate overflow): every (eligible) row is a candidate, in scan order
 int all_candidates(vsb_index *ix, int metric, const uint8_t *d_query, std::vector<uint2> &cands) {
     ix->st_fallbacks++;
     std::vector<float> dist;
@@ -836,26 +877,27 @@ int stage_host_query(vsb_index *ix, const void *query, Slot **slot) {
     return stage_query(ix, *slot, query, ix->stream);
 }
 
-// one query, host in / candidates out (sorted by scan order).  Falls back to the all-distances kernel when the
-// candidate log overflowed or k is larger than the candidate path supports (still GPU-computed distances).
+int large_k_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k, std::vector<uint2> &cands);
+
+// one query, host in / candidates out (sorted by scan order).  k > kMaxK takes the large-k path (DESIGN §3.11).  Falls back to
+// the all-distances kernel when the candidate log overflowed (still GPU-computed distances).
 int query_candidates(vsb_index *ix, int metric, const void *query, int k, std::vector<uint2> &cands) {
     Slot *slot = nullptr;
     int rc = stage_host_query(ix, query, &slot);   // synchronous call: one stream (a possible all-distances fallback reads d_query on it)
     if (rc) return rc;
+    if (k > kMaxK) return large_k_candidates(ix, metric, slot->d_query, k, cands);
     cands.clear();
     cands.reserve(kFirstFetch);                    // one allocation for the usual few hundred survivors
-    bool overflow = (k > kMaxK);
-    if (!overflow) {
-        rc = ensure_workspace(ix, k);
-        if (rc) return rc;
-        if (ix->streamed) {
-            rc = streamed_candidates(ix, metric, slot->d_query, k, cands, &overflow);
-        } else {
-            rc = launch_scan(ix, metric, slot->d_query, k, slot, nullptr, true, ix->stream);
-            if (rc == VSB_OK) rc = visit_survivors(ix, slot, &overflow, [&](uint2 c) { cands.push_back(c); });
-        }
-        if (rc) return rc;
+    bool overflow = false;
+    rc = ensure_workspace(ix, k);
+    if (rc) return rc;
+    if (ix->streamed) {
+        rc = streamed_candidates(ix, metric, slot->d_query, k, cands, &overflow);
+    } else {
+        rc = launch_scan(ix, metric, slot->d_query, k, slot, nullptr, true, ix->stream);
+        if (rc == VSB_OK) rc = visit_survivors(ix, slot, &overflow, [&](uint2 c) { cands.push_back(c); });
     }
+    if (rc) return rc;
     return overflow ? all_candidates(ix, metric, slot->d_query, cands) : VSB_OK;
 }
 
@@ -1047,6 +1089,136 @@ void range_put(vsb_range *r, int q, size_t n, At at) {
         r->ids[(size_t)q][i] = e.first;
         r->dist[(size_t)q][i] = (double)d;
     }
+}
+
+// ------------------------------------------------------------------ large k (k > kMaxK, DESIGN §3.11)
+constexpr size_t kLkHistBytes = sizeof(unsigned) * kLkPasses * kLkMaxSeg * 256;
+
+// the select's histograms and state, and the compaction's offsets for views of up to `rows` rows (grown, never shrunk;
+// large-k calls are synchronous, no launch reads the old buffers)
+int ensure_large_k(vsb_index *ix, long long rows) {
+    if (!ix->d_lk_state) {
+        DeviceBuf<unsigned> hist;
+        DeviceBuf<LkState> st;
+        CU(hist.alloc(kLkHistBytes));
+        CU(st.alloc(sizeof(LkState)));
+        CU(cudaMemset(st, 0, sizeof(LkState)));
+        ix->d_lk_hist = std::move(hist);
+        ix->d_lk_state = std::move(st);
+        ix->dev_bytes += kLkHistBytes + sizeof(LkState);
+    }
+    const long long blocks = std::max<long long>(1, (rows + kLkRows - 1) / kLkRows);
+    if (blocks > ix->lk_boff_cap) {
+        DeviceBuf<unsigned> d;
+        CU(d.alloc(sizeof(unsigned) * (size_t)blocks));
+        ix->dev_bytes += sizeof(unsigned) * (size_t)(blocks - ix->lk_boff_cap);
+        ix->d_lk_boff = std::move(d);
+        ix->lk_boff_cap = blocks;
+    }
+    return VSB_OK;
+}
+
+// the candidates of one view (its n distances at dist, its first row shard row r0) appended to the pair list on ix->stream:
+// segment ends k, 2k, 4k, ... below n, then n; the prefix bounds digit by digit; the ordered compaction.  write_only: only
+// the compaction's write, again (the list grew to the count the offsets kernel left)
+int large_k_view(vsb_index *ix, const float *dist, long long n, long long r0, int k, bool write_only = false) {
+    if (n <= 0) return VSB_OK;
+    LkParams p{};
+    p.dist = dist;
+    p.n = n;
+    p.k = k;
+    for (long long e = k; e < n && p.nseg < kLkMaxSeg - 1; e *= 2) p.ends[p.nseg++] = e;
+    p.ends[p.nseg++] = n;
+    p.allow = ix->flt_d;
+    p.allow_base = r0;
+    p.hist = ix->d_lk_hist;
+    p.st = ix->d_lk_state;
+    p.boff = ix->d_lk_boff;
+    p.total = ix->d_range_count;
+    p.out = ix->d_range;
+    p.cap = ix->range_cap;
+    p.row_base = (unsigned)r0;
+    p.nblocks = (int)((n + kLkRows - 1) / kLkRows);
+    if (!write_only) {
+        const int prefixes = p.nseg - 1;
+        if (prefixes > 0) CU(cudaMemsetAsync(ix->d_lk_hist, 0, kLkHistBytes, ix->stream));
+        for (p.pass = 0; p.pass < kLkPasses; ++p.pass) {
+            if (prefixes > 0) {
+                lk_hist_kernel<<<(unsigned)((p.ends[prefixes - 1] + kLkRows - 1) / kLkRows), kLkThreads, 0, ix->stream>>>(p);
+                CU(cudaGetLastError());
+                ++g_launches;
+            }
+            lk_select_kernel<<<1, kLkMaxSeg * 32, 0, ix->stream>>>(p);   // the last digit also records the segments and bounds
+            CU(cudaGetLastError());
+            ++g_launches;
+        }
+        lk_count_kernel<<<p.nblocks, kLkThreads, 0, ix->stream>>>(p);
+        CU(cudaGetLastError());
+        lk_offsets_kernel<<<1, kLkScanThreads, 0, ix->stream>>>(p);
+        CU(cudaGetLastError());
+        g_launches += 2;
+    }
+    lk_write_kernel<<<p.nblocks, kLkThreads, 0, ix->stream>>>(p);
+    CU(cudaGetLastError());
+    ++g_launches;
+    return VSB_OK;
+}
+
+// the candidates of one query with k > kMaxK staged at d_query: the all-distances scan, then the bounds and the compaction of
+// each view on the device (the resident column, or every window behind its scan), (distance bits, shard row) in scan order.  The
+// first pair list holds kRangeCap0 pairs or twice what rows in random order give; a larger count grows the list to the exact
+// count and, resident, writes again from the distances still in HBM, streamed, runs the windows once more.
+int large_k_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k, std::vector<uint2> &cands) {
+    cands.clear();
+    ix->st_large_k_queries++;
+    if (ix->n == 0) return VSB_OK;
+    const long long view = ix->streamed ? std::min(ix->win_rows, ix->n) : ix->n, views = (ix->n + view - 1) / view;
+    const long long expect = views * k * (2 + (long long)std::log2(std::max(1.0, (double)view / k)));
+    int rc = ensure_dist_all(ix);
+    if (rc == VSB_OK) rc = ensure_large_k(ix, view);
+    if (rc == VSB_OK) rc = ensure_range(ix, std::max(kRangeCap0, std::min(ix->n, 2 * expect)));
+    if (rc) return rc;
+    for (int pass = 0;; ++pass) {
+        CU(cudaMemsetAsync(ix->d_range_count, 0, sizeof(unsigned), ix->stream));
+        if (ix->streamed) {
+            rc = stream_windows(ix, 2,
+                [&](long long w, const uint8_t *vec, long long rows, int s) {
+                    float *dist = ix->d_dist_all + (size_t)s * ix->win_rows;
+                    const int r = launch_scan(ix, metric, d_query, 0, nullptr, dist, false, ix->stream, false, vec, rows, w * ix->win_rows);
+                    return r ? r : large_k_view(ix, dist, rows, w * ix->win_rows, k);
+                },
+                [&](long long, long long, long long, int) { return (int)VSB_OK; });
+        } else {
+            rc = launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all, false, ix->stream);
+            if (rc == VSB_OK) rc = large_k_view(ix, ix->d_dist_all, ix->n, 0, k);
+        }
+        if (rc) return rc;
+        CU(cudaMemcpyAsync(ix->h_range_count, ix->d_range_count, sizeof(unsigned), cudaMemcpyDeviceToHost, ix->stream));
+        CU(cudaStreamSynchronize(ix->stream));
+        const long long cnt = *ix->h_range_count;
+        if (cnt <= ix->range_cap) break;
+        if (pass > 0) return fail(VSB_ECUDA, "large-k candidates: %lld pairs after growing the list to %lld", cnt, ix->range_cap);
+        ix->st_large_k_regrows++;
+        rc = ensure_range(ix, cnt);
+        if (rc) return rc;
+        if (!ix->streamed) {
+            rc = large_k_view(ix, ix->d_dist_all, ix->n, 0, k, true);
+            if (rc) return rc;
+            break;
+        }
+    }
+    const long long cnt = *ix->h_range_count;
+    if (cnt > ix->h_lk_cap) {
+        HostBuf<uint2> h;
+        CU(h.alloc(sizeof(uint2) * (size_t)cnt));
+        ix->h_lk = std::move(h);
+        ix->h_lk_cap = cnt;
+    }
+    if (cnt > 0) CU(cudaMemcpyAsync(ix->h_lk, ix->d_range, sizeof(uint2) * (size_t)cnt, cudaMemcpyDeviceToHost, ix->stream));
+    CU(cudaStreamSynchronize(ix->stream));
+    cands.assign(ix->h_lk.get(), ix->h_lk.get() + cnt);
+    ix->st_large_k_cands += cnt;
+    return VSB_OK;
 }
 
 }  // namespace
@@ -1326,6 +1498,9 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "range_batches")) return ix->st_range_batches;
     if (!strcmp(name, "range_batch_fallbacks")) return ix->st_range_batch_fallbacks;
     if (!strcmp(name, "range_query_fallbacks")) return ix->st_range_query_fallbacks;
+    if (!strcmp(name, "large_k_queries")) return ix->st_large_k_queries;
+    if (!strcmp(name, "large_k_cands")) return ix->st_large_k_cands;
+    if (!strcmp(name, "large_k_regrows")) return ix->st_large_k_regrows;
     return -1;
 }
 void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullptr; }
@@ -1484,8 +1659,9 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
     size_t have = 0;
     if (!strcmp(name, "cta_time")) { src = w.d_cta_time; have = sizeof(unsigned) * (size_t)ix->num_sms; }
     else if (!strcmp(name, "bounds")) { src = w.d_bounds; have = sizeof(long long) * (size_t)(ix->num_sms + 1); }
+    else if (!strcmp(name, "topk_bounds")) { src = ix->d_lk_state; have = offsetof(LkState, sel); }   // segments and bounds of the last large-k view
     else return fail(VSB_EINVAL, "unknown debug buffer %s", name);
-    if (!src) return fail(VSB_EINVAL, "no scan has run yet");
+    if (!src) return fail(VSB_EINVAL, "no %s has run yet", strcmp(name, "topk_bounds") ? "scan" : "large-k query");
     CU(cudaMemcpy(out, src, std::min<size_t>(have, (size_t)bytes), cudaMemcpyDeviceToHost));
     return (int)std::min<size_t>(have, (size_t)bytes);
 }

@@ -716,6 +716,256 @@ __global__ void __launch_bounds__(kRangeSortThreads, 1) range_sort_kernel(const 
     }
 }
 
+// ------------------------------------------------------------------ large k (k > 256): prefix bounds and ordered candidates
+// One scanned view (a resident shard, one streamed window) whose distances scan_kernel wrote to dist_all.  Its rows are cut into
+// segments [0, k), [k, 2k), [2k, 4k), ..., [.., n).  Segment s >= 1 is tested against B_{s-1}, the k-th smallest distance (fkey
+// order) of the eligible, non-NaN rows of the prefix [0, ends[s-1]), +INF when that prefix has fewer than k such rows; segment 0
+// against +INF.  A row that can enter the k slots has d < its segment's bound (DESIGN §3.11), so the eligible rows with
+// d < bound, in scan order, are a superset of the rows the host replay needs.
+//   lk_hist_kernel + lk_select_kernel, once per digit: a radix select of every prefix's k-th key at once, 4 digits of 8 bits,
+//   most significant first, on the device (no host round trip between digits);
+//   lk_count_kernel, lk_offsets_kernel, lk_write_kernel: the ordered compaction of the candidates into the pair list.
+constexpr int kLkMaxSeg = 32;        // segments of a view: n < 2^32 and k > 256 need at most 25
+constexpr int kLkThreads = 256;
+constexpr int kLkRows = 8192;        // rows of one block of the histogram and compaction kernels (32 per thread)
+constexpr int kLkPasses = 4;         // radix digits of 8 bits
+constexpr int kLkScanThreads = 1024; // lk_offsets_kernel; lk_select_kernel runs one warp per prefix (kLkMaxSeg warps)
+
+// the most recent view's segments and bounds (vsb_debug_read "topk_bounds" returns the first three fields) and the select's state
+struct LkState {
+    long long nseg;
+    long long ends[kLkMaxSeg];       // segment s = rows [s ? ends[s - 1] : 0, ends[s]); ends[nseg - 1] = n
+    float bound[kLkMaxSeg];          // bound[0] = +INF, bound[s] = B_{s-1}
+    unsigned sel[kLkMaxSeg];         // prefix j = rows [0, ends[j]): the key digits chosen so far
+    unsigned rank[kLkMaxSeg];        // prefix j: rank (from 1) of the k-th key among the keys that start with sel[j]
+    int live[kLkMaxSeg];             // prefix j holds at least k keys (else its bound is +INF)
+};
+
+struct LkParams {
+    const float *dist;               // [n] distances of the view
+    long long n;
+    int k, nseg;                     // prefixes: nseg - 1
+    long long ends[kLkMaxSeg];
+    const uint32_t *allow;           // row filter as in ScanParams: row r is eligible at bit allow_base + r (nullptr: every row)
+    long long allow_base;
+    unsigned *hist;                  // [kLkPasses][kLkMaxSeg][256], zero before the first digit
+    LkState *st;
+    unsigned *boff;                  // [blocks]: candidates per compaction block (count), then where they start (offsets)
+    unsigned *total;                 // pairs of the views so far (the pair list's counter); the offsets kernel adds this view's
+    uint2 *out;                      // pair list: (distance bits, row_base + row); positions at or past cap are not written
+    long long cap;
+    unsigned row_base;
+    int pass;                        // lk_hist_kernel / lk_select_kernel: the digit (0 = most significant)
+    int nblocks;                     // lk_offsets_kernel: compaction blocks
+};
+
+// the segment ends into shared memory (compile-time parameter offsets only: no local copy of the parameter block)
+__device__ __forceinline__ void lk_load_ends(const LkParams &p, long long *ends) {
+#pragma unroll
+    for (int i = 0; i < kLkMaxSeg; ++i)
+        if ((int)threadIdx.x == i) ends[i] = i < p.nseg ? p.ends[i] : 0x7FFFFFFFFFFFFFFFll;
+}
+
+// histogram of digit p.pass: every eligible, non-NaN row of a prefix whose higher digits match the prefix's chosen ones (all of
+// them at digit 0) adds to that prefix's bin.  Row r lies in the prefixes j >= its segment; rows of the last segment in none.
+__global__ void __launch_bounds__(kLkThreads) lk_hist_kernel(const LkParams p) {
+    __shared__ unsigned h[kLkMaxSeg * 256];
+    __shared__ long long ends[kLkMaxSeg];
+    __shared__ unsigned sel[kLkMaxSeg];
+    __shared__ int live[kLkMaxSeg];
+    const int J = p.nseg - 1;
+    lk_load_ends(p, ends);
+    if ((int)threadIdx.x < J) {
+        sel[threadIdx.x] = p.pass ? p.st->sel[threadIdx.x] : 0u;
+        live[threadIdx.x] = p.pass ? p.st->live[threadIdx.x] : 1;
+    }
+    __syncthreads();
+    const long long c0 = (long long)blockIdx.x * kLkRows, c1 = min(c0 + (long long)kLkRows, ends[J - 1]);
+    int s0 = 0;
+    while (c0 >= ends[s0]) ++s0;
+    for (int i = s0 * 256 + threadIdx.x; i < J * 256; i += kLkThreads) h[i] = 0u;
+    __syncthreads();
+    const int shift = 24 - 8 * p.pass;
+    int s = s0;
+    for (long long r = c0 + threadIdx.x; r < c1; r += kLkThreads) {
+        while (r >= ends[s]) ++s;
+        const float d = p.dist[r];
+        if (d != d || !row_allowed(p.allow, p.allow_base + r)) continue;
+        const uint32_t key = fkey(d), dig = (key >> shift) & 255u;
+        const uint32_t hi = p.pass ? key >> (shift + 8) : 0u;
+        for (int j = s; j < J; ++j)
+            if (live[j] && hi == sel[j]) atomicAdd(&h[j * 256 + dig], 1u);
+    }
+    __syncthreads();
+    unsigned *g = p.hist + (size_t)p.pass * kLkMaxSeg * 256;
+    for (int i = s0 * 256 + threadIdx.x; i < J * 256; i += kLkThreads)
+        if (h[i]) atomicAdd(g + i, h[i]);
+}
+
+// one warp per prefix: the bin of digit p.pass that holds the prefix's k-th key.  At digit 0 a prefix with fewer than k keys
+// is done (bound +INF).  After the last digit the chosen digits are the k-th key; the view's segments and bounds are written.
+__global__ void __launch_bounds__(kLkMaxSeg * 32, 1) lk_select_kernel(const LkParams p) {
+    const int j = threadIdx.x >> 5, lane = threadIdx.x & 31, J = p.nseg - 1;
+    LkState *st = p.st;
+    if (j < J) {
+        unsigned sel = p.pass ? st->sel[j] : 0u, rank = p.pass ? st->rank[j] : (unsigned)p.k;
+        int live = p.pass ? st->live[j] : 1;
+        if (live) {
+            const unsigned *hj = p.hist + ((size_t)p.pass * kLkMaxSeg + j) * 256 + lane * 8;
+            unsigned c[8], sum = 0;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) { c[i] = hj[i]; sum += c[i]; }
+            unsigned incl = sum;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+                if (lane >= o) incl += v;
+            }
+            if (__shfl_sync(0xFFFFFFFFu, incl, 31) < rank) {
+                live = 0;
+            } else {
+                const int src = __ffs(__ballot_sync(0xFFFFFFFFu, incl >= rank)) - 1;
+                unsigned dig = 0, nr = 0, cum = incl - sum;
+                bool found = false;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    if (!found && cum + c[i] >= rank) { dig = (unsigned)(lane * 8 + i); nr = rank - cum; found = true; }
+                    cum += c[i];
+                }
+                sel = (sel << 8) | __shfl_sync(0xFFFFFFFFu, dig, src);
+                rank = __shfl_sync(0xFFFFFFFFu, nr, src);
+            }
+        }
+        if (lane == 0) {
+            st->sel[j] = sel;
+            st->rank[j] = rank;
+            st->live[j] = live;
+            if (p.pass == kLkPasses - 1) st->bound[j + 1] = live ? funkey(sel) : INFINITY;
+        }
+    }
+    if (p.pass == kLkPasses - 1) {
+#pragma unroll
+        for (int i = 0; i < kLkMaxSeg; ++i)
+            if ((int)threadIdx.x == i) st->ends[i] = i < p.nseg ? p.ends[i] : 0;
+        if (threadIdx.x == 0) {
+            st->nseg = p.nseg;
+            st->bound[0] = INFINITY;
+        }
+    }
+}
+
+// the segment ends and bounds of a compaction block, and the segment of its first row
+__device__ __forceinline__ int lk_load_bounds(const LkParams &p, long long *ends, float *bound, long long c0) {
+    lk_load_ends(p, ends);
+    if ((int)threadIdx.x < p.nseg) bound[threadIdx.x] = p.st->bound[threadIdx.x];
+    __syncthreads();
+    int s = 0;
+    while (c0 >= ends[s]) ++s;
+    return s;
+}
+
+__device__ __forceinline__ bool lk_candidate(const LkParams &p, long long r, float d, float bound) {
+    return d < bound && row_allowed(p.allow, p.allow_base + r);
+}
+
+// candidates of each block of kLkRows rows
+__global__ void __launch_bounds__(kLkThreads) lk_count_kernel(const LkParams p) {
+    __shared__ long long ends[kLkMaxSeg];
+    __shared__ float bound[kLkMaxSeg];
+    __shared__ unsigned wsum[kLkThreads / 32];
+    const long long c0 = (long long)blockIdx.x * kLkRows, c1 = min(c0 + (long long)kLkRows, p.n);
+    int s = lk_load_bounds(p, ends, bound, c0);
+    unsigned c = 0;
+    for (long long r = c0 + threadIdx.x; r < c1; r += kLkThreads) {
+        while (r >= ends[s]) ++s;
+        c += lk_candidate(p, r, p.dist[r], bound[s]) ? 1u : 0u;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, o);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned t = 0;
+        for (int w = 0; w < kLkThreads / 32; ++w) t += wsum[w];
+        p.boff[blockIdx.x] = t;
+    }
+}
+
+// one block: the block counts become the positions their candidates start at, after the pairs of the earlier views (*total);
+// *total grows by this view's candidates
+__global__ void __launch_bounds__(kLkScanThreads, 1) lk_offsets_kernel(const LkParams p) {
+    __shared__ unsigned wsum[kLkScanThreads / 32];
+    __shared__ unsigned carry;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = *p.total;
+    __syncthreads();
+    for (int b0 = 0; b0 < p.nblocks; b0 += kLkScanThreads) {
+        const int i = b0 + (int)threadIdx.x;
+        const unsigned v = i < p.nblocks ? p.boff[i] : 0u;
+        unsigned incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned t = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= o) incl += t;
+        }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            unsigned w = wsum[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned t = __shfl_up_sync(0xFFFFFFFFu, w, o);
+                if (lane >= o) w += t;
+            }
+            wsum[lane] = w;
+        }
+        __syncthreads();
+        const unsigned base = carry;
+        if (i < p.nblocks) p.boff[i] = base + (warp ? wsum[warp - 1] : 0u) + incl - v;
+        __syncthreads();
+        if (threadIdx.x == 0) carry = base + wsum[kLkScanThreads / 32 - 1];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *p.total = carry;
+}
+
+// writes each block's candidates in scan order from its offset on (pairs at or past cap are dropped; the host grows the list to
+// the count and runs this kernel again)
+__global__ void __launch_bounds__(kLkThreads) lk_write_kernel(const LkParams p) {
+    __shared__ long long ends[kLkMaxSeg];
+    __shared__ float bound[kLkMaxSeg];
+    __shared__ unsigned wcnt[kLkThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long c0 = (long long)blockIdx.x * kLkRows, c1 = min(c0 + (long long)kLkRows, p.n);
+    int s = lk_load_bounds(p, ends, bound, c0);
+    unsigned pos = p.boff[blockIdx.x];
+    for (long long r0 = c0; r0 < c1; r0 += kLkThreads) {
+        const long long r = r0 + threadIdx.x;
+        bool hit = false;
+        float d = 0.f;
+        if (r < c1) {
+            while (r >= ends[s]) ++s;
+            d = p.dist[r];
+            hit = lk_candidate(p, r, d, bound[s]);
+        }
+        const unsigned m = __ballot_sync(0xFFFFFFFFu, hit);
+        if (lane == 0) wcnt[warp] = (unsigned)__popc(m);
+        __syncthreads();
+        unsigned before = 0, tot = 0;
+#pragma unroll
+        for (int w = 0; w < kLkThreads / 32; ++w) {
+            before += w < warp ? wcnt[w] : 0u;
+            tot += wcnt[w];
+        }
+        if (hit) {
+            const unsigned at = pos + before + (unsigned)__popc(m & ((1u << lane) - 1u));
+            if ((long long)at < p.cap) p.out[at] = make_uint2(__float_as_uint(d), p.row_base + (unsigned)r);
+        }
+        pos += tot;
+        __syncthreads();
+    }
+}
+
 // ------------------------------------------------------------------ candidate filter
 // One warp per stream.  thresholds: a row of stream s can only enter the reference's slots if its distance
 // is below the k-th smallest distance among ALL earlier rows; any subset of earlier rows gives a valid upper

@@ -106,6 +106,19 @@ int elem_size(int vtype) {
     return 0;
 }
 
+// grows buf, which holds cap elements, to need elements (never shrinks).  The old contents are dropped: every caller is a
+// synchronous call, so no launch still reads the old buffer.  counted: the byte count that the growth is added to, or null
+template <template <class> class Buf, class T>
+int grow_buf(Buf<T> &buf, long long &cap, long long need, size_t *counted) {
+    if (need <= cap) return VSB_OK;
+    Buf<T> b;
+    CU(b.alloc(sizeof(T) * (size_t)need));
+    if (counted) *counted += sizeof(T) * (size_t)(need - cap);
+    buf = std::move(b);
+    cap = need;
+    return VSB_OK;
+}
+
 constexpr size_t kStageBuf = 32u << 20;  // pinned staging buffers for preload (two of them)
 constexpr int kOutCap = 1 << 16;         // survivor capacity per query (mapped pinned)
 constexpr int kMaxK = 256;               // candidate path; larger k takes the large-k path (large_k_candidates)
@@ -139,6 +152,17 @@ struct Slot {
     int *d_ctrl = nullptr;                           // inside vsb_index::d_ctrl
     Event done;   // recorded after the result block of this slot has been copied to the host
     int seq = 0;
+};
+
+// The pair list of range search and large k (pair_list_run): the (row, distance bits) pairs the kernels append, their counter,
+// which keeps counting past cap, and the counter's host copy.  Large k reads the list back through the pinned h_pairs.
+struct PairList {
+    DeviceBuf<uint2> d_pairs;
+    long long cap = 0;
+    DeviceBuf<unsigned> d_count;
+    HostBuf<unsigned> h_count;
+    HostBuf<uint2> h_pairs;
+    long long h_cap = 0;
 };
 
 struct BatchWs;   // batch_host.inc
@@ -202,26 +226,21 @@ struct vsb_index {
     // bit i & 31 of word i >> 5) on the host and in d_allow; both null outside such a call, when every row is eligible
     const uint32_t *flt_h = nullptr, *flt_d = nullptr;
     DeviceBuf<uint32_t> d_allow;      // rows / 32 words + 1: a warp's read past the last row stays inside
-    size_t allow_words = 0;
+    long long allow_words = 0;
     // rowid -> row lookup of explicit rowids (vsb_index_rowid_bitmap): (rowid, row) sorted, built for rowid_rows rows on first
     // need; an append changes n and so rebuilds it
     std::vector<std::pair<int64_t, long long>> rowid_sorted;
     long long rowid_rows = -1;
-    // range search (vsb_scan_range): the pair list the range scan appends to, its counter, and the counter's host copy; the list
-    // starts at kRangeCap0 pairs and grows to the exact count of a query that needed more
-    DeviceBuf<uint2> d_range;
-    long long range_cap = 0;
-    DeviceBuf<unsigned> d_range_count;
-    HostBuf<unsigned> h_range_count;
+    // range search (vsb_scan_range) and large k: the pair list, which starts at kRangeCap0 pairs or more and grows to the exact
+    // count of a query that needed more
+    PairList plist;
     long long st_range_pairs = 0, st_range_passes = 0, st_range_host_sorts = 0;
     long long st_range_batches = 0, st_range_batch_fallbacks = 0, st_range_query_fallbacks = 0;
-    // large k (k > kMaxK, DESIGN §3.11): the prefix select's histograms and state, the compaction's per-block offsets (for
-    // lk_boff_cap blocks) and the pinned copy of the candidates; the candidates themselves go to the range search's pair list
+    // large k (k > kMaxK, DESIGN §3.11): the prefix select's histograms and state and the compaction's per-block offsets (for
+    // lk_boff_cap blocks); the candidates themselves go to the pair list
     DeviceBuf<unsigned> d_lk_hist, d_lk_boff;
     DeviceBuf<LkState> d_lk_state;
     long long lk_boff_cap = 0;
-    HostBuf<uint2> h_lk;
-    long long h_lk_cap = 0;
     long long st_large_k_queries = 0, st_large_k_cands = 0, st_large_k_regrows = 0;
 };
 
@@ -387,6 +406,31 @@ int ensure_workspace(vsb_index *ix, int k) {
     return VSB_OK;
 }
 
+// the ScanParams of a top-k and a range launch alike: rows [0, n) of vec, whose first row is shard row r0 (the row filter is
+// indexed by shard rows), scanned with plan pl for the query at d_query
+ScanParams scan_params(const vsb_index *ix, const Plan &pl, int root, const uint8_t *d_query, const uint8_t *vec, long long n, long long r0) {
+    ScanParams p{};
+    p.vec = vec;
+    p.n = n;
+    p.pitch = ix->pitch;
+    p.nc = ix->pitch / 16;
+    p.log2P = pl.log2P;
+    p.wtile_bytes = pl.wtile_bytes;
+    p.nsw = pl.nsw;
+    p.root = root;
+    p.query = d_query;
+    p.allow = ix->flt_d;
+    p.allow_base = r0;
+    return p;
+}
+
+// the plan of the most recent scan launch (vsb_index_stat "plan_*")
+void note_plan(vsb_index *ix, const Plan &pl) {
+    ix->last_log2p = pl.log2P;
+    ix->last_nsw = pl.nsw;
+    ix->last_direct = pl.direct ? 1 : 0;
+}
+
 unsigned exchange_next_seq(vsb_index *ix, int slot);
 int merge_blocks_strided(const uint8_t *blocks, int world, size_t stride, const int64_t *first_seq, int k, int64_t *out_rowids, double *out_dist);
 int exchange_fill_push(vsb_index *ix, PushParams *pp);
@@ -437,19 +481,10 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
         CU(cudaMemsetAsync(wk->d_cta_time, 0, sizeof(unsigned) * (size_t)ix->num_sms, ss));
         wk->bounds_tiles = total_tiles;
     }
-    ScanParams p{};
-    p.vec = scan_vec;
-    p.n = scan_n;
-    p.pitch = ix->pitch;
-    p.nc = ix->pitch / 16;
-    p.log2P = pl.log2P;
-    p.wtile_bytes = pl.wtile_bytes;
-    p.nsw = pl.nsw;
-    p.root = root;
+    ScanParams p = scan_params(ix, pl, root, d_query, scan_vec, scan_n, view_r0);
     p.k = k;
     p.kcap = kcap;
     p.logcap = ix->ws_logcap;
-    p.query = d_query;
     p.lists = wk ? wk->d_lists.get() : nullptr;
     p.tlocal = wk ? wk->d_tlocal.get() : nullptr;
     p.logs = wk ? wk->d_logs.get() : nullptr;
@@ -458,8 +493,6 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
     p.dist_all = d_dist_all;
     p.bounds = balance ? wk->d_bounds.get() : nullptr;
     p.cta_time = balance ? wk->d_cta_time.get() : nullptr;
-    p.allow = ix->flt_d;
-    p.allow_base = view_r0;
     Event *pev = nullptr;
     if (g_opt_time_kernels > 0 && (ix->prof_tick++ % g_opt_time_kernels) == 0) {   // time_kernels = N: every N-th launch
         if (ix->prof_used + 4 > ix->prof_ev.size()) {
@@ -477,7 +510,7 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
     fn<<<ix->num_sms, kThreads, pl.smem, ss>>>(p);
     CU(cudaGetLastError());
     ++g_launches;
-    ix->last_log2p = pl.log2P; ix->last_nsw = pl.nsw; ix->last_direct = pl.direct ? 1 : 0;
+    note_plan(ix, pl);
     if (pev) CU(cudaEventRecord(pev[1], ss));
     if (k > 0) {
         CU(cudaEventRecord(wk->scanned, ss));
@@ -682,8 +715,6 @@ int visit_survivors(vsb_index *ix, Slot *slot, bool *overflow, Visit visit) {
     return VSB_OK;
 }
 
-int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *out_dist);
-
 // the all-distances buffer, allocated on first use: capacity floats for a resident index, two window halves for a streamed one
 int ensure_dist_all(vsb_index *ix) {
     if (ix->d_dist_all) return VSB_OK;
@@ -697,21 +728,6 @@ int ensure_dist_all(vsb_index *ix) {
     return VSB_OK;
 }
 
-int scan_all_into(vsb_index *ix, int metric, const uint8_t *d_query, std::vector<float> &dist) {
-    if (ix->streamed) {
-        dist.resize((size_t)ix->n);
-        return streamed_scan_all(ix, metric, d_query, dist.data());
-    }
-    int rc = ensure_dist_all(ix);
-    if (rc) return rc;
-    rc = launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all, true, ix->stream);
-    if (rc) return rc;
-    dist.resize((size_t)ix->n);
-    CU(cudaMemcpyAsync(dist.data(), ix->d_dist_all, sizeof(float) * (size_t)ix->n, cudaMemcpyDeviceToHost, ix->stream));
-    CU(cudaStreamSynchronize(ix->stream));
-    return VSB_OK;
-}
-
 int stage_query(vsb_index *ix, Slot *slot, const void *query, cudaStream_t ss) {
     const int qbytes = ix->dim * ix->esize;
     memcpy(slot->h_query, query, (size_t)qbytes);
@@ -720,70 +736,75 @@ int stage_query(vsb_index *ix, Slot *slot, const void *query, cudaStream_t ss) {
     return VSB_OK;
 }
 
-// ---- streamed index: the window loop.  Window w (rows [w * win_rows, ...)) is copied into d_win[w & 1] on the copy stream
-// while window w-1 is being scanned; a window is scanned exactly like a shard (scan + filter into a result slot), its survivors
-// carry window-local rows.  visit(w, first_row, rows, slot) is called in window order once the slot's head is on the host.
+// ---- the view loop.  A view is rows [r0, r0 + rows) of the column in device memory at vec.  A resident index is one view, its
+// whole column in d_vec.  A streamed index is one view per window: window w (rows [w * win_rows, ...)) is copied into
+// d_win[w & 1] on the copy stream while window w-1 is being scanned, and its scan reads the window buffer with window-local rows.
+struct View {
+    long long index;      // window number
+    long long r0, rows;   // shard row of the view's first row, and its rows
+    const uint8_t *vec;
+    int buf;              // window buffer, 0 or 1
+    int slot;             // index % depth
+};
+
+// launch(view) enqueues the work of each view; visit(view) is called in view order, for a streamed index once `depth` later
+// views are enqueued or the loop ends (a visit that waits for its view's result frees the slot that view index + depth uses).
 // host_clock: add the loop's host time to stream_us, which measures the stream only when the visits wait for the windows (the
-// batch path waits for nothing here and times its windows with events, batch_account)
+// batch path waits for nothing here and times its windows with events, batch_account).  A resident view copies nothing and
+// counts no stream time or bytes.
 template <class Launch, class Visit>
-int stream_windows(vsb_index *ix, int depth, Launch launch, Visit visit, bool host_clock = true) {
+int for_each_view(vsb_index *ix, int depth, Launch launch, Visit visit, bool host_clock = true) {
+    if (!ix->streamed) {
+        const View v{0, 0, ix->n, ix->d_vec, 0, 0};
+        const int rc = launch(v);
+        return rc ? rc : visit(v);
+    }
+    const auto view_of = [&](long long w) {
+        const long long r0 = w * ix->win_rows;
+        return View{w, r0, std::min(ix->win_rows, ix->n - r0), ix->d_win[w & 1].get(), (int)(w & 1), (int)(w % depth)};
+    };
     const long long W = (ix->n + ix->win_rows - 1) / ix->win_rows;
     const auto t0 = std::chrono::steady_clock::now();
     long long next_visit = 0;
     for (long long w = 0; w < W; ++w) {
-        const int b = (int)(w & 1);
-        const long long r0 = w * ix->win_rows, rows = std::min(ix->win_rows, ix->n - r0);
-        if (w >= 2) CU(cudaStreamWaitEvent(ix->cstream, ix->win_scanned[b], 0));       // the scan of window w-2 has read this buffer
-        CU(cudaMemcpyAsync(ix->d_win[b], ix->h_arena + (size_t)r0 * ix->pitch, (size_t)rows * ix->pitch, cudaMemcpyHostToDevice, ix->cstream));
-        CU(cudaEventRecord(ix->win_copied[b], ix->cstream));
-        CU(cudaStreamWaitEvent(ix->stream, ix->win_copied[b], 0));
-        while (w - next_visit >= depth) {                                                // free the slot this window will use
-            const int rc = visit(next_visit, next_visit * ix->win_rows, std::min(ix->win_rows, ix->n - next_visit * ix->win_rows), (int)(next_visit % depth));
+        const View v = view_of(w);
+        if (w >= 2) CU(cudaStreamWaitEvent(ix->cstream, ix->win_scanned[v.buf], 0));   // the scan of window w-2 has read this buffer
+        CU(cudaMemcpyAsync(ix->d_win[v.buf], ix->h_arena + (size_t)v.r0 * ix->pitch, (size_t)v.rows * ix->pitch, cudaMemcpyHostToDevice, ix->cstream));
+        CU(cudaEventRecord(ix->win_copied[v.buf], ix->cstream));
+        CU(cudaStreamWaitEvent(ix->stream, ix->win_copied[v.buf], 0));
+        for (; w - next_visit >= depth; ++next_visit) {                                  // free the slot this window will use
+            const int rc = visit(view_of(next_visit));
             if (rc) return rc;
-            ++next_visit;
         }
-        const int rc = launch(w, ix->d_win[b], rows, (int)(w % depth));
+        const int rc = launch(v);
         if (rc) return rc;
-        CU(cudaEventRecord(ix->win_scanned[b], ix->stream));
-        ix->st_stream_bytes += rows * ix->pitch;
+        CU(cudaEventRecord(ix->win_scanned[v.buf], ix->stream));
+        ix->st_stream_bytes += v.rows * ix->pitch;
     }
     for (; next_visit < W; ++next_visit) {
-        const int rc = visit(next_visit, next_visit * ix->win_rows, std::min(ix->win_rows, ix->n - next_visit * ix->win_rows), (int)(next_visit % depth));
+        const int rc = visit(view_of(next_visit));
         if (rc) return rc;
     }
     if (host_clock) ix->st_stream_us += std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t0).count();
     return VSB_OK;
 }
 
-// all distances of a streamed index (stream modules, overflow fallback)
-int streamed_scan_all(vsb_index *ix, int metric, const uint8_t *d_query, float *out_dist) {
+// the visit of a view loop that waits for nothing: its work stays enqueued, the caller waits for the stream once
+int no_visit(const View &) { return VSB_OK; }
+
+// all distances of the column (stream modules, overflow fallback).  The distances of a view sit in half buf of d_dist_all
+// (resident: win_rows is 0, the whole buffer); each copy is ordered behind its view's scan on the same stream.
+int scan_all_into(vsb_index *ix, int metric, const uint8_t *d_query, std::vector<float> &dist) {
     const int rc = ensure_dist_all(ix);
     if (rc) return rc;
-    return stream_windows(ix, 2,
-        [&](long long, const uint8_t *vec, long long rows, int s) {
-            return launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all + (size_t)s * ix->win_rows, false, ix->stream, false, vec, rows);
+    dist.resize((size_t)ix->n);
+    return for_each_view(ix, 2,
+        [&](const View &v) {
+            return launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all + (size_t)v.buf * ix->win_rows, false, ix->stream, false, v.vec, v.rows, v.r0);
         },
-        [&](long long, long long r0, long long rows, int s) {
-            // distances of window w sit in half s of d_dist_all; the copy is ordered behind that window's scan on the same stream
-            CU(cudaMemcpyAsync(out_dist + r0, ix->d_dist_all + (size_t)s * ix->win_rows, sizeof(float) * (size_t)rows, cudaMemcpyDeviceToHost, ix->stream));
+        [&](const View &v) {
+            CU(cudaMemcpyAsync(dist.data() + v.r0, ix->d_dist_all + (size_t)v.buf * ix->win_rows, sizeof(float) * (size_t)v.rows, cudaMemcpyDeviceToHost, ix->stream));
             CU(cudaStreamSynchronize(ix->stream));
-            return (int)VSB_OK;
-        });
-}
-
-// candidates of a streamed index: every window's survivors, in scan order, rows made column-global
-int streamed_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k, std::vector<uint2> &cands, bool *overflow) {
-    *overflow = false;
-    const int depth = 4;                                  // result slots 0..3 rotate over the windows
-    return stream_windows(ix, depth,
-        [&](long long w, const uint8_t *vec, long long rows, int s) {
-            return launch_scan(ix, metric, d_query, k, &ix->slot[s], nullptr, true, ix->stream, false, vec, rows, w * ix->win_rows);
-        },
-        [&](long long, long long r0, long long, int s) {
-            bool ovf = false;
-            const int rc = visit_survivors(ix, &ix->slot[s], &ovf, [&](uint2 c) { cands.push_back(make_uint2(c.x, c.y + (uint32_t)r0)); });
-            if (rc) return rc;
-            if (ovf) *overflow = true;
             return (int)VSB_OK;
         });
 }
@@ -830,14 +851,9 @@ struct FilterScope {
 
 int filter_begin(vsb_index *ix, const uint32_t *bits, FilterScope *scope) {
     CU(cudaSetDevice(ix->device));
-    const size_t words = (size_t)((ix->n + 31) / 32) + 1;
-    if (words > ix->allow_words) {        // filtered calls are synchronous: no launch still reads the old buffer
-        DeviceBuf<uint32_t> d;
-        CU(d.alloc(4 * words));
-        ix->dev_bytes += 4 * (words - ix->allow_words);
-        ix->d_allow = std::move(d);
-        ix->allow_words = words;
-    }
+    const long long words = (ix->n + 31) / 32 + 1;
+    const int rc = grow_buf(ix->d_allow, ix->allow_words, words, &ix->dev_bytes);
+    if (rc) return rc;
     if (words > 1) CU(cudaMemcpyAsync(ix->d_allow, bits, 4 * (words - 1), cudaMemcpyHostToDevice, ix->stream));
     CU(cudaMemsetAsync(ix->d_allow + (words - 1), 0, 4, ix->stream));
     CU(cudaStreamSynchronize(ix->stream));   // the scans of a group may run on the second scan stream
@@ -891,12 +907,15 @@ int query_candidates(vsb_index *ix, int metric, const void *query, int k, std::v
     bool overflow = false;
     rc = ensure_workspace(ix, k);
     if (rc) return rc;
-    if (ix->streamed) {
-        rc = streamed_candidates(ix, metric, slot->d_query, k, cands, &overflow);
-    } else {
-        rc = launch_scan(ix, metric, slot->d_query, k, slot, nullptr, true, ix->stream);
-        if (rc == VSB_OK) rc = visit_survivors(ix, slot, &overflow, [&](uint2 c) { cands.push_back(c); });
-    }
+    // every view's survivors in scan order, rows made column-global; a streamed index rotates result slots 0..3 over its windows
+    rc = for_each_view(ix, ix->streamed ? 4 : 1,
+        [&](const View &v) { return launch_scan(ix, metric, slot->d_query, k, &ix->slot[v.slot], nullptr, true, ix->stream, false, v.vec, v.rows, v.r0); },
+        [&](const View &v) {
+            bool ovf = false;
+            const int r = visit_survivors(ix, &ix->slot[v.slot], &ovf, [&](uint2 c) { cands.push_back(make_uint2(c.x, c.y + (uint32_t)v.r0)); });
+            if (ovf) overflow = true;
+            return r;
+        });
     if (rc) return rc;
     return overflow ? all_candidates(ix, metric, slot->d_query, cands) : VSB_OK;
 }
@@ -948,24 +967,50 @@ float range_threshold(double r) {
     return t;
 }
 
-// the pair list holds at least cap pairs (grown, never shrunk; range calls are synchronous, no launch reads the old list)
-int ensure_range(vsb_index *ix, long long cap) {
-    if (!ix->d_range_count) {
+// the pair list holds at least cap pairs (grow_buf)
+int pair_list_reserve(vsb_index *ix, long long cap) {
+    PairList &pl = ix->plist;
+    if (!pl.d_count) {
         DeviceBuf<unsigned> d;
         HostBuf<unsigned> h;
         CU(d.alloc(sizeof(unsigned)));
         CU(h.alloc(sizeof(unsigned)));
-        ix->d_range_count = std::move(d);
-        ix->h_range_count = std::move(h);
+        pl.d_count = std::move(d);
+        pl.h_count = std::move(h);
         ix->dev_bytes += sizeof(unsigned);
     }
-    if (cap <= ix->range_cap) return VSB_OK;
-    DeviceBuf<uint2> d;
-    CU(d.alloc(sizeof(uint2) * (size_t)cap));
-    ix->dev_bytes += sizeof(uint2) * (size_t)(cap - ix->range_cap);
-    ix->d_range = std::move(d);
-    ix->range_cap = cap;
+    return grow_buf(pl.d_pairs, pl.cap, cap, &ix->dev_bytes);
+}
+
+int pair_list_reset(vsb_index *ix) {
+    CU(cudaMemsetAsync(ix->plist.d_count, 0, sizeof(unsigned), ix->stream));
     return VSB_OK;
+}
+
+// One query into the pair list, which first grows to first_cap pairs: the counter is reset, fill() appends on ix->stream and the
+// count comes back in *count.  A count above the list's capacity grows the list to exactly that count, adds one to *regrows
+// and calls refill() once, which writes the list again (resetting the counter itself if it appends everything again).  A count
+// that still does not fit is an error; `what` names the caller in its message.
+template <class Fill, class Refill>
+int pair_list_run(vsb_index *ix, long long first_cap, const char *what, long long *regrows, Fill fill, Refill refill, long long *count) {
+    PairList &pl = ix->plist;
+    const auto read_count = [&]() -> int {
+        CU(cudaMemcpyAsync(pl.h_count, pl.d_count, sizeof(unsigned), cudaMemcpyDeviceToHost, ix->stream));
+        CU(cudaStreamSynchronize(ix->stream));
+        *count = *pl.h_count;
+        return VSB_OK;
+    };
+    int rc = pair_list_reserve(ix, first_cap);
+    if (rc == VSB_OK) rc = pair_list_reset(ix);
+    if (rc == VSB_OK) rc = fill();
+    if (rc == VSB_OK) rc = read_count();
+    if (rc || *count <= pl.cap) return rc;
+    ++*regrows;
+    rc = pair_list_reserve(ix, *count);
+    if (rc == VSB_OK) rc = refill();
+    if (rc == VSB_OK) rc = read_count();
+    if (rc == VSB_OK && *count > pl.cap) return fail(VSB_ECUDA, "%s: %lld pairs after growing the list to %lld", what, *count, pl.cap);
+    return rc;
 }
 
 // one range-mode scan over rows [0, n) of vec, whose first row is shard row r0, appending to the pair list on ix->stream
@@ -977,27 +1022,16 @@ int launch_range(vsb_index *ix, int metric, const uint8_t *d_query, float t, con
     ScanFn fn = pick_kernel(ix->vtype, mc, pl.direct, true);
     if (!fn) return fail(VSB_EINVAL, "unsupported vector type %d", ix->vtype);
     CU((cudaError_t)set_smem_limit((const void *)fn, pl.smem));
-    ScanParams p{};
-    p.vec = vec;
-    p.n = n;
-    p.pitch = ix->pitch;
-    p.nc = ix->pitch / 16;
-    p.log2P = pl.log2P;
-    p.wtile_bytes = pl.wtile_bytes;
-    p.nsw = pl.nsw;
-    p.root = root;
-    p.query = d_query;
-    p.allow = ix->flt_d;
-    p.allow_base = r0;
+    ScanParams p = scan_params(ix, pl, root, d_query, vec, n, r0);
     p.range_t = t;
-    p.range_pairs = ix->d_range;
-    p.range_count = ix->d_range_count;
-    p.range_cap = ix->range_cap;
+    p.range_pairs = ix->plist.d_pairs;
+    p.range_count = ix->plist.d_count;
+    p.range_cap = ix->plist.cap;
     p.range_row_base = (unsigned)r0;
     fn<<<ix->num_sms, kThreads, pl.smem, ix->stream>>>(p);
     CU(cudaGetLastError());
     ++g_launches;
-    ix->last_log2p = pl.log2P; ix->last_nsw = pl.nsw; ix->last_direct = pl.direct ? 1 : 0;
+    note_plan(ix, pl);
     return VSB_OK;
 }
 
@@ -1019,42 +1053,30 @@ int range_query(vsb_index *ix, int metric, const uint8_t *d_query, double r, std
     out.clear();
     const float t = range_threshold(r);
     if (ix->n == 0 || t == -INFINITY) return VSB_OK;            // nothing is below -INF (and NaN radii select nothing)
-    int rc = ensure_range(ix, kRangeCap0);
+    const auto scan = [&]() {
+        return for_each_view(ix, 2, [&](const View &v) { return launch_range(ix, metric, d_query, t, v.vec, v.rows, v.r0); }, no_visit);
+    };
+    long long cnt = 0;
+    const int rc = pair_list_run(ix, kRangeCap0, "range scan", &ix->st_range_passes, scan,
+        [&]() {
+            const int r = pair_list_reset(ix);
+            return r ? r : scan();
+        }, &cnt);
     if (rc) return rc;
-    unsigned cnt = 0;
-    for (int pass = 0;; ++pass) {
-        CU(cudaMemsetAsync(ix->d_range_count, 0, sizeof(unsigned), ix->stream));
-        if (ix->streamed) {
-            rc = stream_windows(ix, 2,
-                [&](long long w, const uint8_t *vec, long long rows, int) { return launch_range(ix, metric, d_query, t, vec, rows, w * ix->win_rows); },
-                [&](long long, long long, long long, int) { return (int)VSB_OK; });
-        } else {
-            rc = launch_range(ix, metric, d_query, t, ix->d_vec, ix->n, 0);
-        }
-        if (rc) return rc;
-        CU(cudaMemcpyAsync(ix->h_range_count, ix->d_range_count, sizeof(unsigned), cudaMemcpyDeviceToHost, ix->stream));
-        CU(cudaStreamSynchronize(ix->stream));
-        cnt = *ix->h_range_count;
-        if ((long long)cnt <= ix->range_cap) break;
-        if (pass > 0) return fail(VSB_ECUDA, "range scan: %u pairs after growing the list to %lld", cnt, ix->range_cap);
-        ix->st_range_passes++;
-        rc = ensure_range(ix, (long long)cnt);
-        if (rc) return rc;
-    }
-    if (cnt >= 2 && cnt <= (unsigned)kRangeSortCap) {
+    if (cnt >= 2 && cnt <= kRangeSortCap) {
         size_t n2 = 2;
         while (n2 < cnt) n2 <<= 1;
         const size_t smem = sizeof(unsigned long long) * n2;
         CU((cudaError_t)set_smem_limit((const void *)range_sort_kernel, smem));
-        RangeSortParams sp{ix->d_range, ix->d_range_count, 0, nullptr, nullptr};
+        RangeSortParams sp{ix->plist.d_pairs, ix->plist.d_count, 0, nullptr, nullptr};
         range_sort_kernel<<<1, kRangeSortThreads, smem, ix->stream>>>(sp);
         CU(cudaGetLastError());
         ++g_launches;
     }
-    out.resize(cnt);
-    if (cnt > 0) CU(cudaMemcpyAsync(out.data(), ix->d_range, sizeof(uint2) * (size_t)cnt, cudaMemcpyDeviceToHost, ix->stream));
+    out.resize((size_t)cnt);
+    if (cnt > 0) CU(cudaMemcpyAsync(out.data(), ix->plist.d_pairs, sizeof(uint2) * (size_t)cnt, cudaMemcpyDeviceToHost, ix->stream));
     CU(cudaStreamSynchronize(ix->stream));
-    if (cnt > (unsigned)kRangeSortCap) {
+    if (cnt > kRangeSortCap) {
         ix->st_range_host_sorts++;
         range_sort_host(out.data(), out.size());
     }
@@ -1108,14 +1130,7 @@ int ensure_large_k(vsb_index *ix, long long rows) {
         ix->dev_bytes += kLkHistBytes + sizeof(LkState);
     }
     const long long blocks = std::max<long long>(1, (rows + kLkRows - 1) / kLkRows);
-    if (blocks > ix->lk_boff_cap) {
-        DeviceBuf<unsigned> d;
-        CU(d.alloc(sizeof(unsigned) * (size_t)blocks));
-        ix->dev_bytes += sizeof(unsigned) * (size_t)(blocks - ix->lk_boff_cap);
-        ix->d_lk_boff = std::move(d);
-        ix->lk_boff_cap = blocks;
-    }
-    return VSB_OK;
+    return grow_buf(ix->d_lk_boff, ix->lk_boff_cap, blocks, &ix->dev_bytes);
 }
 
 // the candidates of one view (its n distances at dist, its first row shard row r0) appended to the pair list on ix->stream:
@@ -1134,9 +1149,9 @@ int large_k_view(vsb_index *ix, const float *dist, long long n, long long r0, in
     p.hist = ix->d_lk_hist;
     p.st = ix->d_lk_state;
     p.boff = ix->d_lk_boff;
-    p.total = ix->d_range_count;
-    p.out = ix->d_range;
-    p.cap = ix->range_cap;
+    p.total = ix->plist.d_count;
+    p.out = ix->plist.d_pairs;
+    p.cap = ix->plist.cap;
     p.row_base = (unsigned)r0;
     p.nblocks = (int)((n + kLkRows - 1) / kLkRows);
     if (!write_only) {
@@ -1176,47 +1191,31 @@ int large_k_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k,
     const long long expect = views * k * (2 + (long long)std::log2(std::max(1.0, (double)view / k)));
     int rc = ensure_dist_all(ix);
     if (rc == VSB_OK) rc = ensure_large_k(ix, view);
-    if (rc == VSB_OK) rc = ensure_range(ix, std::max(kRangeCap0, std::min(ix->n, 2 * expect)));
     if (rc) return rc;
-    for (int pass = 0;; ++pass) {
-        CU(cudaMemsetAsync(ix->d_range_count, 0, sizeof(unsigned), ix->stream));
-        if (ix->streamed) {
-            rc = stream_windows(ix, 2,
-                [&](long long w, const uint8_t *vec, long long rows, int s) {
-                    float *dist = ix->d_dist_all + (size_t)s * ix->win_rows;
-                    const int r = launch_scan(ix, metric, d_query, 0, nullptr, dist, false, ix->stream, false, vec, rows, w * ix->win_rows);
-                    return r ? r : large_k_view(ix, dist, rows, w * ix->win_rows, k);
-                },
-                [&](long long, long long, long long, int) { return (int)VSB_OK; });
-        } else {
-            rc = launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all, false, ix->stream);
-            if (rc == VSB_OK) rc = large_k_view(ix, ix->d_dist_all, ix->n, 0, k);
-        }
-        if (rc) return rc;
-        CU(cudaMemcpyAsync(ix->h_range_count, ix->d_range_count, sizeof(unsigned), cudaMemcpyDeviceToHost, ix->stream));
-        CU(cudaStreamSynchronize(ix->stream));
-        const long long cnt = *ix->h_range_count;
-        if (cnt <= ix->range_cap) break;
-        if (pass > 0) return fail(VSB_ECUDA, "large-k candidates: %lld pairs after growing the list to %lld", cnt, ix->range_cap);
-        ix->st_large_k_regrows++;
-        rc = ensure_range(ix, cnt);
-        if (rc) return rc;
-        if (!ix->streamed) {
-            rc = large_k_view(ix, ix->d_dist_all, ix->n, 0, k, true);
-            if (rc) return rc;
-            break;
-        }
-    }
-    const long long cnt = *ix->h_range_count;
-    if (cnt > ix->h_lk_cap) {
-        HostBuf<uint2> h;
-        CU(h.alloc(sizeof(uint2) * (size_t)cnt));
-        ix->h_lk = std::move(h);
-        ix->h_lk_cap = cnt;
-    }
-    if (cnt > 0) CU(cudaMemcpyAsync(ix->h_lk, ix->d_range, sizeof(uint2) * (size_t)cnt, cudaMemcpyDeviceToHost, ix->stream));
+    // the distances of a view sit in half buf of d_dist_all (resident: win_rows is 0, the whole buffer)
+    const auto scan = [&]() {
+        return for_each_view(ix, 2,
+            [&](const View &v) {
+                float *dist = ix->d_dist_all + (size_t)v.buf * ix->win_rows;
+                const int r = launch_scan(ix, metric, d_query, 0, nullptr, dist, false, ix->stream, false, v.vec, v.rows, v.r0);
+                return r ? r : large_k_view(ix, dist, v.rows, v.r0, k);
+            },
+            no_visit);
+    };
+    long long cnt = 0;
+    rc = pair_list_run(ix, std::max(kRangeCap0, std::min(ix->n, 2 * expect)), "large-k candidates", &ix->st_large_k_regrows, scan,
+        [&]() {
+            // a resident column's distances are still in HBM: only the compaction's write runs again.  A streamed column's
+            // windows have been overwritten and run again.
+            if (!ix->streamed) return large_k_view(ix, ix->d_dist_all, ix->n, 0, k, true);
+            const int r = pair_list_reset(ix);
+            return r ? r : scan();
+        }, &cnt);
+    if (rc == VSB_OK) rc = grow_buf(ix->plist.h_pairs, ix->plist.h_cap, cnt, nullptr);
+    if (rc) return rc;
+    if (cnt > 0) CU(cudaMemcpyAsync(ix->plist.h_pairs, ix->plist.d_pairs, sizeof(uint2) * (size_t)cnt, cudaMemcpyDeviceToHost, ix->stream));
     CU(cudaStreamSynchronize(ix->stream));
-    cands.assign(ix->h_lk.get(), ix->h_lk.get() + cnt);
+    cands.assign(ix->plist.h_pairs.get(), ix->plist.h_pairs.get() + cnt);
     ix->st_large_k_cands += cnt;
     return VSB_OK;
 }

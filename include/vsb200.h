@@ -102,7 +102,10 @@ VSB_API void vsb_index_free(vsb_index *ix);
  * refined exactly and results are the same as nq single calls.
  * k > 256 (any nq, one query at a time): the all-distances scan, then on the device the exact k-th distance of every prefix
  * [0, k 2^j) of the column and the rows below their segment's bound in scan order (DESIGN §3.11); the host replays only those.
- * Results are the same bits as a replay over every row ("large_k_queries", "large_k_cands", "large_k_regrows"). */
+ * Results are the same bits as a replay over every row ("large_k_queries", "large_k_cands", "large_k_regrows").
+ * k > 256 with nq >= 16 where the batch path above runs: the batch levels find every query's candidates with per-query bounds,
+ * one pass of the column per batch (DESIGN §3.12), and the host replays each query's; the same bits as nq single calls
+ * ("large_k_batches", "large_k_batch_fallbacks", "large_k_query_fallbacks"). */
 VSB_API int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k, int64_t *out_rowids,
                           double *out_dist, int *out_counts, int *max_index);
 
@@ -286,7 +289,11 @@ VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row o
  * pass), "range_host_sorts" (range results too long for the GPU sort, ordered on the host), "range_batches",
  * "range_batch_fallbacks", "range_query_fallbacks" (see vsb_scan_range), "large_k_queries" (queries with k > 256),
  * "large_k_cands" (their candidates replayed on the host), "large_k_regrows" (large-k queries whose candidates outgrew the pair
- * list, which then grew to the exact count)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * list, which then grew to the exact count), "large_k_batches" (calls whose k > 256 queries took the batch levels),
+ * "large_k_batch_fallbacks" (such calls answered query by query: a candidate log overflowed), "large_k_query_fallbacks" (queries
+ * of such a batch answered alone: their bucket or a sort segment overflowed), "large_k_levels_us" (host clock around the batch
+ * levels, sort and candidate copy, which end in a stream synchronise), "large_k_replay_us" (host clock around the threaded slot
+ * replay of such batches; a group counts it on its first shard), "large_k_replay_threads" (host threads of the last replay)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
  * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */
@@ -301,7 +308,11 @@ VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches,
 /* diagnostics: copies an internal device buffer of the most recent single-query scan to `out`; name in {"cta_time" (unsigned
  * cycles per scan CTA), "bounds" (int64 tile boundaries of the adaptive row partition), "topk_bounds" (the most recent k > 256
  * view, a resident column or one streamed window: int64 segment count S, int64 segment ends[32] (the first S used), float
- * bounds[32] (segment 0: +INF, segment s: the k-th distance of rows [0, ends[s - 1])))}.  Returns the bytes copied or < 0. */
+ * bounds[32] (segment 0: +INF, segment s: the k-th distance of rows [0, ends[s - 1]))), "large_k_batch_bounds" (the most recent
+ * large-k batch on this index: int64 piece count P, int64 query count Q, int64 [P][3] each piece's shard rows [first, end) and
+ * level, float [P][Q] the bound each piece was refined against, +INF for level 0), "large_k_batch_cands" (the same batch's
+ * candidates: int64 query count Q, int64 [Q] each query's count (-1: answered alone), then the queries' (uint32 distance bits,
+ * uint32 shard row) pairs in scan order, query after query)}.  Returns the bytes copied or < 0. */
 VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes);
 /* diagnostics: the counterpart of vsb_debug_read for name "bounds": plants a row partition (int64 tile boundaries, one per scan
  * CTA plus one, non-decreasing from 0 to the tile count of the k <= 32 plan; vsb_index_stat "sms" CTAs) into every scan

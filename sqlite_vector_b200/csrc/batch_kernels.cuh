@@ -658,6 +658,114 @@ __global__ void refine_kernel(const RefineParams rp) {
     }
 }
 
+// ------------------------------------------------------------------ large-k batches (batch_large_k, DESIGN §3.12)
+// The refinement of a large-k batch computes every distance exactly as the single-query large-k path's scan_kernel does (plan
+// make_plan(ix, 0)): 1 << log2P lanes per row, lane p owning chunks p + (i << log2P) taken in the order rotated by the row's
+// position in its warp tile, (view-local row mod rows per warp) mod chunks (for a DIRECT plan, one row per warp, that is 0),
+// accum_reduce over those lanes, the query norm of row_norm_kernel (scan_kernel's lane-strided sum), finalize and the
+// special-value rows.  So a batch keeps and replays the same distance bits as single calls, for every element type.
+struct PlanRefineParams {
+    RefineParams r;          // candidates, rows, queries, bounds and buckets as refine_kernel
+    int log2P;               // lanes per row of the single-query plan
+    long long lrow0;         // view-local row of r.vec's first row (the rotation counts rows from the view's start)
+    const void *qnorm;       // [nq] the queries' sums of squares (float, or int for u8 / i8); nullptr for L1
+};
+
+template <int VT, int MC>
+__device__ __noinline__ float plan_special_row_distance(const uint8_t *row, const uint8_t *query, int nelem, int root) {
+    return special_row_distance_body<VT, MC>(row, query, nelem, root);
+}
+
+template <int VT, int MC>
+__global__ void __launch_bounds__(256) plan_refine_kernel(const PlanRefineParams pp) {
+    const RefineParams &rp = pp.r;
+    const unsigned ncand_raw = *rp.cand_count;
+    const unsigned ncand = min(ncand_raw, rp.cand_cap);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        atomicAdd(&rp.stats[0], ncand);
+        if (ncand_raw > rp.cand_cap) atomicOr(&rp.stats[2], 1u);
+    }
+    const int log2P = pp.log2P, P = 1 << log2P, rpw = 32 >> log2P;
+    const int lane = threadIdx.x & 31, grp = lane >> log2P, p = lane & (P - 1);
+    const int nc = rp.pitch / 16;
+    const int cnt = (nc > p) ? (nc - p + P - 1) >> log2P : 0;               // chunks owned by this lane
+    const unsigned wpb = blockDim.x >> 5;
+    const unsigned steps = (ncand + rpw - 1) / rpw;
+    for (unsigned st = blockIdx.x * wpb + (threadIdx.x >> 5); st < steps; st += gridDim.x * wpb) {
+        const unsigned c = st * rpw + grp;
+        const bool live = c < ncand;
+        uint2 cq = make_uint2(0, 0);
+        if (live) cq = rp.cand[c];
+        const uint8_t *rowp = rp.vec + (size_t)cq.x * rp.pitch, *qp = rp.queries + (size_t)cq.y * rp.pitch;
+        Accum A = {0.f, 0.f, 0.f, 0, 0};
+        if (live) {
+            const int i0 = cnt ? (int)((pp.lrow0 + cq.x) % rpw) % cnt : 0;
+            for (int i = 0; i < cnt; ++i) {
+                int ii = i0 + i;
+                if (ii >= cnt) ii -= cnt;
+                const int ch = p + (ii << log2P);
+                accum16<VT, MC>(A, __ldg(reinterpret_cast<const uint4 *>(rowp) + ch), __ldg(reinterpret_cast<const uint4 *>(qp) + ch));
+            }
+        }
+        accum_reduce(A, P);
+        QueryNorm qn = {0.f, 0};
+        if (live && pp.qnorm) {
+            if constexpr (VT == T_U8 || VT == T_I8) qn.i = reinterpret_cast<const int *>(pp.qnorm)[cq.y];
+            else qn.f = reinterpret_cast<const float *>(pp.qnorm)[cq.y];
+        }
+        float d = finalize<VT, MC>(A, qn, rp.root);
+        if constexpr (has_special_policy<VT, MC>()) {
+            if (live && p == 0 && row_needs_exact<VT, MC>(A, qn)) d = plan_special_row_distance<VT, MC>(rowp, qp, rp.pitch / 2, rp.root);
+        }
+        if (live && p == 0 && d < rp.U[cq.y]) {
+            const unsigned w = atomicAdd(&rp.bcount[cq.y], 1u);
+            if (w < rp.bucket_cap) rp.bucket[(size_t)cq.y * rp.bucket_cap + w] = make_uint2(cq.x + rp.row_base, __float_as_uint(d));
+        }
+    }
+}
+
+// One block per query: U[q] = the k-th smallest distance (fkey order) among the query's first min(bcount[q], cap) bucket entries,
+// +INF when there are fewer than k; a radix select of 4 digits of 8 bits, most significant first.  Any subset of the eligible rows
+// before the next level gives a valid bound (DESIGN §3.12), so an overflowed bucket's first entries serve too.  U_log[q] keeps a
+// copy (vsb_debug_read "large_k_batch_bounds").
+constexpr int kLkbBoundThreads = 256;
+__global__ void __launch_bounds__(kLkbBoundThreads) lkb_bound_kernel(const uint2 *bucket, long long stride, const unsigned *bcount,
+                                                                     unsigned cap, int k, float *U, float *U_log) {
+    __shared__ unsigned hist[256];
+    __shared__ unsigned sel_s, rank_s;
+    const int q = blockIdx.x;
+    const unsigned n = min(bcount[q], cap);
+    const uint2 *b = bucket + (size_t)q * (size_t)stride;
+    if (n < (unsigned)k) {
+        if (threadIdx.x == 0) { U[q] = INFINITY; U_log[q] = INFINITY; }
+        return;
+    }
+    if (threadIdx.x == 0) { sel_s = 0u; rank_s = (unsigned)k; }
+    for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 24 - 8 * pass;
+        for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0u;
+        __syncthreads();
+        const unsigned sel = sel_s;
+        for (unsigned i = threadIdx.x; i < n; i += blockDim.x) {
+            const uint32_t key = fkey(__uint_as_float(b[i].y));
+            if (pass == 0 || (key >> (shift + 8)) == (sel >> (shift + 8))) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned rank = rank_s, d = 0;
+            while (hist[d] < rank) rank -= hist[d++];
+            sel_s = sel | (d << shift);
+            rank_s = rank;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        const float u = funkey(sel_s);
+        U[q] = u;
+        U_log[q] = u;
+    }
+}
+
 // final exchange sort of each query's slots, literally the loop of vFullScanSortSlots (src/sqlite-vector.c:2057-2065):
 // one thread per query, its k slots staged in shared memory.  Unused slots stay +INF and sort to the end.
 __global__ void final_sort_kernel(float *slot_d, unsigned *slot_row, int nq, int k, int kcap) {

@@ -242,6 +242,8 @@ struct vsb_index {
     DeviceBuf<LkState> d_lk_state;
     long long lk_boff_cap = 0;
     long long st_large_k_queries = 0, st_large_k_cands = 0, st_large_k_regrows = 0;
+    long long st_large_k_batches = 0, st_large_k_batch_fallbacks = 0, st_large_k_query_fallbacks = 0;   // DESIGN §3.12
+    long long st_large_k_levels_us = 0, st_large_k_replay_us = 0, st_large_k_replay_threads = 0;
 };
 
 // result of a range call (vsb_scan_range): per query, rowids and distances in result order
@@ -1500,6 +1502,12 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "large_k_queries")) return ix->st_large_k_queries;
     if (!strcmp(name, "large_k_cands")) return ix->st_large_k_cands;
     if (!strcmp(name, "large_k_regrows")) return ix->st_large_k_regrows;
+    if (!strcmp(name, "large_k_batches")) return ix->st_large_k_batches;
+    if (!strcmp(name, "large_k_batch_fallbacks")) return ix->st_large_k_batch_fallbacks;
+    if (!strcmp(name, "large_k_query_fallbacks")) return ix->st_large_k_query_fallbacks;
+    if (!strcmp(name, "large_k_levels_us")) return ix->st_large_k_levels_us;
+    if (!strcmp(name, "large_k_replay_us")) return ix->st_large_k_replay_us;
+    if (!strcmp(name, "large_k_replay_threads")) return ix->st_large_k_replay_threads;
     return -1;
 }
 void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullptr; }
@@ -1529,6 +1537,16 @@ int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k,
         if (rc == VSB_OK) return VSB_OK;
         if (rc != VSB_ERANGE) return rc;
         ix->st_fallbacks++;                      // capacity exceeded: per-query path below
+    }
+    LkbPlan lkb;
+    if (large_k_batch_supported(ix, metric, nq, k, lkb)) {   // k > kMaxK: the large-k batch (DESIGN §3.12), every query from max_index 0
+        std::vector<std::vector<uint2>> all;
+        const int rc = large_k_index(ix, metric, queries, nq, k, lkb, all);
+        if (rc) return rc;
+        replay_queries(ix, nq, k, out_rowids, out_dist, out_counts, [&](int q, SlotState &s) {
+            slots_offer_cands(s, all[(size_t)q].data(), all[(size_t)q].size(), [&](uint32_t row) { return rowid_of(ix, row); });
+        });
+        return VSB_OK;
     }
     std::vector<uint2> cands;
     QueryCursor cur(max_index, nq);
@@ -1659,6 +1677,28 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
     if (!strcmp(name, "cta_time")) { src = w.d_cta_time; have = sizeof(unsigned) * (size_t)ix->num_sms; }
     else if (!strcmp(name, "bounds")) { src = w.d_bounds; have = sizeof(long long) * (size_t)(ix->num_sms + 1); }
     else if (!strcmp(name, "topk_bounds")) { src = ix->d_lk_state; have = offsetof(LkState, sel); }   // segments and bounds of the last large-k view
+    else if (!strcmp(name, "large_k_batch_bounds")) {                   // host copy: pieces and bounds of the last large-k batch
+        if (!ix->batch || ix->batch->lkb_debug.empty()) return fail(VSB_EINVAL, "no large-k batch has run yet");
+        const std::vector<uint8_t> &d = ix->batch->lkb_debug;
+        memcpy(out, d.data(), std::min<size_t>(d.size(), (size_t)bytes));
+        return (int)std::min<size_t>(d.size(), (size_t)bytes);
+    }
+    else if (!strcmp(name, "large_k_batch_cands")) {                    // host copy: every query's candidates of the last large-k batch
+        if (!ix->batch || ix->batch->lkb_cnt.empty()) return fail(VSB_EINVAL, "no large-k batch has run yet");
+        const BatchWs &b = *ix->batch;
+        std::vector<uint8_t> d(8 + 8 * b.lkb_cnt.size());
+        const long long nq = (long long)b.lkb_cnt.size();
+        memcpy(d.data(), &nq, 8);
+        memcpy(d.data() + 8, b.lkb_cnt.data(), 8 * b.lkb_cnt.size());
+        for (size_t q = 0; q < b.lkb_cnt.size(); ++q)
+            if (b.lkb_cnt[q] > 0) {
+                const uint8_t *src = reinterpret_cast<const uint8_t *>(b.h_kout.get() + b.lkb_off[q]);
+                d.insert(d.end(), src, src + sizeof(uint2) * (size_t)b.lkb_cnt[q]);
+            }
+        const size_t n = std::min<size_t>({d.size(), (size_t)bytes, (size_t)INT32_MAX});
+        memcpy(out, d.data(), n);
+        return (int)n;
+    }
     else return fail(VSB_EINVAL, "unknown debug buffer %s", name);
     if (!src) return fail(VSB_EINVAL, "no %s has run yet", strcmp(name, "topk_bounds") ? "scan" : "large-k query");
     CU(cudaMemcpy(out, src, std::min<size_t>(have, (size_t)bytes), cudaMemcpyDeviceToHost));

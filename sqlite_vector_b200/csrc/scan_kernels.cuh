@@ -676,23 +676,15 @@ struct RangeSortParams {
     uint2 *out;               // nullptr: in place; else query q's ordered pairs go to out + out_off[q] (the batch's compaction)
     const long long *out_off;
 };
-__global__ void __launch_bounds__(kRangeSortThreads, 1) range_sort_kernel(const RangeSortParams sp) {
-    extern __shared__ __align__(16) unsigned long long rkeys[];
-    const unsigned cnt = sp.count[blockIdx.x];
-    if (cnt > (unsigned)kRangeSortCap) return;
-    uint2 *pr = sp.pairs + (size_t)blockIdx.x * (size_t)sp.stride;
-    uint2 *dst = sp.out ? sp.out + sp.out_off[blockIdx.x] : pr;
-    if (cnt < 2u) {
-        if (cnt == 1u && threadIdx.x == 0 && dst != pr) dst[0] = pr[0];
-        return;
-    }
-    const int n = (int)cnt;
+// The block's bitonic sort of n >= 2 pairs from pr into dst (may be pr) by the 64-bit key to_key(pair); from_key(key) restores the
+// pair.  rkeys: shared memory for the next power of two >= n keys.
+template <class ToKey, class FromKey>
+__device__ __forceinline__ void block_sort_pairs(const uint2 *pr, uint2 *dst, int n, unsigned long long *rkeys, ToKey to_key, FromKey from_key) {
     int n2 = 2;
     while (n2 < n) n2 <<= 1;
     for (int i = threadIdx.x; i < n2; i += blockDim.x) {
         if (i < n) {
-            const uint2 e = pr[i];
-            rkeys[i] = ((unsigned long long)fkey(__uint_as_float(e.y)) << 32) | e.x;
+            rkeys[i] = to_key(pr[i]);
         } else {
             rkeys[i] = ~0ull;
         }
@@ -710,10 +702,53 @@ __global__ void __launch_bounds__(kRangeSortThreads, 1) range_sort_kernel(const 
             __syncthreads();
         }
     }
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const unsigned long long key = rkeys[i];
-        dst[i] = make_uint2((unsigned)key, __float_as_uint(funkey((uint32_t)(key >> 32))));
+    for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = from_key(rkeys[i]);
+}
+
+__global__ void __launch_bounds__(kRangeSortThreads, 1) range_sort_kernel(const RangeSortParams sp) {
+    extern __shared__ __align__(16) unsigned long long rkeys[];
+    const unsigned cnt = sp.count[blockIdx.x];
+    if (cnt > (unsigned)kRangeSortCap) return;
+    uint2 *pr = sp.pairs + (size_t)blockIdx.x * (size_t)sp.stride;
+    uint2 *dst = sp.out ? sp.out + sp.out_off[blockIdx.x] : pr;
+    if (cnt < 2u) {
+        if (cnt == 1u && threadIdx.x == 0 && dst != pr) dst[0] = pr[0];
+        return;
     }
+    block_sort_pairs(pr, dst, (int)cnt, rkeys,
+        [](const uint2 e) { return ((unsigned long long)fkey(__uint_as_float(e.y)) << 32) | e.x; },
+        [](const unsigned long long key) { return make_uint2((unsigned)key, __float_as_uint(funkey((uint32_t)(key >> 32)))); });
+}
+
+// ---- large-k batches (batch_large_k, DESIGN §3.12): each query's bucket holds its kept (distance bits, shard row) pairs of every
+// piece back to back, each piece's entries unordered (the refine appends with atomics).  One block per (query, piece) orders that
+// segment by row and writes it to out + out_off[query] + the segment's start, so that every query's candidates come out in scan
+// order.  A query with out_off < 0 is skipped (it is answered alone); no segment is longer than kRangeSortCap (the host checks).
+struct LkbSortParams {
+    const uint2 *bucket;      // query q: bucket + q * stride
+    long long stride;
+    const unsigned *pcount;   // [pieces][nq] the query's bucket count after each piece
+    int nq;
+    uint2 *out;
+    const long long *out_off; // [nq]
+};
+constexpr int kLkbSortThreads = 512;
+__global__ void __launch_bounds__(kLkbSortThreads) lkb_sort_kernel(const LkbSortParams sp) {
+    extern __shared__ __align__(16) unsigned long long lkeys[];
+    const int q = blockIdx.x, piece = blockIdx.y;
+    const long long off = sp.out_off[q];
+    if (off < 0) return;
+    const unsigned a = piece ? sp.pcount[(size_t)(piece - 1) * sp.nq + q] : 0u, b = sp.pcount[(size_t)piece * sp.nq + q];
+    if (b <= a || b - a > (unsigned)kRangeSortCap) return;
+    const uint2 *pr = sp.bucket + (size_t)q * (size_t)sp.stride + a;
+    uint2 *dst = sp.out + off + a;
+    if (b - a == 1u) {
+        if (threadIdx.x == 0) dst[0] = make_uint2(pr[0].y, pr[0].x);
+        return;
+    }
+    block_sort_pairs(pr, dst, (int)(b - a), lkeys,
+        [](const uint2 e) { return ((unsigned long long)e.x << 32) | e.y; },
+        [](const unsigned long long key) { return make_uint2((unsigned)key, (unsigned)(key >> 32)); });
 }
 
 // ------------------------------------------------------------------ large k (k > 256): prefix bounds and ordered candidates

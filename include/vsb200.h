@@ -123,6 +123,19 @@ VSB_API int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *querie
  * on first use and rebuilt after an append. */
 VSB_API int64_t vsb_index_rowid_bitmap(vsb_index *ix, const int64_t *rowids, int64_t n, uint32_t *out_bits);
 
+/* ---- listed rows: the k nearest among a per-query list of rowids, reading only the listed rows (no counterpart in the
+ * reference; the rerank step of vector_quantize_scan_rerank) -------------------------------------------------------------------
+ * Query q's rowids are rowids[offsets[q], offsets[q + 1]) (offsets: nq + 1 non-decreasing values from 0).  For each query the
+ * result is bit for bit what vsb_scan_topk_filtered returns for that one query with the bitmap of its rowids: the same rowids,
+ * order and distances, for every element type, metric and k (k > 256 included), the same max_index carry (nq == 1 only), exchange
+ * sort and INF trim.  Rowids not in the column are ignored, duplicates are harmless, an empty list gives zero rows and a list
+ * shorter than k fewer than k rows.  A batch of nq queries equals nq single calls bit for bit, floating-point types included, and
+ * each query starts from a fresh cursor.  Only the listed rows are read: one kernel computes the distance of every (query, row)
+ * pair with the single-query scan's arithmetic (DESIGN §3.13); a streamed index reads those rows from its pinned host memory in
+ * place, with no window copy.  Counters: "rows_queries", "rows_pairs", "rows_host_bytes". */
+VSB_API int vsb_scan_topk_rows(vsb_index *ix, int metric, const void *queries, int nq, int k, const int64_t *rowids,
+                               const int64_t *offsets, int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
+
 /* ---- range search: every row closer than a radius (no counterpart in the reference, whose stream modules answer it as
  * SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < r ORDER BY distance) --------------------------------------
  * For query b (nq HOST queries, as for vsb_scan_topk) the result is every row with (double)d < radius[b], d being the distance
@@ -257,6 +270,9 @@ VSB_API int vsb_group_scan_all(vsb_group *g, int metric, const void *query, floa
 VSB_API int vsb_group_scan_topk_filtered(vsb_group *g, int metric, const void *queries, int nq, int k, const uint32_t *allow, int64_t nbits,
                                          int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
 VSB_API int64_t vsb_group_rowid_bitmap(vsb_group *g, const int64_t *rowids, int64_t n, uint32_t *out_bits);
+/* vsb_scan_topk_rows over the group's global scan order: every shard computes the distances of its own listed rows */
+VSB_API int vsb_group_scan_topk_rows(vsb_group *g, int metric, const void *queries, int nq, int k, const int64_t *rowids,
+                                     const int64_t *offsets, int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
 /* vsb_scan_range over the group's global scan order (nbits = vsb_group_rows): every shard scans its rows, the shards' lists are
  * merged by (distance, global scan row) */
 VSB_API int vsb_group_scan_range(vsb_group *g, int metric, const void *queries, int nq, const double *radius, const uint32_t *allow,
@@ -293,7 +309,9 @@ VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row o
  * "large_k_batch_fallbacks" (such calls answered query by query: a candidate log overflowed), "large_k_query_fallbacks" (queries
  * of such a batch answered alone: their bucket or a sort segment overflowed), "large_k_levels_us" (host clock around the batch
  * levels, sort and candidate copy, which end in a stream synchronise), "large_k_replay_us" (host clock around the threaded slot
- * replay of such batches; a group counts it on its first shard), "large_k_replay_threads" (host threads of the last replay)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * replay of such batches; a group counts it on its first shard), "large_k_replay_threads" (host threads of the last replay),
+ * "rows_queries" (queries answered by vsb_scan_topk_rows), "rows_pairs" (their listed (query, row) pairs, each row counted once
+ * per query), "rows_host_bytes" (bytes a streamed index's listed-rows kernel read from pinned host memory: pitch bytes per pair)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
  * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */

@@ -50,6 +50,7 @@ _SIGNATURES = {
     "vsb_scan_topk": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "vsb_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vsb_index_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
+    "vsb_scan_topk_rows": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vsb_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_range_get": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_i64)]),
     "vsb_range_free": (None, [_vp]),
@@ -81,6 +82,7 @@ _SIGNATURES = {
     "vsb_group_scan_all": (_i, [_vp, _i, _vp, _vp, _vp]),
     "vsb_group_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vsb_group_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
+    "vsb_group_scan_topk_rows": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vsb_group_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_group_gpus": (_i, [_vp]),
     "vsb_group_rows": (_i64, [_vp]),
@@ -212,6 +214,21 @@ def _topk(eng: "Engine", call, queries: np.ndarray, k: int, max_index: int | Non
     return (out, mi.value) if max_index is not None else out
 
 
+def _rows_topk(eng: "Engine", fn, h, metric: int, queries: np.ndarray, k: int, rowid_lists, max_index: int | None, as_arrays: bool):
+    """the listed-rows entry points: fn(handle, metric, queries, nq, k, rowids, offsets, ids, dist, counts, max_index) -> rc;
+    rowid_lists holds one sequence of rowids per query"""
+    q = np.ascontiguousarray(queries)
+    nq = 1 if q.ndim == 1 else int(np.prod(q.shape[:-1]))
+    lists = [np.asarray(r, dtype=np.int64).reshape(-1) for r in rowid_lists]
+    if len(lists) != nq:
+        raise ValueError(f"{len(lists)} rowid lists for {nq} queries")
+    offsets = np.zeros(nq + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([len(r) for r in lists])
+    flat = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.int64))
+    return _topk(eng, lambda qp, n, ids, dist, counts, mi: fn(h, metric, qp, n, k, _ptr(flat), _ptr(offsets), ids, dist, counts, mi),
+                 q, k, max_index, as_arrays)
+
+
 def _range(eng: "Engine", fn, h, rows: int, metric: int, queries: np.ndarray, radius, allow):
     """the range entry points: fn(handle, metric, queries, nq, radius, allow, nbits, &result) -> rc; one (rowids, distances) pair
     per query, rows ordered by ascending distance (equal distances in scan order)"""
@@ -319,6 +336,11 @@ class Index:
         return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
                                                                                                ids, dist, counts, mi),
                      queries, k, max_index, as_arrays)
+
+    def scan_topk_rows(self, metric: int, queries: np.ndarray, k: int, rowid_lists, max_index: int | None = None, as_arrays: bool = False):
+        """scan_topk among per-query lists of rowids, reading only the listed rows (vsb_scan_topk_rows): rowid_lists holds one
+        sequence of rowids per query; each query's result equals scan_topk_filtered with the bitmap of its rowids"""
+        return _rows_topk(self.eng, self.eng.lib.vsb_scan_topk_rows, self.h, metric, queries, k, rowid_lists, max_index, as_arrays)
 
     def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
         """every row with distance < radius (vsb_scan_range), for one query or a batch; radius: one value or one per query, allow:
@@ -593,6 +615,10 @@ class Group:
         return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_group_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
                                                                                                      ids, dist, counts, mi),
                      queries, k, max_index, False)
+
+    def scan_topk_rows(self, metric: int, queries: np.ndarray, k: int, rowid_lists, max_index: int | None = None, as_arrays: bool = False):
+        """Index.scan_topk_rows over the group's global scan order (vsb_group_scan_topk_rows)"""
+        return _rows_topk(self.eng, self.eng.lib.vsb_group_scan_topk_rows, self.h, metric, queries, k, rowid_lists, max_index, as_arrays)
 
     def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
         """Index.scan_range over the group's global scan order (vsb_group_scan_range)"""

@@ -676,14 +676,29 @@ __device__ __noinline__ float plan_special_row_distance(const uint8_t *row, cons
     return special_row_distance_body<VT, MC>(row, query, nelem, root);
 }
 
+// the out-of-line special-value distance of rows_distance_kernel: a copy of its own, since a noinline function is
+// register-allocated for all of its callers and sharing plan_special_row_distance would change plan_refine_kernel's code
 template <int VT, int MC>
-__global__ void __launch_bounds__(256) plan_refine_kernel(const PlanRefineParams pp) {
+__device__ __noinline__ float rows_special_row_distance(const uint8_t *row, const uint8_t *query, int nelem, int root) {
+    return special_row_distance_body<VT, MC>(row, query, nelem, root);
+}
+
+// The body of plan_refine_kernel (ROWS false) and rows_distance_kernel (ROWS true): the distance of every (row, query) pair in
+// pp.r.cand[0, min(*pp.r.cand_count, pp.r.cand_cap)), computed with the single-query plan's arithmetic.  ROWS false keeps the
+// pairs below their query's bound in its bucket; ROWS true writes every pair's distance bits to out[pair] and rotates the chunks by
+// the row's place in its window of win_rows rows (0: a resident column, rows counted from pp.lrow0 = 0).  Rows or queries with
+// NaN / Inf take the reference's own element loop, in each kernel's own out-of-line copy (a noinline function is register-
+// allocated for all of its callers).
+template <int VT, int MC, bool ROWS>
+__device__ __forceinline__ void plan_distance_body(const PlanRefineParams pp, unsigned *out, long long win_rows) {
     const RefineParams &rp = pp.r;
     const unsigned ncand_raw = *rp.cand_count;
     const unsigned ncand = min(ncand_raw, rp.cand_cap);
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        atomicAdd(&rp.stats[0], ncand);
-        if (ncand_raw > rp.cand_cap) atomicOr(&rp.stats[2], 1u);
+    if constexpr (!ROWS) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            atomicAdd(&rp.stats[0], ncand);
+            if (ncand_raw > rp.cand_cap) atomicOr(&rp.stats[2], 1u);
+        }
     }
     const int log2P = pp.log2P, P = 1 << log2P, rpw = 32 >> log2P;
     const int lane = threadIdx.x & 31, grp = lane >> log2P, p = lane & (P - 1);
@@ -699,7 +714,7 @@ __global__ void __launch_bounds__(256) plan_refine_kernel(const PlanRefineParams
         const uint8_t *rowp = rp.vec + (size_t)cq.x * rp.pitch, *qp = rp.queries + (size_t)cq.y * rp.pitch;
         Accum A = {0.f, 0.f, 0.f, 0, 0};
         if (live) {
-            const int i0 = cnt ? (int)((pp.lrow0 + cq.x) % rpw) % cnt : 0;
+            const int i0 = cnt ? (int)((ROWS && win_rows > 0 ? (long long)cq.x % win_rows : pp.lrow0 + cq.x) % rpw) % cnt : 0;
             for (int i = 0; i < cnt; ++i) {
                 int ii = i0 + i;
                 if (ii >= cnt) ii -= cnt;
@@ -715,13 +730,43 @@ __global__ void __launch_bounds__(256) plan_refine_kernel(const PlanRefineParams
         }
         float d = finalize<VT, MC>(A, qn, rp.root);
         if constexpr (has_special_policy<VT, MC>()) {
-            if (live && p == 0 && row_needs_exact<VT, MC>(A, qn)) d = plan_special_row_distance<VT, MC>(rowp, qp, rp.pitch / 2, rp.root);
+            if (live && p == 0 && row_needs_exact<VT, MC>(A, qn)) {
+                if constexpr (ROWS) d = rows_special_row_distance<VT, MC>(rowp, qp, rp.pitch / 2, rp.root);
+                else d = plan_special_row_distance<VT, MC>(rowp, qp, rp.pitch / 2, rp.root);
+            }
         }
-        if (live && p == 0 && d < rp.U[cq.y]) {
-            const unsigned w = atomicAdd(&rp.bcount[cq.y], 1u);
-            if (w < rp.bucket_cap) rp.bucket[(size_t)cq.y * rp.bucket_cap + w] = make_uint2(cq.x + rp.row_base, __float_as_uint(d));
+        if constexpr (ROWS) {
+            if (live && p == 0) out[c] = __float_as_uint(d);
+        } else {
+            if (live && p == 0 && d < rp.U[cq.y]) {
+                const unsigned w = atomicAdd(&rp.bcount[cq.y], 1u);
+                if (w < rp.bucket_cap) rp.bucket[(size_t)cq.y * rp.bucket_cap + w] = make_uint2(cq.x + rp.row_base, __float_as_uint(d));
+            }
         }
     }
+}
+
+template <int VT, int MC>
+__global__ void __launch_bounds__(256) plan_refine_kernel(const PlanRefineParams pp) {
+    plan_distance_body<VT, MC, false>(pp, nullptr, 0);
+}
+
+// ------------------------------------------------------------------ listed rows (vsb_scan_topk_rows, DESIGN §3.13)
+// The distance of every (row, query) pair of a list, with the arithmetic of the single-query scan's plan (plan_distance_body):
+// no bound, no bucket, one distance per pair.  rows_distance_kernel reads only the listed rows, from the device column or, for a
+// streamed index, straight from its pinned host arena (zero-copy under unified addressing).
+struct RowsParams {
+    PlanRefineParams pp;     // pp.r.vec: the shard's rows (d_vec, or a streamed index's pinned arena by its device address);
+                             // pp.r.queries: [nq][pitch] zero padded; pp.r.cand: the (shard row, query) pairs, *pp.r.cand_count of
+                             // them (pp.r.cand_cap the same); pp.r.pitch, pp.r.root; pp.log2P: lanes per row of the single-query plan;
+                             // pp.qnorm: [nq] the queries' sums of squares as row_norm_kernel computes them; pp.lrow0 = 0
+    unsigned *out;           // [pairs] distance bits
+    long long win_rows;      // streamed: rows per window (the rotation counts rows from the window's start); resident: 0
+};
+
+template <int VT, int MC>
+__global__ void __launch_bounds__(256) rows_distance_kernel(const RowsParams wp) {
+    plan_distance_body<VT, MC, true>(wp.pp, wp.out, wp.win_rows);
 }
 
 // One block per query: U[q] = the k-th smallest distance (fkey order) among the query's first min(bcount[q], cap) bucket entries,

@@ -244,6 +244,14 @@ struct vsb_index {
     long long st_large_k_queries = 0, st_large_k_cands = 0, st_large_k_regrows = 0;
     long long st_large_k_batches = 0, st_large_k_batch_fallbacks = 0, st_large_k_query_fallbacks = 0;   // DESIGN §3.12
     long long st_large_k_levels_us = 0, st_large_k_replay_us = 0, st_large_k_replay_threads = 0;
+    // listed rows (vsb_scan_topk_rows, DESIGN §3.13): one staging area on each side for the queries, their norms, the (row,
+    // query) pairs and the distances, grown never shrunk; a streamed index's kernel reads its rows at arena_dev, h_arena's
+    // device address, checked on first use
+    DeviceBuf<uint8_t> d_rows;
+    HostBuf<uint8_t> h_rows;
+    long long rows_cap = 0, rows_hcap = 0;
+    const uint8_t *arena_dev = nullptr;
+    long long st_rows_queries = 0, st_rows_pairs = 0, st_rows_host_bytes = 0;
 };
 
 // result of a range call (vsb_scan_range): per query, rowids and distances in result order
@@ -1508,6 +1516,9 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "large_k_levels_us")) return ix->st_large_k_levels_us;
     if (!strcmp(name, "large_k_replay_us")) return ix->st_large_k_replay_us;
     if (!strcmp(name, "large_k_replay_threads")) return ix->st_large_k_replay_threads;
+    if (!strcmp(name, "rows_queries")) return ix->st_rows_queries;
+    if (!strcmp(name, "rows_pairs")) return ix->st_rows_pairs;
+    if (!strcmp(name, "rows_host_bytes")) return ix->st_rows_host_bytes;
     return -1;
 }
 void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullptr; }
@@ -1572,6 +1583,25 @@ int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *queries, int n
     const int rc = filter_begin(ix, allow, &scope);
     if (rc) return rc;
     return vsb_scan_topk(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts, max_index);
+}
+
+int vsb_scan_topk_rows(vsb_index *ix, int metric, const void *queries, int nq, int k, const int64_t *rowids, const int64_t *offsets,
+                       int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index) {
+    if (check_index(ix)) return VSB_EINVAL;
+    int rc = rows_check(metric, queries, nq, k, rowids, offsets);
+    if (rc) return rc;
+    if (k == 0) {
+        for (int b = 0; b < nq; ++b) if (out_counts) out_counts[b] = 0;
+        return VSB_OK;
+    }
+    if (!out_rowids || !out_dist) return fail(VSB_EINVAL, "output buffers are null");
+    std::vector<std::vector<uint2>> cands;
+    rc = rows_index(ix, metric, queries, nq, k, rowids, offsets, cands);
+    if (rc) return rc;
+    rows_replay(nq, k, out_rowids, out_dist, out_counts, max_index, [&](int q, SlotState &s) {
+        slots_offer_cands(s, cands[(size_t)q].data(), cands[(size_t)q].size(), [&](uint32_t row) { return rowid_of(ix, row); });
+    });
+    return VSB_OK;
 }
 
 int vsb_scan_range(vsb_index *ix, int metric, const void *queries, int nq, const double *radius, const uint32_t *allow, int64_t nbits,

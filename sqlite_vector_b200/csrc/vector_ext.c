@@ -8,7 +8,9 @@
  *                 vector_full_scan_stream, vector_quantize_scan_stream (tbl, col, vector)
  * additions: vector_*_scan_batch (tbl, col, vectors, k); vector_*_scan_filtered (tbl, col, vector, k, rowids),
  *            vector_*_scan_batch_filtered (tbl, col, vectors, k, rowids) and the aggregate vector_rowid_set(x) that builds rowids;
- *            vector_*_scan_range (tbl, col, vector, radius), vector_*_scan_range_filtered (tbl, col, vector, radius, rowids)
+ *            vector_*_scan_range (tbl, col, vector, radius), vector_*_scan_range_filtered (tbl, col, vector, radius, rowids);
+ *            vector_quantize_scan_rerank (tbl, col, vector, k, candidates), vector_quantize_scan_rerank_batch (tbl, col, vectors, k,
+ *            candidates)
  * Column state, option parsing, JSON vectors, quantization build and the shadow-table chunk format are host
  * C and behave like the reference (citations at each function).  What differs is where a scan runs:
  *   vector_quantize_preload  -> chunks are staged through pinned memory into HBM (vsb_group_append_quant_chunk), row-sharded
@@ -1561,6 +1563,148 @@ SCAN_MODULE(mod_quant_range, vt_connect, vt_best_index, vt_filter_quant_range);
 SCAN_MODULE(mod_full_range_filtered, vt_connect_filtered, vt_best_index, vt_filter_full_range_filtered);
 SCAN_MODULE(mod_quant_range_filtered, vt_connect_filtered, vt_best_index, vt_filter_quant_range_filtered);
 
+/* ------------------------------------------------------------------------------------------------ reranked quantized scans
+ * vector_quantize_scan_rerank(tbl, col, vector, k, candidates) / vector_quantize_scan_rerank_batch(tbl, col, vectors, k, candidates):
+ * the top `candidates` rows of the quantized column, reranked by their raw-column distance.  No counterpart in the reference; the
+ * single function returns row for row what
+ *   SELECT id, distance FROM vector_full_scan_filtered(tbl, col, vector, k,
+ *       (SELECT vector_rowid_set(id) FROM vector_quantize_scan(tbl, col, vector, candidates)))
+ * returns, but the rerank reads only the candidate rows of the raw column (vsb_group_scan_topk_rows) instead of all of it.  The
+ * batch function returns (query, id, distance), each query's rows those of the single function.  Distances are raw-column
+ * distances.  candidates may be smaller than k (fewer rows come back) or 0 (no rows). */
+static int vt_connect_rerank(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
+    (void)argc; (void)argv; (void)err;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, candidates hidden, id, distance);", 1, out);
+}
+static int vt_connect_rerank_batch(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
+    (void)argc; (void)argv; (void)err;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, candidates hidden, query, id, distance);", 1, out);
+}
+
+static int filter_rerank(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int batch) {
+    scan_cursor *c = (scan_cursor *)cur;
+    scan_vtab *vt = (scan_vtab *)cur->pVtab;
+    if (batch) { c->batch = 1; c->bnq = 0; c->bq = 0; c->bj = 0; }
+    else { c->streaming = 0; c->row_index = 0; c->row_count = 0; }
+    if (argc != 5) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, 5, argc);
+    for (int i = 0; i < argc; ++i) {
+        int t = sqlite3_value_type(argv[i]);
+        if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
+        if (i >= 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
+    }
+    const char *tbl = (const char *)sqlite3_value_text(argv[0]);
+    const char *col = (const char *)sqlite3_value_text(argv[1]);
+    vcolumn *v = ctx_find(vt->ctx, tbl, col);
+    if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
+    const int need = v->dim * elem_size(v->vtype);
+    void *owned = 0;
+    const uint8_t *queries = 0;
+    int bytes = 0;
+    if (sqlite3_value_type(argv[2]) == SQLITE_TEXT) {
+        owned = json_to_blob(0, &vt->base, v->vtype, (const char *)sqlite3_value_text(argv[2]), &bytes, batch ? 0 : v->dim);
+        if (!owned) return SQLITE_ERROR;
+        queries = (const uint8_t *)owned;
+    } else {
+        queries = (const uint8_t *)sqlite3_value_blob(argv[2]);
+        bytes = sqlite3_value_bytes(argv[2]);
+        if (!queries) return vtab_error(&vt->base, "%s: input vector%s cannot be NULL.", fname, batch ? "s" : "");
+        if (!batch && bytes < need) return vtab_error(&vt->base, "%s: input vector has %d bytes, expected %d.", fname, bytes, need);
+    }
+    int rc = SQLITE_OK, nq = 1;
+    uint8_t *qq = 0;
+    int64_t *qids = 0, *offsets = 0;
+    double *qdist = 0;
+    int *qcounts = 0;
+    vsb_group *qix = 0, *fix = 0;
+    if (batch) {
+        if (bytes <= 0 || bytes % need != 0) {
+            rc = vtab_error(&vt->base, "%s: input has %d bytes, expected a positive multiple of %d (dimension %d).", fname, bytes, need, v->dim);
+            goto out;
+        }
+        nq = bytes / need;
+    }
+    rc = resident_index(vt, v, tbl, col, fname, 1, &qix);
+    if (rc != SQLITE_OK) goto out;
+    qq = (uint8_t *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)v->dim);   /* quantize every query (:2162-2177) */
+    if (!qq) { rc = SQLITE_NOMEM; goto out; }
+    for (int b = 0; b < nq; ++b) quantize_vec(v->vtype, queries + (size_t)b * need, qq + (size_t)b * v->dim, v->offset, v->scale, v->dim, v->qtype);
+    {
+        const int k = sqlite3_value_int(argv[3]);
+        const sqlite3_int64 cand64 = sqlite3_value_int64(argv[4]);
+        if (k == 0) { rc = batch ? SQLITE_OK : SQLITE_DONE; goto out; }   /* as the single- and multi-query scans (:1795-1796) */
+        if (k < 0) { rc = vtab_error(&vt->base, "%s: k must not be negative.", fname); goto out; }
+        if (cand64 < 0 || cand64 > INT32_MAX) { rc = vtab_error(&vt->base, "%s: candidates must be between 0 and %d.", fname, INT32_MAX); goto out; }
+        const int cand = (int)cand64;
+        /* 1: the top `candidates` of the quantized column, every query from a fresh cursor, as the subquery of the composed statement */
+        qcounts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
+        offsets = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(nq + 1) * sizeof(int64_t));
+        qids = (int64_t *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)(cand > 0 ? cand : 1) * sizeof(int64_t));
+        qdist = (double *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)(cand > 0 ? cand : 1) * sizeof(double));
+        if (!qcounts || !offsets || !qids || !qdist) { rc = SQLITE_NOMEM; goto out; }
+        memset(qcounts, 0, (size_t)nq * sizeof(int));
+        if (cand > 0) {
+            int mi = 0;
+            if (vsb_group_scan_topk(qix, v->metric, qq, nq, cand, qids, qdist, qcounts, &mi) != VSB_OK) {
+                rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
+                goto out;
+            }
+        }
+        /* each query's candidate rowids, back to back */
+        offsets[0] = 0;
+        for (int b = 0; b < nq; ++b) {
+            memmove(qids + offsets[b], qids + (size_t)b * (size_t)cand, (size_t)qcounts[b] * sizeof(int64_t));
+            offsets[b + 1] = offsets[b] + qcounts[b];
+        }
+        /* 2: the rerank on the raw column, reading only the candidate rows */
+        rc = resident_index(vt, v, tbl, col, fname, 0, &fix);
+        if (rc != SQLITE_OK) goto out;
+        int src;
+        if (batch) {
+            sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->bcounts);
+            c->k_alloc = 0;
+            c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)k * sizeof(sqlite3_int64));
+            c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)k * sizeof(double));
+            c->bcounts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
+            if (!c->ids || !c->dist || !c->bcounts) { rc = SQLITE_NOMEM; goto out; }
+            src = vsb_group_scan_topk_rows(fix, v->metric, queries, nq, k, qids, offsets, (int64_t *)c->ids, c->dist, c->bcounts, 0);
+        } else {
+            if (c->k_alloc != k) {                                          /* :1798-1806 */
+                sqlite3_free(c->ids); sqlite3_free(c->dist);
+                c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)k * sizeof(sqlite3_int64));
+                c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)k * sizeof(double));
+                if (!c->ids || !c->dist) { c->k_alloc = 0; rc = SQLITE_NOMEM; goto out; }
+                c->k_alloc = k;
+            }
+            int count = 0;
+            src = vsb_group_scan_topk_rows(fix, v->metric, queries, 1, k, qids, offsets, (int64_t *)c->ids, c->dist, &count, &c->max_index);
+            if (src == VSB_OK) c->row_count = count;
+        }
+        if (src != VSB_OK) {
+            rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
+            goto out;
+        }
+        if (batch) {
+            c->bnq = nq;
+            c->bk = k;
+            batch_skip_empty(c);
+        }
+    }
+out:
+    sqlite3_free(owned);
+    sqlite3_free(qq);
+    sqlite3_free(qids);
+    sqlite3_free(qdist);
+    sqlite3_free(qcounts);
+    sqlite3_free(offsets);
+    return rc;
+}
+static int vt_filter_rerank(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_rerank(c, argc, argv, "vector_quantize_scan_rerank", 0); }
+static int vt_filter_rerank_batch(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_rerank(c, argc, argv, "vector_quantize_scan_rerank_batch", 1); }
+SCAN_MODULE(mod_quant_rerank, vt_connect_rerank, vt_best_index, vt_filter_rerank);
+static sqlite3_module mod_quant_rerank_batch = {0, 0, vt_connect_rerank_batch, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_rerank_batch,
+                                                vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+
 /* vector_rowid_set(x): aggregate of the non-NULL x as the rowids BLOB of the *_filtered modules (int64, host byte order =
  * little-endian), e.g. (SELECT vector_rowid_set(rowid) FROM docs WHERE lang = 'en'); no rows give an empty BLOB */
 typedef struct {
@@ -1639,5 +1783,7 @@ __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range", &mod_quant_range, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_full_scan_range_filtered", &mod_full_range_filtered, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range_filtered", &mod_quant_range_filtered, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_rerank", &mod_quant_rerank, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_rerank_batch", &mod_quant_rerank_batch, ctx)) != SQLITE_OK) return rc;
     return SQLITE_OK;
 }

@@ -123,6 +123,24 @@ VSB_API int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *querie
  * on first use and rebuilt after an append. */
 VSB_API int64_t vsb_index_rowid_bitmap(vsb_index *ix, const int64_t *rowids, int64_t n, uint32_t *out_bits);
 
+/* ---- per-query eligible sets: each query's k nearest among its own set of rows, in one pass of the column (no counterpart in
+ * the reference) -------------------------------------------------------------------------------------------------------------------
+ * sets: nsets HOST bitmaps over the scan-order rows, each (nbits + 31) / 32 words, back to back, in the layout of
+ * vsb_scan_topk_filtered; nbits == vsb_index_rows.  set_of_query[b] in [0, nsets) names query b's set (NULL: query b uses set b,
+ * nsets == nq).  Query b's result is exactly what vsb_scan_topk_filtered returns for b under bitmap sets[set_of_query[b]]: the
+ * same rowids, order and distances, exchange sort and INF trim (an empty set gives zero rows, a set of fewer than k rows fewer
+ * than k rows), bit for bit for every element type.  max_index is carried for nq == 1 only; every query of a larger batch starts
+ * from a fresh cursor.  A batch that vsb_scan_topk's batch path admits (nq >= 16, k <= 256) runs as ONE batch: the union of the
+ * sets is the row filter, each scored pair is also tested against its query's set, and the levels are planned so that every set
+ * keeps the bucket bound of the batch path (DESIGN §3.14).  A capacity overflow, a plan of more than 256 levels in a view, set
+ * bitmaps and plan larger than 1/8 of free device memory (option "sets_mem_mb": that many MB), and every call outside those conditions answer set by set: one
+ * vsb_scan_topk_filtered per distinct set over its queries in call order.  The bitmaps live on the device for the call only.
+ * Counters: "sets_batches" (one-pass calls), "sets_fallbacks" (admitted calls answered set by set), "sets_levels" (levels of
+ * the most recent one-pass call), "sets_plan_us" (time of its level plans).  SQL: vector_*_scan_batch_sets, vector_rowid_sets. */
+VSB_API int vsb_scan_topk_sets(vsb_index *ix, int metric, const void *queries, int nq, int k, const uint32_t *sets, int nsets,
+                               int64_t nbits, const int32_t *set_of_query, int64_t *out_rowids, double *out_dist, int *out_counts,
+                               int *max_index);
+
 /* ---- listed rows: the k nearest among a per-query list of rowids, reading only the listed rows (no counterpart in the
  * reference; the rerank step of vector_quantize_scan_rerank) -------------------------------------------------------------------
  * Query q's rowids are rowids[offsets[q], offsets[q + 1]) (offsets: nq + 1 non-decreasing values from 0).  For each query the
@@ -270,6 +288,11 @@ VSB_API int vsb_group_scan_all(vsb_group *g, int metric, const void *query, floa
 VSB_API int vsb_group_scan_topk_filtered(vsb_group *g, int metric, const void *queries, int nq, int k, const uint32_t *allow, int64_t nbits,
                                          int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
 VSB_API int64_t vsb_group_rowid_bitmap(vsb_group *g, const int64_t *rowids, int64_t n, uint32_t *out_bits);
+/* vsb_scan_topk_sets over the group's global scan order: every set is cut per shard, each shard runs the one-pass batch and the
+ * shards' entry logs merge as in vsb_group_scan_topk (counters on shard 0) */
+VSB_API int vsb_group_scan_topk_sets(vsb_group *g, int metric, const void *queries, int nq, int k, const uint32_t *sets, int nsets,
+                                     int64_t nbits, const int32_t *set_of_query, int64_t *out_rowids, double *out_dist,
+                                     int *out_counts, int *max_index);
 /* vsb_scan_topk_rows over the group's global scan order: every shard computes the distances of its own listed rows */
 VSB_API int vsb_group_scan_topk_rows(vsb_group *g, int metric, const void *queries, int nq, int k, const int64_t *rowids,
                                      const int64_t *offsets, int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
@@ -311,7 +334,8 @@ VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row o
  * levels, sort and candidate copy, which end in a stream synchronise), "large_k_replay_us" (host clock around the threaded slot
  * replay of such batches; a group counts it on its first shard), "large_k_replay_threads" (host threads of the last replay),
  * "rows_queries" (queries answered by vsb_scan_topk_rows), "rows_pairs" (their listed (query, row) pairs, each row counted once
- * per query), "rows_host_bytes" (bytes a streamed index's listed-rows kernel read from pinned host memory: pitch bytes per pair)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * per query), "rows_host_bytes" (bytes a streamed index's listed-rows kernel read from pinned host memory: pitch bytes per pair),
+ * "sets_batches", "sets_fallbacks", "sets_levels", "sets_plan_us" (see vsb_scan_topk_sets)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
  * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */
@@ -366,7 +390,7 @@ VSB_API int vsb_debug_refine(vsb_index *ix, int metric, const void *queries, int
 VSB_API int vsb_debug_replay(vsb_index *ix, int metric, const void *queries, int nq, int k, int level0, const uint32_t *bucket,
                              const uint32_t *bcount, float *slot_d, uint32_t *slot_row, int *slot_mi, int acc_cap, uint32_t *acc_log,
                              int *acc_count, int final_sort, float *out_U, uint32_t *out_qc, uint32_t *out_bcount, uint32_t *out_stats);
-/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","scan_streams","xwait_ms","epi_chunk","f32_batch"};
+/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","scan_streams","xwait_ms","epi_chunk","f32_batch","sets_mem_mb"};
  * "f32_batch" = 1: f32 columns batch L2 / cosine / dot queries on the tensor cores in TF32 (default 0, or VSB_F32_BATCH=1 in the
  * environment when the library loads; per process).  Values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);

@@ -51,6 +51,7 @@ _SIGNATURES = {
     "vsb_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vsb_index_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
     "vsb_scan_topk_rows": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vsb_scan_topk_sets": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
     "vsb_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_range_get": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_i64)]),
     "vsb_range_free": (None, [_vp]),
@@ -83,6 +84,7 @@ _SIGNATURES = {
     "vsb_group_scan_topk_filtered": (_i, [_vp, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp]),
     "vsb_group_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
     "vsb_group_scan_topk_rows": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vsb_group_scan_topk_sets": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
     "vsb_group_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_group_gpus": (_i, [_vp]),
     "vsb_group_rows": (_i64, [_vp]),
@@ -229,6 +231,23 @@ def _rows_topk(eng: "Engine", fn, h, metric: int, queries: np.ndarray, k: int, r
                  q, k, max_index, as_arrays)
 
 
+def _sets_topk(eng: "Engine", fn, h, rows: int, metric: int, queries: np.ndarray, k: int, sets, set_of_query, as_arrays: bool):
+    """the per-query sets entry points: fn(handle, metric, queries, nq, k, sets, nsets, nbits, set_of_query, ids, dist, counts,
+    max_index) -> rc; sets holds boolean masks or row bitmaps (or is one uint32 array [nsets, words]), set_of_query one set index per query (None: query b uses set b)"""
+    words = (rows + 31) // 32
+    if isinstance(sets, np.ndarray) and sets.dtype == np.uint32 and sets.ndim == 2 and sets.shape[1] == words and words > 0:
+        flat = np.ascontiguousarray(sets)                      # already nsets bitmaps back to back
+    else:
+        bits = np.zeros((len(sets), max(words, 1)), dtype=np.uint32)
+        for i, a in enumerate(sets):
+            bits[i, :words] = _allow_words(a, rows)[:words]
+        flat = np.ascontiguousarray(bits[:, :words]) if words > 0 else np.zeros(1, np.uint32)
+    soq = None if set_of_query is None else np.ascontiguousarray(set_of_query, dtype=np.int32).reshape(-1)
+    return _topk(eng, lambda qp, n, ids, dist, counts, mi: fn(h, metric, qp, n, k, _ptr(flat), len(sets), rows, _ptr(soq), ids, dist,
+                                                            counts, mi),
+                 queries, k, None, as_arrays)
+
+
 def _range(eng: "Engine", fn, h, rows: int, metric: int, queries: np.ndarray, radius, allow):
     """the range entry points: fn(handle, metric, queries, nq, radius, allow, nbits, &result) -> rc; one (rowids, distances) pair
     per query, rows ordered by ascending distance (equal distances in scan order)"""
@@ -341,6 +360,12 @@ class Index:
         """scan_topk among per-query lists of rowids, reading only the listed rows (vsb_scan_topk_rows): rowid_lists holds one
         sequence of rowids per query; each query's result equals scan_topk_filtered with the bitmap of its rowids"""
         return _rows_topk(self.eng, self.eng.lib.vsb_scan_topk_rows, self.h, metric, queries, k, rowid_lists, max_index, as_arrays)
+
+    def scan_topk_sets(self, metric: int, queries: np.ndarray, k: int, sets, set_of_query=None, as_arrays: bool = False):
+        """scan_topk of each query among its own set of rows (vsb_scan_topk_sets), one pass of the column for the whole batch:
+        `sets` is a list of boolean masks over the scan-order rows or of uint32 row bitmaps, set_of_query[b] the index of query
+        b's set (None: query b uses set b); each query's result equals scan_topk_filtered with its set"""
+        return _sets_topk(self.eng, self.eng.lib.vsb_scan_topk_sets, self.h, self.rows, metric, queries, k, sets, set_of_query, as_arrays)
 
     def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
         """every row with distance < radius (vsb_scan_range), for one query or a batch; radius: one value or one per query, allow:
@@ -619,6 +644,10 @@ class Group:
     def scan_topk_rows(self, metric: int, queries: np.ndarray, k: int, rowid_lists, max_index: int | None = None, as_arrays: bool = False):
         """Index.scan_topk_rows over the group's global scan order (vsb_group_scan_topk_rows)"""
         return _rows_topk(self.eng, self.eng.lib.vsb_group_scan_topk_rows, self.h, metric, queries, k, rowid_lists, max_index, as_arrays)
+
+    def scan_topk_sets(self, metric: int, queries: np.ndarray, k: int, sets, set_of_query=None, as_arrays: bool = False):
+        """Index.scan_topk_sets over the group's global scan order (vsb_group_scan_topk_sets)"""
+        return _sets_topk(self.eng, self.eng.lib.vsb_group_scan_topk_sets, self.h, self.rows, metric, queries, k, sets, set_of_query, as_arrays)
 
     def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
         """Index.scan_range over the group's global scan order (vsb_group_scan_range)"""

@@ -50,7 +50,18 @@ struct TcParams {
     // row filter: a row whose bit allow_base + row is clear is never a hit (ScanParams::allow); nullptr: every row is eligible
     const uint32_t *allow;
     long long allow_base;
+    // per-query eligible sets (vsb_scan_topk_sets): query q may only see the rows whose bit allow_base + row is set in bitmap
+    // set_of_query[q] of `sets` (set_words words each); nullptr: every query sees every eligible row.  Tested per pair, only
+    // in the rare path behind the warp's ballot
+    const uint32_t *sets;
+    long long set_words;
+    const int *set_of_query;
 };
+
+// bit allow_base + row of query q's set (TcParams::sets); true without sets
+__device__ __forceinline__ bool pair_in_set(const TcParams &prm, long long row, int q) {
+    return prm.sets == nullptr || row_allowed(prm.sets + (size_t)__ldg(prm.set_of_query + q) * prm.set_words, prm.allow_base + row);
+}
 
 // ------------------------------------------------------------------ PTX wrappers (TMA / wgmma)
 __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
@@ -348,17 +359,44 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_scan_kernel(const __grid_con
         if (__ballot_sync(0xFFFFFFFFu, any)) {                                 // rare: append (row, query) hits
             const int ncol = prm.nq - ng * N;                                  // padded query columns are never reported
             int mine = 0;
-            if (any) {
+            if (prm.sets == nullptr) {
+                if (any) {
 #pragma unroll
-                for (int i = 0; i < N / 2; ++i) mine += (hit(i) && 8 * (i >> 2) + cq + (i & 1) < ncol) ? 1 : 0;
-            }
-            append_hits(prm, lane, mine, [&](auto emit) {
-#pragma unroll
-                for (int i = 0; i < N / 2; ++i) {
-                    const int col = 8 * (i >> 2) + cq + (i & 1);
-                    if (hit(i) && col < ncol) emit(row[(i >> 1) & 1], ng * N + col);
+                    for (int i = 0; i < N / 2; ++i) mine += (hit(i) && 8 * (i >> 2) + cq + (i & 1) < ncol) ? 1 : 0;
                 }
-            });
+                append_hits(prm, lane, mine, [&](auto emit) {
+#pragma unroll
+                    for (int i = 0; i < N / 2; ++i) {
+                        const int col = 8 * (i >> 2) + cq + (i & 1);
+                        if (hit(i) && col < ncol) emit(row[(i >> 1) & 1], ng * N + col);
+                    }
+                });
+            } else {
+                // per-query sets: bit c = 2 (i >> 2) + (i & 1) of adm[h] says whether row h's pair with the thread's column c
+                // is in that query's set, looked up once per column and row.  (Looking up only the hit columns needs a first
+                // pass that packs the hits of all N / 2 accumulators into masks; with N = 256 that makes ptxas spill.)
+                uint64_t adm[2] = {0ull, 0ull};
+                if (any) {
+#pragma unroll 1
+                    for (int c = 0; c < N / 4; ++c) {
+                        const int col = 8 * (c >> 1) + cq + (c & 1);
+                        if (col >= ncol) break;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            if (rowvalid[h] && pair_in_set(prm, row[h], ng * N + col)) adm[h] |= 1ull << c;
+                    }
+                }
+                auto take = [&](int i) -> bool { return hit(i) && ((adm[(i >> 1) & 1] >> (2 * (i >> 2) + (i & 1))) & 1ull); };
+                if (any) {
+#pragma unroll
+                    for (int i = 0; i < N / 2; ++i) mine += take(i) ? 1 : 0;
+                }
+                append_hits(prm, lane, mine, [&](auto emit) {
+#pragma unroll
+                    for (int i = 0; i < N / 2; ++i)
+                        if (take(i)) emit(row[(i >> 1) & 1], ng * N + 8 * (i >> 2) + cq + (i & 1));
+                });
+            }
         }
     }
 }
@@ -500,13 +538,29 @@ __global__ void __launch_bounds__(kL1Threads, 1) l1_batch_kernel(const __grid_co
 #pragma unroll
             for (int j = 0; j < C; ++j) mine += hit(i, j) ? 1 : 0;
         if (__ballot_sync(0xFFFFFFFFu, mine != 0)) {                           // rare: append (row, query) hits
-            append_hits(prm, lane, mine, [&](auto emit) {
+            if (prm.sets == nullptr) {
+                append_hits(prm, lane, mine, [&](auto emit) {
+#pragma unroll
+                    for (int i = 0; i < R; ++i)
+#pragma unroll
+                        for (int j = 0; j < C; ++j)
+                            if (hit(i, j)) emit(row[i], qbase + j);
+                });
+            } else {                                                           // per-query sets: only the pairs they admit
+                auto take = [&](int i, int j) -> bool { return hit(i, j) && pair_in_set(prm, row[i], qbase + j); };
+                mine = 0;
 #pragma unroll
                 for (int i = 0; i < R; ++i)
 #pragma unroll
-                    for (int j = 0; j < C; ++j)
-                        if (hit(i, j)) emit(row[i], qbase + j);
-            });
+                    for (int j = 0; j < C; ++j) mine += take(i, j) ? 1 : 0;
+                append_hits(prm, lane, mine, [&](auto emit) {
+#pragma unroll
+                    for (int i = 0; i < R; ++i)
+#pragma unroll
+                        for (int j = 0; j < C; ++j)
+                            if (take(i, j)) emit(row[i], qbase + j);
+                });
+            }
         }
     }
 }
@@ -567,6 +621,142 @@ __global__ void all_pairs_kernel(uint2 *cand, unsigned *count, long long m0, int
         base = __shfl_sync(0xFFFFFFFFu, base, 0);
         for (int q = lane; q < nq; q += 32) cand[base + q] = make_uint2((uint32_t)row, (uint32_t)q);
     }
+}
+
+// ------------------------------------------------------------------ per-query sets (vsb_scan_topk_sets, DESIGN.md §3.14)
+// Bitmaps of nsets sets, `words` words each, back to back; query q's set is set_of_query[q].
+
+// level 0 of a sets call: the pairs (row, q) of rows [0, m0) with row in q's set, one warp per row of the union `allow`
+// (the caller has checked their number against the log; *count starts at 0)
+__global__ void sets_pairs_kernel(uint2 *cand, unsigned *count, long long m0, int nq, const uint32_t *allow, long long allow_base,
+                                  const uint32_t *sets, long long words, const int *set_of_query) {
+    const int lane = threadIdx.x & 31;
+    const long long nwarps = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < m0; row += nwarps) {
+        if (!row_allowed(allow, allow_base + row)) continue;                  // warp-uniform
+        for (int q0 = 0; q0 < nq; q0 += 32) {
+            const int q = q0 + lane;
+            const bool in = q < nq && row_allowed(sets + (size_t)set_of_query[q] * words, allow_base + row);
+            const unsigned m = __ballot_sync(0xFFFFFFFFu, in);
+            if (m == 0u) continue;
+            unsigned base = 0;
+            if (lane == 0) base = atomicAdd(count, (unsigned)__popc(m));
+            base = __shfl_sync(0xFFFFFFFFu, base, 0);
+            if (in) cand[base + __popc(m & ((1u << lane) - 1u))] = make_uint2((uint32_t)row, (uint32_t)q);
+        }
+    }
+}
+
+// the union of the sets, word by word (out: words entries)
+__global__ void sets_union_kernel(const uint32_t *sets, int nsets, long long words, uint32_t *out) {
+    for (long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x; w < words; w += (long long)gridDim.x * blockDim.x) {
+        uint32_t v = 0u;
+        for (int s = 0; s < nsets; ++s) v |= __ldg(sets + (size_t)s * words + w);
+        out[w] = v;
+    }
+}
+
+// set bits of rows [a, b) of a bitmap
+__device__ __forceinline__ unsigned bitmap_count(const uint32_t *bits, long long a, long long b) {
+    unsigned c = 0;
+    for (long long r = a; r < b;) {
+        const long long w = r >> 5;
+        const int lo = (int)(r & 31), hi = (int)min(32ll, b - (w << 5));
+        uint32_t v = __ldg(bits + w) >> lo;
+        if (hi - lo < 32) v &= (1u << (hi - lo)) - 1u;
+        c += (unsigned)__popc(v);
+        r = (w + 1) << 5;
+    }
+    return c;
+}
+
+constexpr int kSetsThreads = 1024;
+
+// prefix[s][j] = rows of set s in tile rows [tb[0], tb[j]), j = 0 .. T; one block per set, the tiles in chunks of one per thread
+__global__ void __launch_bounds__(kSetsThreads) sets_prefix_kernel(const uint32_t *sets, long long words, const long long *tb, int T,
+                                                                   unsigned *prefix) {
+    __shared__ unsigned wsum[kSetsThreads / 32], total;
+    const int s = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t *bits = sets + (size_t)s * words;
+    unsigned *out = prefix + (size_t)s * (T + 1);
+    if (threadIdx.x == 0) out[0] = 0u;
+    unsigned carry = 0;
+    for (int j0 = 0; j0 < T; j0 += kSetsThreads) {
+        const int j = j0 + threadIdx.x;
+        unsigned incl = j < T ? bitmap_count(bits, tb[j], tb[j + 1]) : 0u;
+        for (int off = 1; off < 32; off <<= 1) {
+            const unsigned o = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+            if (lane >= off) incl += o;
+        }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            const unsigned v = wsum[lane];
+            unsigned x = v;
+            for (int off = 1; off < 32; off <<= 1) {
+                const unsigned o = __shfl_up_sync(0xFFFFFFFFu, x, off);
+                if (lane >= off) x += o;
+            }
+            wsum[lane] = x - v;                                                // the warps before this one
+            if (lane == 31) total = x;
+        }
+        __syncthreads();
+        if (j < T) out[j + 1] = carry + wsum[warp] + incl;
+        carry += total;
+        __syncthreads();                                                       // wsum and total are rewritten by the next chunk
+    }
+}
+
+// The levels of a sets call (DESIGN.md §3.14), one block.  Views v = 0 .. V-1 hold the tiles [vt[v], vt[v+1]) of prefix.  A level
+// starting at tile t ends at the smallest u over the sets of the largest u <= the view's end with prefix[s][u] <=
+// max(m0, growth * prefix[s][t]), and holds at least one tile.  Writes each view's level ends (tile indices, at most `budget`
+// per view) to ends[v * budget ..] and their number to nlev[v], and the pairs of level 0 (the sum over the queries of their
+// set's rows in it) to *pairs0.  *over = 1: a view needs more than `budget` levels (nothing else is then valid).
+__global__ void __launch_bounds__(kSetsThreads) sets_plan_kernel(const unsigned *prefix, int nsets, int T, const int *vt, int V,
+                                                                 long long m0, int growth, int budget, const int *set_of_query, int nq,
+                                                                 int *ends, int *nlev, unsigned long long *pairs0, int *over) {
+    __shared__ int umin;
+    __shared__ unsigned long long psum;
+    if (threadIdx.x == 0) { *over = 0; psum = 0ull; }
+    bool first = true;
+    for (int v = 0; v < V; ++v) {
+        const int te = vt[v + 1];
+        int t = vt[v], nl = 0;
+        while (t < te) {
+            if (nl == budget) {
+                if (threadIdx.x == 0) *over = 1;
+                return;
+            }
+            if (threadIdx.x == 0) umin = te;
+            __syncthreads();
+            for (int s = threadIdx.x; s < nsets; s += blockDim.x) {
+                const unsigned *p = prefix + (size_t)s * (T + 1);
+                const unsigned long long cap = max((unsigned long long)m0, (unsigned long long)growth * p[t]);
+                int lo = t, hi = te;                                           // p[t] <= cap: the answer is in [t, te]
+                while (lo < hi) {
+                    const int mid = (lo + hi + 1) >> 1;
+                    if (p[mid] <= cap) lo = mid;
+                    else hi = mid - 1;
+                }
+                atomicMin(&umin, lo);
+            }
+            __syncthreads();
+            const int u = max(t + 1, umin);
+            if (first) {
+                unsigned long long c = 0;
+                for (int q = threadIdx.x; q < nq; q += blockDim.x) c += prefix[(size_t)set_of_query[q] * (T + 1) + u];
+                atomicAdd(&psum, c);
+                first = false;
+            }
+            if (threadIdx.x == 0) ends[(size_t)v * budget + nl] = u;
+            __syncthreads();
+            t = u;
+            ++nl;
+        }
+        if (threadIdx.x == 0) nlev[v] = nl;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *pairs0 = psum;
 }
 
 struct RefineParams {

@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -55,6 +56,7 @@ int g_opt_f32_batch = [] {
     const char *e = getenv("VSB_F32_BATCH");
     return (e && atoi(e) > 0) ? 1 : 0;
 }();
+int g_opt_sets_mem_mb = 0;     // vsb_scan_topk_sets: device memory its one-pass buffers may take, in MB (0: 1/8 of the free memory)
 int g_opt_xwait_ms = 10000;    // exchange: how long the receiving side waits for a peer's head before it reports an error (a dead
                                // peer, not a slow one: ranks sharing one GPU or a busy host can start a batch seconds apart)
 
@@ -166,6 +168,7 @@ struct PairList {
 };
 
 struct BatchWs;   // batch_host.inc
+struct SetsState;   // batch_host.inc
 
 }  // namespace
 
@@ -252,6 +255,10 @@ struct vsb_index {
     long long rows_cap = 0, rows_hcap = 0;
     const uint8_t *arena_dev = nullptr;
     long long st_rows_queries = 0, st_rows_pairs = 0, st_rows_host_bytes = 0;
+    // per-query sets of the sets call in progress (vsb_scan_topk_sets, SetsScope): their device bitmaps, whose union is flt_d;
+    // null outside such a call
+    const SetsState *sets = nullptr;
+    long long st_sets_batches = 0, st_sets_fallbacks = 0, st_sets_levels = 0, st_sets_plan_us = 0;
 };
 
 // result of a range call (vsb_scan_range): per query, rowids and distances in result order
@@ -1279,6 +1286,7 @@ int vsb_set_option(const char *name, int value) {
     else if (!strcmp(name, "scan_streams")) p = &g_opt_scan_streams;
     else if (!strcmp(name, "xwait_ms")) p = &g_opt_xwait_ms;
     else if (!strcmp(name, "f32_batch")) p = &g_opt_f32_batch;
+    else if (!strcmp(name, "sets_mem_mb")) p = &g_opt_sets_mem_mb;
     if (!p) return fail(VSB_EINVAL, "unknown option %s", name);
     if (value < 0) return fail(VSB_EINVAL, "option %s: values are non-negative", name);   // so that a negative return is always an error
     int old = *p;
@@ -1519,6 +1527,10 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "rows_queries")) return ix->st_rows_queries;
     if (!strcmp(name, "rows_pairs")) return ix->st_rows_pairs;
     if (!strcmp(name, "rows_host_bytes")) return ix->st_rows_host_bytes;
+    if (!strcmp(name, "sets_batches")) return ix->st_sets_batches;
+    if (!strcmp(name, "sets_fallbacks")) return ix->st_sets_fallbacks;
+    if (!strcmp(name, "sets_levels")) return ix->st_sets_levels;
+    if (!strcmp(name, "sets_plan_us")) return ix->st_sets_plan_us;
     return -1;
 }
 void *vsb_index_stream(vsb_index *ix) { return ix ? (void *)ix->fstream : nullptr; }
@@ -1583,6 +1595,39 @@ int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *queries, int n
     const int rc = filter_begin(ix, allow, &scope);
     if (rc) return rc;
     return vsb_scan_topk(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts, max_index);
+}
+
+int vsb_scan_topk_sets(vsb_index *ix, int metric, const void *queries, int nq, int k, const uint32_t *sets, int nsets, int64_t nbits,
+                       const int32_t *set_of_query, int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index) {
+    if (check_index(ix)) return VSB_EINVAL;
+    std::vector<int> soq;
+    int rc = sets_check(queries, nq, k, sets, nsets, nbits, ix->n, set_of_query, soq);
+    if (rc) return rc;
+    if (k == 0 || nq == 0) {
+        for (int b = 0; b < nq; ++b) if (out_counts) out_counts[b] = 0;
+        return VSB_OK;
+    }
+    if (!out_rowids || !out_dist) return fail(VSB_EINVAL, "output buffers are null");
+    const long long words = (ix->n + 31) / 32;
+    if (batch_supported(ix, metric, nq, k)) {   // one pass of the column for every set (DESIGN §3.14)
+        {
+            std::vector<int> dense = soq;
+            const std::vector<int> used = sets_used(dense, nsets);
+            SetsScope scope;
+            rc = sets_begin(ix, used, [&](int i) { return sets + (size_t)used[(size_t)i] * words; }, dense, k, &scope);
+            if (rc == VSB_OK) rc = batch_scan(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts);
+        }
+        if (rc == VSB_OK) {
+            ix->st_sets_batches++;
+            return VSB_OK;
+        }
+        if (rc != VSB_ERANGE) return rc;
+        ix->st_sets_fallbacks++;
+    }
+    return sets_by_set(queries, nq, k, (size_t)ix->dim * ix->esize, soq, out_rowids, out_dist, out_counts, max_index,
+                       [&](const void *q, int m, int s, int64_t *ids, double *dist, int *cnt, int *mi) {
+                           return vsb_scan_topk_filtered(ix, metric, q, m, k, sets + (size_t)s * words, nbits, ids, dist, cnt, mi);
+                       });
 }
 
 int vsb_scan_topk_rows(vsb_index *ix, int metric, const void *queries, int nq, int k, const int64_t *rowids, const int64_t *offsets,

@@ -8,6 +8,7 @@
  *                 vector_full_scan_stream, vector_quantize_scan_stream (tbl, col, vector)
  * additions: vector_*_scan_batch (tbl, col, vectors, k); vector_*_scan_filtered (tbl, col, vector, k, rowids),
  *            vector_*_scan_batch_filtered (tbl, col, vectors, k, rowids) and the aggregate vector_rowid_set(x) that builds rowids;
+ *            vector_*_scan_batch_sets (tbl, col, vectors, k, sets, query_sets) and the aggregate vector_rowid_sets(set, rowid);
  *            vector_*_scan_range (tbl, col, vector, radius), vector_*_scan_range_filtered (tbl, col, vector, radius, rowids);
  *            vector_quantize_scan_rerank (tbl, col, vector, k, candidates), vector_quantize_scan_rerank_batch (tbl, col, vectors, k,
  *            candidates)
@@ -70,7 +71,7 @@ typedef struct {
     sqlite3_vtab base;
     sqlite3 *db;
     vcontext *ctx;
-    int filtered;                  /* the *_filtered modules: one more hidden column (rowids) before the visible ones */
+    int filtered;                  /* hidden columns before the visible ones beyond memidx: 1 for *_filtered (rowids), 2 for *_sets (sets, query_sets) */
 } scan_vtab;
 
 typedef struct {
@@ -1422,6 +1423,70 @@ static int vt_connect_batch_filtered(sqlite3 *db, void *aux, int argc, const cha
     (void)argc; (void)argv; (void)err;
     return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, rowids hidden, query, id, distance);", 1, out);
 }
+static int vt_connect_batch_sets(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
+    (void)argc; (void)argv; (void)err;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, sets hidden, query_sets hidden, query, id, distance);", 2, out);
+}
+
+/* ------------------------------------------------------------------------------------------------ per-query sets
+ * vector_*_scan_batch_sets(tbl, col, vectors, k, sets, query_sets): query b's k nearest among the rows of its own set.  `sets` is a
+ * BLOB of little-endian (int64 set, int64 rowid) pairs (vector_rowid_sets builds it); `query_sets` a BLOB of nq int64 set indexes
+ * (vector_rowid_set builds it), or NULL: query b uses set b.  Set indexes may be sparse; one that no pair names is an empty set.
+ * Each query's rows equal vector_*_scan_batch_filtered with that query's set (vsb_group_scan_topk_sets, DESIGN §3.14). */
+static int check_sets_args(scan_vtab *vt, const char *fname, sqlite3_value *sets, sqlite3_value *qsets) {
+    int t = sqlite3_value_type(sets);
+    if (t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument 5 must be of type BLOB (got %s).", fname, sql_type_name(t));
+    if (sqlite3_value_bytes(sets) % 16 != 0)
+        return vtab_error(&vt->base, "%s: sets has %d bytes, expected a multiple of 16 (int64 set, int64 rowid pairs).", fname, sqlite3_value_bytes(sets));
+    t = sqlite3_value_type(qsets);
+    if (t != SQLITE_BLOB && t != SQLITE_NULL)
+        return vtab_error(&vt->base, "%s: argument 6 must be of type BLOB or NULL (got %s).", fname, sql_type_name(t));
+    if (t == SQLITE_BLOB && sqlite3_value_bytes(qsets) % 8 != 0)
+        return vtab_error(&vt->base, "%s: query_sets has %d bytes, expected a multiple of 8 (int64 set indexes).", fname, sqlite3_value_bytes(qsets));
+    return SQLITE_OK;
+}
+
+static int cmp_i64(const void *a, const void *b) {
+    const int64_t x = *(const int64_t *)a, y = *(const int64_t *)b;
+    return x < y ? -1 : x > y;
+}
+static int cmp_pair(const void *a, const void *b) { return cmp_i64(a, b); }   /* (set, rowid) pairs by set */
+
+/* the sets the nq queries name, as dense bitmaps over the resident column ix (*bits: nsets x (rows + 31) / 32 words) and each
+ * query's dense set index (*soq); sqlite3_free both */
+static int sets_bitmaps(scan_vtab *vt, const char *fname, sqlite3_value *sets, sqlite3_value *qsets, int nq, vsb_group *ix,
+                        uint32_t **bits, int32_t **soq, int *nsets) {
+    const sqlite3_int64 npairs = sqlite3_value_bytes(sets) / 16, rows = vsb_group_rows(ix), words = (rows + 31) / 32;
+    int64_t *q = (int64_t *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int64_t));
+    int64_t *keys = (int64_t *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int64_t));
+    int64_t *pairs = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * 16);
+    int64_t *ids = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * sizeof(int64_t));
+    int32_t *dense = (int32_t *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int32_t));
+    uint32_t *out = 0;
+    int rc = (q && keys && pairs && ids && dense) ? SQLITE_OK : SQLITE_NOMEM, n = 0;
+    if (rc != SQLITE_OK) goto done;
+    for (int b = 0; b < nq; ++b) q[b] = sqlite3_value_type(qsets) == SQLITE_NULL ? b : ((const int64_t *)sqlite3_value_blob(qsets))[b];
+    memcpy(keys, q, (size_t)nq * sizeof(int64_t));
+    qsort(keys, (size_t)nq, sizeof(int64_t), cmp_i64);
+    for (int b = 0; b < nq; ++b) if (n == 0 || keys[n - 1] != keys[b]) keys[n++] = keys[b];     /* distinct set indexes -> dense 0 .. n-1 */
+    for (int b = 0; b < nq; ++b) dense[b] = (int32_t)((const int64_t *)bsearch(&q[b], keys, (size_t)n, sizeof(int64_t), cmp_i64) - keys);
+    if (npairs > 0) memcpy(pairs, sqlite3_value_blob(sets), (size_t)npairs * 16);   /* little-endian host */
+    qsort(pairs, (size_t)npairs, 16, cmp_pair);
+    out = (uint32_t *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * (sqlite3_uint64)(words + 1) * sizeof(uint32_t));
+    if (!out) { rc = SQLITE_NOMEM; goto done; }
+    for (sqlite3_int64 i = 0, d = 0; d < n; ++d) {                       /* pairs and keys both ascending by set */
+        while (i < npairs && pairs[2 * i] < keys[d]) ++i;
+        sqlite3_int64 m = 0;
+        for (; i < npairs && pairs[2 * i] == keys[d]; ++i) ids[m++] = pairs[2 * i + 1];
+        if (vsb_group_rowid_bitmap(ix, ids, m, out + d * words) < 0) { rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error()); goto done; }
+    }
+done:
+    sqlite3_free(q); sqlite3_free(keys); sqlite3_free(pairs); sqlite3_free(ids);
+    if (rc != SQLITE_OK) { sqlite3_free(out); sqlite3_free(dense); return rc; }
+    *bits = out; *soq = dense; *nsets = n;
+    return SQLITE_OK;
+}
+
 static void batch_skip_empty(scan_cursor *c) {
     while (c->bq < c->bnq && c->bj >= c->bcounts[c->bq]) { ++c->bq; c->bj = 0; }
 }
@@ -1461,13 +1526,16 @@ static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv
         if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
         if (i == 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 4) { int rc = check_rowids_arg(vt, fname, argv[4]); if (rc != SQLITE_OK) return rc; }
+        if (i == 4 && filtered == 1) { int rc = check_rowids_arg(vt, fname, argv[4]); if (rc != SQLITE_OK) return rc; }
+        if (i == 4 && filtered == 2) { int rc = check_sets_args(vt, fname, argv[4], argv[5]); if (rc != SQLITE_OK) return rc; }
     }
     const char *tbl = (const char *)sqlite3_value_text(argv[0]);
     const char *col = (const char *)sqlite3_value_text(argv[1]);
     vcolumn *v = ctx_find(vt->ctx, tbl, col);
     if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
     const int need = v->dim * elem_size(v->vtype);
+    uint32_t *setbits = 0;
+    int32_t *soq = 0;
     void *owned = 0;
     const uint8_t *queries = 0;
     int bytes = 0;
@@ -1489,6 +1557,10 @@ static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv
         goto out;
     }
     const int nq = bytes / need;
+    if (filtered == 2 && sqlite3_value_type(argv[5]) == SQLITE_BLOB && sqlite3_value_bytes(argv[5]) / 8 != nq) {
+        rc = vtab_error(&vt->base, "%s: query_sets holds %d set indexes for %d queries.", fname, sqlite3_value_bytes(argv[5]) / 8, nq);
+        goto out;
+    }
     rc = resident_index(vt, v, tbl, col, fname, quantized, &ix);
     if (rc != SQLITE_OK) goto out;
     if (quantized) {                                                     /* quantize every query like vQuantRun does for one (:2162-2177) */
@@ -1508,7 +1580,13 @@ static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv
         c->bcounts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
         if (!c->ids || !c->dist || !c->bcounts) { rc = SQLITE_NOMEM; goto out; }
         int src;
-        if (filtered) {
+        if (filtered == 2) {
+            int nsets = 0;
+            rc = sets_bitmaps(vt, fname, argv[4], argv[5], nq, ix, &setbits, &soq, &nsets);
+            if (rc != SQLITE_OK) goto out;
+            src = vsb_group_scan_topk_sets(ix, v->metric, queries, nq, k, setbits, nsets, vsb_group_rows(ix), soq, (int64_t *)c->ids, c->dist,
+                                           c->bcounts, 0);
+        } else if (filtered) {
             rc = rowids_bitmap(vt, fname, argv[4], ix, &allow);
             if (rc != SQLITE_OK) goto out;
             src = vsb_group_scan_topk_filtered(ix, v->metric, queries, nq, k, allow, vsb_group_rows(ix), (int64_t *)c->ids, c->dist, c->bcounts, 0);
@@ -1527,6 +1605,8 @@ out:
     sqlite3_free(owned);
     sqlite3_free(qq);
     sqlite3_free(allow);
+    sqlite3_free(setbits);
+    sqlite3_free(soq);
     return rc;
 }
 static int vt_filter_full_batch(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_full_scan_batch", 0); }
@@ -1541,6 +1621,12 @@ static sqlite3_module mod_full_batch_filtered = {0, 0, vt_connect_batch_filtered
                                                  vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 static sqlite3_module mod_quant_batch_filtered = {0, 0, vt_connect_batch_filtered, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch_filtered,
                                                   vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+static int vt_filter_full_batch_sets(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_full_scan_batch_sets", 0); }
+static int vt_filter_quant_batch_sets(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_quantize_scan_batch_sets", 1); }
+static sqlite3_module mod_full_batch_sets = {0, 0, vt_connect_batch_sets, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_full_batch_sets,
+                                             vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+static sqlite3_module mod_quant_batch_sets = {0, 0, vt_connect_batch_sets, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch_sets,
+                                              vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 
 #define SCAN_MODULE(NAME, CONNECT, BEST, FILTER)                                                                          \
     static sqlite3_module NAME = {0, 0, CONNECT, BEST, vt_disconnect, 0, vt_open, vt_close, FILTER, vt_next, vt_eof, \
@@ -1727,17 +1813,29 @@ static void rowid_set_step(sqlite3_context *ctx, int argc, sqlite3_value **argv)
     }
     s->v[s->n++] = (int64_t)sqlite3_value_int64(argv[0]);
 }
-static void rowid_set_final(sqlite3_context *ctx) {
+static void rowid_set_emit(sqlite3_context *ctx, const char *fname, const char *what) {
     rowid_set *s = (rowid_set *)sqlite3_aggregate_context(ctx, 0);
     if (!s || s->n == 0) {
         sqlite3_result_blob(ctx, "", 0, SQLITE_STATIC);
     } else if (s->n > INT32_MAX / 8) {
-        fn_error(ctx, SQLITE_ERROR,"vector_rowid_set: %lld rowids do not fit in one BLOB.", (long long)s->n);
+        fn_error(ctx, SQLITE_ERROR,"%s: %lld %s do not fit in one BLOB.", fname, (long long)s->n, what);
     } else {
         sqlite3_result_blob(ctx, s->v, (int)(s->n * 8), SQLITE_TRANSIENT);
     }
     if (s) sqlite3_free(s->v);
 }
+static void rowid_set_final(sqlite3_context *ctx) { rowid_set_emit(ctx, "vector_rowid_set", "rowids"); }
+
+/* vector_rowid_sets(set, rowid): aggregate of the rows where neither is NULL as the `sets` BLOB of vector_*_scan_batch_sets:
+ * little-endian (int64 set, int64 rowid) pairs, e.g. (SELECT vector_rowid_sets(tenant, rowid) FROM docs) */
+static void rowid_sets_step(sqlite3_context *ctx, int argc, sqlite3_value **argv) {
+    (void)argc;
+    if (sqlite3_value_type(argv[0]) == SQLITE_NULL || sqlite3_value_type(argv[1]) == SQLITE_NULL) return;
+    rowid_set_step(ctx, 1, argv);
+    rowid_set *s = (rowid_set *)sqlite3_aggregate_context(ctx, 0);
+    if (s && s->n % 2 == 1) rowid_set_step(ctx, 1, argv + 1);         /* the set was appended: now its rowid */
+}
+static void rowid_sets_final(sqlite3_context *ctx) { rowid_set_emit(ctx, "vector_rowid_sets", "values"); }
 
 /* ------------------------------------------------------------------------------------------------ entry point */
 __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char **err, const sqlite3_api_routines *api) { /* :2555-2638 */
@@ -1778,6 +1876,9 @@ __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char
     if ((rc = sqlite3_create_module(db, "vector_full_scan_batch_filtered", &mod_full_batch_filtered, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch_filtered", &mod_quant_batch_filtered, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_function(db, "vector_rowid_set", 1, SQLITE_UTF8, ctx, 0, rowid_set_step, rowid_set_final)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_function(db, "vector_rowid_sets", 2, SQLITE_UTF8, ctx, 0, rowid_sets_step, rowid_sets_final)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_full_scan_batch_sets", &mod_full_batch_sets, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch_sets", &mod_quant_batch_sets, ctx)) != SQLITE_OK) return rc;
     /* additions: range scans */
     if ((rc = sqlite3_create_module(db, "vector_full_scan_range", &mod_full_range, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range", &mod_quant_range, ctx)) != SQLITE_OK) return rc;

@@ -275,7 +275,8 @@ VSB_API int vsb_exchange_batch_collect(vsb_index *ix, int ticket, int nq, int k,
  * order: shard s holds rows [capacity*s/ngpus, capacity*(s+1)/ngpus).  Rows are appended in scan order exactly like the
  * single-index calls; scans have the contract of vsb_scan_topk / vsb_scan_all.  Every shard's filter pushes its head to the
  * leader GPU over NVLink peer memory (cudaDeviceEnablePeerAccess); batched queries gather the shards' entry logs with
- * cudaMemcpyPeerAsync and merge on the leader.  ngpus == 1 is exactly a vsb_index. */
+ * cudaMemcpyPeerAsync and merge on the leader.  Every query kind runs the same code for an index and a group, chosen by the
+ * shard count: ngpus == 1 takes exactly the paths of a vsb_index. */
 typedef struct vsb_group vsb_group;
 VSB_API int vsb_group_create(vsb_group **out, int first_device, int ngpus, int vtype, int dim, int64_t capacity_rows);
 VSB_API int vsb_group_append_dense(vsb_group *g, const void *vectors, const int64_t *rowids, int64_t nrows);

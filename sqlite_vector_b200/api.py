@@ -293,8 +293,63 @@ def load_engine() -> Engine:
     return _ENGINE
 
 
-class Index:
+class _Column:
+    """The query methods of a column's shards, shared by Index and Group: each calls the C entry point `_prefix` + its name
+    (vsb_scan_topk or vsb_group_scan_topk, ...); rows are in the column's scan order"""
+
+    _prefix = ""
+    _rowid_bitmap = ""
+
+    def _fn(self, name: str):
+        return getattr(self.eng.lib, self._prefix + name)
+
+    def scan_topk(self, metric: int, queries: np.ndarray, k: int, max_index: int | None = None, as_arrays: bool = False):
+        """top-k of one query or a batch.  Returns one (rowids, distances) pair per query, or with as_arrays the C-ABI's own
+        output (rowids[nq, k], distances[nq, k], counts[nq]) without the per-query Python objects."""
+        fn = self._fn("scan_topk")
+        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: fn(self.h, metric, q, nq, k, ids, dist, counts, mi),
+                     queries, k, max_index, as_arrays)
+
+    def scan_topk_filtered(self, metric: int, queries: np.ndarray, k: int, allow, max_index: int | None = None, as_arrays: bool = False):
+        """scan_topk among the eligible rows only (vsb_scan_topk_filtered): `allow` is a boolean mask over the scan-order rows or
+        a uint32 row bitmap (row_bitmap, rowid_bitmap)"""
+        bits, rows, fn = _allow_words(allow, self.rows), self.rows, self._fn("scan_topk_filtered")
+        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: fn(self.h, metric, q, nq, k, _ptr(bits), rows, ids, dist, counts, mi),
+                     queries, k, max_index, as_arrays)
+
+    def scan_topk_rows(self, metric: int, queries: np.ndarray, k: int, rowid_lists, max_index: int | None = None, as_arrays: bool = False):
+        """scan_topk among per-query lists of rowids, reading only the listed rows (vsb_scan_topk_rows): rowid_lists holds one
+        sequence of rowids per query; each query's result equals scan_topk_filtered with the bitmap of its rowids"""
+        return _rows_topk(self.eng, self._fn("scan_topk_rows"), self.h, metric, queries, k, rowid_lists, max_index, as_arrays)
+
+    def scan_topk_sets(self, metric: int, queries: np.ndarray, k: int, sets, set_of_query=None, as_arrays: bool = False):
+        """scan_topk of each query among its own set of rows (vsb_scan_topk_sets), one pass of the column for the whole batch:
+        `sets` is a list of boolean masks over the scan-order rows or of uint32 row bitmaps, set_of_query[b] the index of query
+        b's set (None: query b uses set b); each query's result equals scan_topk_filtered with its set"""
+        return _sets_topk(self.eng, self._fn("scan_topk_sets"), self.h, self.rows, metric, queries, k, sets, set_of_query, as_arrays)
+
+    def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
+        """every row with distance < radius (vsb_scan_range), for one query or a batch; radius: one value or one per query, allow:
+        None, a boolean mask over the scan-order rows or a uint32 row bitmap.  Returns one (rowids, distances) pair per query"""
+        return _range(self.eng, self._fn("scan_range"), self.h, self.rows, metric, queries, radius, allow)
+
+    def rowid_bitmap(self, rowids) -> tuple[np.ndarray, int]:
+        """(row bitmap of the rows whose rowid is in `rowids`, number of such rows) (vsb_index_rowid_bitmap)"""
+        return _rowid_bitmap(self.eng, getattr(self.eng.lib, self._rowid_bitmap), self.h, self.rows, rowids)
+
+    def scan_all(self, metric: int, query: np.ndarray, want_rowids: bool = False):
+        n = self.rows
+        dist = np.zeros(n, dtype=np.float32)
+        ids = np.zeros(n, dtype=np.int64) if want_rowids else None
+        self.eng.check(self._fn("scan_all")(self.h, metric, _ptr(np.ascontiguousarray(query)), _ptr(dist), _ptr(ids)))
+        return (dist, ids) if want_rowids else dist
+
+
+class Index(_Column):
     """A resident shard of one column on one GPU (table_context.preloaded on the device)."""
+
+    _prefix = "vsb_"
+    _rowid_bitmap = "vsb_index_rowid_bitmap"
 
     def __init__(self, vtype: int, dim: int, capacity: int, device: int = 0, first_seq: int = 0, engine: Engine | None = None,
                  window_rows: int = 0):
@@ -340,48 +395,6 @@ class Index:
 
     def finalize(self):
         self.eng.check(self.eng.lib.vsb_index_finalize(self.h))
-
-    def scan_topk(self, metric: int, queries: np.ndarray, k: int, max_index: int | None = None, as_arrays: bool = False):
-        """top-k of one query or a batch.  Returns one (rowids, distances) pair per query, or with as_arrays the C-ABI's own
-        output (rowids[nq, k], distances[nq, k], counts[nq]) without the per-query Python objects."""
-        lib = self.eng.lib
-        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_scan_topk(self.h, metric, q, nq, k, ids, dist, counts, mi),
-                     queries, k, max_index, as_arrays)
-
-    def scan_topk_filtered(self, metric: int, queries: np.ndarray, k: int, allow, max_index: int | None = None, as_arrays: bool = False):
-        """scan_topk among the eligible rows only (vsb_scan_topk_filtered): `allow` is a boolean mask over the scan-order rows or
-        a uint32 row bitmap (row_bitmap, rowid_bitmap)"""
-        bits, lib = _allow_words(allow, self.rows), self.eng.lib
-        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
-                                                                                               ids, dist, counts, mi),
-                     queries, k, max_index, as_arrays)
-
-    def scan_topk_rows(self, metric: int, queries: np.ndarray, k: int, rowid_lists, max_index: int | None = None, as_arrays: bool = False):
-        """scan_topk among per-query lists of rowids, reading only the listed rows (vsb_scan_topk_rows): rowid_lists holds one
-        sequence of rowids per query; each query's result equals scan_topk_filtered with the bitmap of its rowids"""
-        return _rows_topk(self.eng, self.eng.lib.vsb_scan_topk_rows, self.h, metric, queries, k, rowid_lists, max_index, as_arrays)
-
-    def scan_topk_sets(self, metric: int, queries: np.ndarray, k: int, sets, set_of_query=None, as_arrays: bool = False):
-        """scan_topk of each query among its own set of rows (vsb_scan_topk_sets), one pass of the column for the whole batch:
-        `sets` is a list of boolean masks over the scan-order rows or of uint32 row bitmaps, set_of_query[b] the index of query
-        b's set (None: query b uses set b); each query's result equals scan_topk_filtered with its set"""
-        return _sets_topk(self.eng, self.eng.lib.vsb_scan_topk_sets, self.h, self.rows, metric, queries, k, sets, set_of_query, as_arrays)
-
-    def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
-        """every row with distance < radius (vsb_scan_range), for one query or a batch; radius: one value or one per query, allow:
-        None, a boolean mask over the scan-order rows or a uint32 row bitmap.  Returns one (rowids, distances) pair per query"""
-        return _range(self.eng, self.eng.lib.vsb_scan_range, self.h, self.rows, metric, queries, radius, allow)
-
-    def rowid_bitmap(self, rowids) -> tuple[np.ndarray, int]:
-        """(row bitmap of the rows whose rowid is in `rowids`, number of such rows) (vsb_index_rowid_bitmap)"""
-        return _rowid_bitmap(self.eng, self.eng.lib.vsb_index_rowid_bitmap, self.h, self.rows, rowids)
-
-    def scan_all(self, metric: int, query: np.ndarray, want_rowids: bool = False):
-        n = self.rows
-        dist = np.zeros(n, dtype=np.float32)
-        ids = np.zeros(n, dtype=np.int64) if want_rowids else None
-        self.eng.check(self.eng.lib.vsb_scan_all(self.h, metric, _ptr(np.ascontiguousarray(query)), _ptr(dist), _ptr(ids)))
-        return (dist, ids) if want_rowids else dist
 
     def scan_candidates(self, metric: int, queries: np.ndarray, k: int, cap: int = 8192):
         q2 = np.ascontiguousarray(queries).reshape(-1, queries.shape[-1])
@@ -594,8 +607,11 @@ class Index:
         return ids[:cnt.value].copy(), dist[:cnt.value].copy()
 
 
-class Group:
+class Group(_Column):
     """One column row-sharded over several GPUs inside ONE process (what the SQLite extension uses with gpus=N)."""
+
+    _prefix = "vsb_group_"
+    _rowid_bitmap = "vsb_group_rowid_bitmap"
 
     def __init__(self, vtype: int, dim: int, capacity: int, ngpus: int, first_device: int = 0, engine: Engine | None = None):
         self.eng = engine or load_engine()
@@ -628,41 +644,6 @@ class Group:
 
     def finalize(self):
         self.eng.check(self.eng.lib.vsb_group_finalize(self.h))
-
-    def scan_topk(self, metric: int, queries: np.ndarray, k: int, max_index: int | None = None):
-        lib = self.eng.lib
-        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_group_scan_topk(self.h, metric, q, nq, k, ids, dist, counts, mi),
-                     queries, k, max_index, False)
-
-    def scan_topk_filtered(self, metric: int, queries: np.ndarray, k: int, allow, max_index: int | None = None):
-        """Index.scan_topk_filtered over the group's global scan order (vsb_group_scan_topk_filtered)"""
-        bits, lib = _allow_words(allow, self.rows), self.eng.lib
-        return _topk(self.eng, lambda q, nq, ids, dist, counts, mi: lib.vsb_group_scan_topk_filtered(self.h, metric, q, nq, k, _ptr(bits), self.rows,
-                                                                                                     ids, dist, counts, mi),
-                     queries, k, max_index, False)
-
-    def scan_topk_rows(self, metric: int, queries: np.ndarray, k: int, rowid_lists, max_index: int | None = None, as_arrays: bool = False):
-        """Index.scan_topk_rows over the group's global scan order (vsb_group_scan_topk_rows)"""
-        return _rows_topk(self.eng, self.eng.lib.vsb_group_scan_topk_rows, self.h, metric, queries, k, rowid_lists, max_index, as_arrays)
-
-    def scan_topk_sets(self, metric: int, queries: np.ndarray, k: int, sets, set_of_query=None, as_arrays: bool = False):
-        """Index.scan_topk_sets over the group's global scan order (vsb_group_scan_topk_sets)"""
-        return _sets_topk(self.eng, self.eng.lib.vsb_group_scan_topk_sets, self.h, self.rows, metric, queries, k, sets, set_of_query, as_arrays)
-
-    def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
-        """Index.scan_range over the group's global scan order (vsb_group_scan_range)"""
-        return _range(self.eng, self.eng.lib.vsb_group_scan_range, self.h, self.rows, metric, queries, radius, allow)
-
-    def rowid_bitmap(self, rowids) -> tuple[np.ndarray, int]:
-        """Index.rowid_bitmap over the group's global scan order (vsb_group_rowid_bitmap)"""
-        return _rowid_bitmap(self.eng, self.eng.lib.vsb_group_rowid_bitmap, self.h, self.rows, rowids)
-
-    def scan_all(self, metric: int, query: np.ndarray, want_rowids: bool = False):
-        n = self.rows
-        dist = np.zeros(n, dtype=np.float32)
-        ids = np.zeros(n, dtype=np.int64) if want_rowids else None
-        self.eng.check(self.eng.lib.vsb_group_scan_all(self.h, metric, _ptr(np.ascontiguousarray(query)), _ptr(dist), _ptr(ids)))
-        return (dist, ids) if want_rowids else dist
 
 
 class Quantizer:

@@ -1241,6 +1241,7 @@ int large_k_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k,
 
 #include "batch_host.inc"
 #include "exchange.inc"
+#include "column.inc"
 #include "quantize.inc"
 
 // ====================================================================== C ABI
@@ -1543,134 +1544,6 @@ void vsb_index_free(vsb_index *ix) {
     delete ix;
 }
 
-int vsb_scan_topk(vsb_index *ix, int metric, const void *queries, int nq, int k, int64_t *out_rowids, double *out_dist,
-                  int *out_counts, int *max_index) {
-    if (check_index(ix)) return VSB_EINVAL;
-    if (!queries || nq < 0 || k < 0) return fail(VSB_EINVAL, "bad scan arguments");
-    if (k == 0) {  // k == 0 yields an empty result (src/sqlite-vector.c:1795-1796)
-        for (int b = 0; b < nq; ++b) if (out_counts) out_counts[b] = 0;
-        return VSB_OK;
-    }
-    if (!out_rowids || !out_dist) return fail(VSB_EINVAL, "output buffers are null");
-    const size_t qbytes = (size_t)ix->dim * ix->esize;
-    if (batch_supported(ix, metric, nq, k)) {   // tensor-core path; every query starts from a fresh cursor (max_index 0)
-        const auto t0 = std::chrono::steady_clock::now();
-        int rc = batch_scan(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts);
-        ix->st_batch_us += std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t0).count();
-        if (rc == VSB_OK) return VSB_OK;
-        if (rc != VSB_ERANGE) return rc;
-        ix->st_fallbacks++;                      // capacity exceeded: per-query path below
-    }
-    LkbPlan lkb;
-    if (large_k_batch_supported(ix, metric, nq, k, lkb)) {   // k > kMaxK: the large-k batch (DESIGN §3.12), every query from max_index 0
-        std::vector<std::vector<uint2>> all;
-        const int rc = large_k_index(ix, metric, queries, nq, k, lkb, all);
-        if (rc) return rc;
-        replay_queries(ix, nq, k, out_rowids, out_dist, out_counts, [&](int q, SlotState &s) {
-            slots_offer_cands(s, all[(size_t)q].data(), all[(size_t)q].size(), [&](uint32_t row) { return rowid_of(ix, row); });
-        });
-        return VSB_OK;
-    }
-    std::vector<uint2> cands;
-    QueryCursor cur(max_index, nq);
-    for (int b = 0; b < nq; ++b) {
-        int rc = query_candidates(ix, metric, (const uint8_t *)queries + (size_t)b * qbytes, k, cands);
-        if (rc) return rc;
-        const int cnt = slots_replay(k, cur.next(), out_dist + (size_t)b * k, out_rowids + (size_t)b * k, [&](SlotState &s) {
-            slots_offer_cands(s, cands.data(), cands.size(), [&](uint32_t row) { return rowid_of(ix, row); });
-            return (int)VSB_OK;
-        });
-        if (out_counts) out_counts[b] = cnt;
-    }
-    cur.finish();
-    return VSB_OK;
-}
-
-int vsb_scan_topk_filtered(vsb_index *ix, int metric, const void *queries, int nq, int k, const uint32_t *allow, int64_t nbits,
-                           int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index) {
-    if (check_index(ix)) return VSB_EINVAL;
-    if (nbits != ix->n) return fail(VSB_EINVAL, "the row bitmap has %lld bits, the index %lld rows", (long long)nbits, ix->n);
-    if (!allow && nbits > 0) return fail(VSB_EINVAL, "the row bitmap is null");
-    FilterScope scope;
-    const int rc = filter_begin(ix, allow, &scope);
-    if (rc) return rc;
-    return vsb_scan_topk(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts, max_index);
-}
-
-int vsb_scan_topk_sets(vsb_index *ix, int metric, const void *queries, int nq, int k, const uint32_t *sets, int nsets, int64_t nbits,
-                       const int32_t *set_of_query, int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index) {
-    if (check_index(ix)) return VSB_EINVAL;
-    std::vector<int> soq;
-    int rc = sets_check(queries, nq, k, sets, nsets, nbits, ix->n, set_of_query, soq);
-    if (rc) return rc;
-    if (k == 0 || nq == 0) {
-        for (int b = 0; b < nq; ++b) if (out_counts) out_counts[b] = 0;
-        return VSB_OK;
-    }
-    if (!out_rowids || !out_dist) return fail(VSB_EINVAL, "output buffers are null");
-    const long long words = (ix->n + 31) / 32;
-    if (batch_supported(ix, metric, nq, k)) {   // one pass of the column for every set (DESIGN §3.14)
-        {
-            std::vector<int> dense = soq;
-            const std::vector<int> used = sets_used(dense, nsets);
-            SetsScope scope;
-            rc = sets_begin(ix, used, [&](int i) { return sets + (size_t)used[(size_t)i] * words; }, dense, k, &scope);
-            if (rc == VSB_OK) rc = batch_scan(ix, metric, queries, nq, k, out_rowids, out_dist, out_counts);
-        }
-        if (rc == VSB_OK) {
-            ix->st_sets_batches++;
-            return VSB_OK;
-        }
-        if (rc != VSB_ERANGE) return rc;
-        ix->st_sets_fallbacks++;
-    }
-    return sets_by_set(queries, nq, k, (size_t)ix->dim * ix->esize, soq, out_rowids, out_dist, out_counts, max_index,
-                       [&](const void *q, int m, int s, int64_t *ids, double *dist, int *cnt, int *mi) {
-                           return vsb_scan_topk_filtered(ix, metric, q, m, k, sets + (size_t)s * words, nbits, ids, dist, cnt, mi);
-                       });
-}
-
-int vsb_scan_topk_rows(vsb_index *ix, int metric, const void *queries, int nq, int k, const int64_t *rowids, const int64_t *offsets,
-                       int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index) {
-    if (check_index(ix)) return VSB_EINVAL;
-    int rc = rows_check(metric, queries, nq, k, rowids, offsets);
-    if (rc) return rc;
-    if (k == 0) {
-        for (int b = 0; b < nq; ++b) if (out_counts) out_counts[b] = 0;
-        return VSB_OK;
-    }
-    if (!out_rowids || !out_dist) return fail(VSB_EINVAL, "output buffers are null");
-    std::vector<std::vector<uint2>> cands;
-    rc = rows_index(ix, metric, queries, nq, k, rowids, offsets, cands);
-    if (rc) return rc;
-    rows_replay(nq, k, out_rowids, out_dist, out_counts, max_index, [&](int q, SlotState &s) {
-        slots_offer_cands(s, cands[(size_t)q].data(), cands[(size_t)q].size(), [&](uint32_t row) { return rowid_of(ix, row); });
-    });
-    return VSB_OK;
-}
-
-int vsb_scan_range(vsb_index *ix, int metric, const void *queries, int nq, const double *radius, const uint32_t *allow, int64_t nbits,
-                   vsb_range **out) {
-    if (check_index(ix)) return VSB_EINVAL;
-    int rc = range_begin(metric, queries, nq, radius, out);
-    if (rc) return rc;
-    std::unique_ptr<vsb_range> res(*out);
-    *out = nullptr;
-    FilterScope scope;
-    if (allow) {
-        if (nbits != ix->n) return fail(VSB_EINVAL, "the row bitmap has %lld bits, the index %lld rows", (long long)nbits, ix->n);
-        rc = filter_begin(ix, allow, &scope);
-        if (rc) return rc;
-    }
-    std::vector<std::vector<uint2>> all;
-    rc = range_index(ix, metric, queries, nq, radius, all);
-    if (rc) return rc;
-    for (int b = 0; b < nq; ++b)
-        range_put(res.get(), b, all[(size_t)b].size(), [&](size_t i) { return std::make_pair(rowid_of(ix, all[(size_t)b][i].x), all[(size_t)b][i].y); });
-    *out = res.release();
-    return VSB_OK;
-}
-
 int vsb_range_get(const vsb_range *r, int q, const int64_t **rowids, const double **dist, int64_t *count) {
     if (!r || q < 0 || (size_t)q >= r->ids.size()) return fail(VSB_EINVAL, "bad range result or query %d", q);
     if (rowids) *rowids = r->ids[(size_t)q].data();
@@ -1680,29 +1553,6 @@ int vsb_range_get(const vsb_range *r, int q, const int64_t **rowids, const doubl
 }
 
 void vsb_range_free(vsb_range *r) { delete r; }
-
-int64_t vsb_index_rowid_bitmap(vsb_index *ix, const int64_t *rowids, int64_t n, uint32_t *out_bits) {
-    if (check_index(ix)) return VSB_EINVAL;
-    if (n < 0 || (!rowids && n > 0) || !out_bits) return fail(VSB_EINVAL, "bad rowid bitmap arguments");
-    memset(out_bits, 0, sizeof(uint32_t) * (size_t)((ix->n + 31) / 32));
-    rows_of_rowids(ix, rowids, n, [&](long long row) { out_bits[row >> 5] |= 1u << (row & 31); });
-    return count_bits(out_bits, 0, ix->n);
-}
-
-int vsb_scan_all(vsb_index *ix, int metric, const void *query, float *out_dist, int64_t *out_rowids) {
-    if (check_index(ix)) return VSB_EINVAL;
-    if (!query || !out_dist) return fail(VSB_EINVAL, "bad scan arguments");
-    Slot *slot = nullptr;
-    int rc = stage_host_query(ix, query, &slot);
-    if (rc) return rc;
-    std::vector<float> dist;
-    rc = scan_all_into(ix, metric, slot->d_query, dist);
-    if (rc) return rc;
-    memcpy(out_dist, dist.data(), sizeof(float) * (size_t)ix->n);
-    if (out_rowids)
-        for (long long i = 0; i < ix->n; ++i) out_rowids[i] = rowid_of(ix, (uint32_t)i);
-    return VSB_OK;
-}
 
 int vsb_scan_candidates(vsb_index *ix, int metric, const void *queries, int nq, int k, vsb_candidate *out, int cap_per_query,
                         int *out_counts) {

@@ -196,13 +196,20 @@ VSB_API int vsb_replay_topk(const vsb_candidate *cands, int n, int k, int *max_i
 /* runs the scan kernels for ONE query that is already in device memory (pitch-padded, see
  * vsb_index_query_pitch) and leaves the candidates in the engine's output buffer; no host copies. */
 VSB_API int vsb_scan_device_query(vsb_index *ix, int metric, const void *d_query, int k); /* returns the result slot or <0 */
-/* general form: launches scan + filter for ONE query and returns immediately with the result slot (>= 0).  The query is
- * either in device memory (query_on_device != 0, pitch-padded) or in HOST memory (dim elements; staged through the
- * slot's pinned buffer with cudaMemcpyAsync, the xFilter argument of the reference, src/sqlite-vector.c:1774-1776).
- * fetch != 0 also copies the slot's result block to pinned host memory for vsb_collect; pass 0 when the block is
- * exchanged on the device (vsb_result_block + all-gather).  Up to vsb_index_stat("slots") queries may be in flight:
- * slot < 0 hands slots out round-robin, slot >= 0 names the slot (a launcher that gathers groups of consecutive
- * slots manages them itself); either way a slot must be collected/merged before it is used again. */
+/* general form: submits scan + filter for ONE query and returns immediately with the result slot (>= 0).  The query is
+ * either in device memory (query_on_device != 0, pitch-padded; read when its pass runs) or in HOST memory (dim elements;
+ * staged through the slot's pinned buffer with cudaMemcpyAsync at submission, the xFilter argument of the reference,
+ * src/sqlite-vector.c:1774-1776).  fetch != 0 also copies the slot's result block to pinned host memory for vsb_collect;
+ * pass 0 when the block is exchanged on the device (vsb_result_block + all-gather).  Up to vsb_index_stat("slots") queries
+ * may be in flight: slot < 0 hands slots out round-robin, slot >= 0 names the slot (a launcher that gathers groups of
+ * consecutive slots manages them itself); either way a slot must be collected/merged before it is used again.
+ * Queries share passes of the column (DESIGN §3.2): while the caller has an uncollected query (fetch != 0) on this index, a
+ * new submission is held, and the held queries run as ONE pass, which reads the column once for all of them, at the first
+ * of: the pass is full (vsb_index_stat "plan_pass_max"), a held query is collected, a submission with another metric or k
+ * (or for a held query's slot) arrives, any other call on the index (vsb_collect_last, vsb_result_block, vsb_scan_topk*,
+ * range, batch, profile or debug calls, close).  A submission with nothing outstanding, or with fetch == 0, launches at
+ * once.  So "submit i+1, collect i" pairs the queries; a caller who submits a second query and then does host work before
+ * collecting the first leaves the second waiting until it does.  Sharing a pass never changes a result. */
 VSB_API int vsb_scan_submit(vsb_index *ix, int metric, const void *query, int query_on_device, int k, int fetch, int slot);
 /* blocks until the engine stream is idle and converts the last device-side result into top-k. */
 VSB_API int vsb_collect_last(vsb_index *ix, int k, int64_t *out_rowids, double *out_dist, int *out_count);
@@ -219,7 +226,8 @@ VSB_API int vsb_merge_result_blocks(const void *blocks, int world, int64_t block
                                     int64_t *out_rowids, double *out_dist);
 /* the same for a GROUP of nq independent queries in one call (query j at queries + j * query_stride; slots first_slot ..
  * first_slot + nq - 1): what the sharded launcher uses so that its per-query host cost stays far below one shard scan.
- * Each query gets its own scan and filter launch, exactly as from vsb_scan_submit. */
+ * The queries are launched at once, as passes of up to vsb_index_stat("plan_pass_max") queries (one read of the column per
+ * pass, one filter launch per query); each query's result is what it gets alone. */
 VSB_API int vsb_scan_submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device,
                                   int k, int fetch, int first_slot);
 /* vsb_merge_result_blocks for a gathered group: query j's block of shard r is at blocks + r * rank_stride + j * block_stride;
@@ -336,8 +344,11 @@ VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row o
  * replay of such batches; a group counts it on its first shard), "large_k_replay_threads" (host threads of the last replay),
  * "rows_queries" (queries answered by vsb_scan_topk_rows), "rows_pairs" (their listed (query, row) pairs, each row counted once
  * per query), "rows_host_bytes" (bytes a streamed index's listed-rows kernel read from pinned host memory: pitch bytes per pair),
- * "sets_batches", "sets_fallbacks", "sets_levels", "sets_plan_us" (see vsb_scan_topk_sets)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
- * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging); -1 if unknown (or, for plan_*, before any scan) */
+ * "sets_batches", "sets_fallbacks", "sets_levels", "sets_plan_us" (see vsb_scan_topk_sets), "scan_passes" (top-k passes of
+ * the single-query scan kernel), "pass_queries" (the queries they scored: pass_queries / scan_passes queries per read of the
+ * column)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging), "plan_pass_max" (the widest pass of the shape at the k
+ * of the most recent top-k pass, k <= 32 before any); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);
 VSB_API void *vsb_index_stream(vsb_index *ix);           /* cudaStream_t of the engine, for event timing */
 /* kernel launch counter (all kernels launched by this library since load) */

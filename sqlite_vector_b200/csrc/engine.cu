@@ -127,8 +127,9 @@ constexpr int kMaxK = 256;               // candidate path; larger k takes the l
 constexpr int kSlots = 32;               // result slots: queries in flight (the sharded exchange moves groups of them; a rank may have at most
                                          // kSlots / 2 queries in flight so that a peer never overwrites a gather row that is still being read)
 
-// Scan workspace of one query (per-stream k-lists / CTA lists, in-CTA bounds, candidate logs): written by scan_kernel, read
-// by filter_kernel.  The Works rotate so that the filter of launch i (filter stream) overlaps the scan of launch i+1.
+// Scan workspace of one pass (per query of the pass: per-stream k-lists / CTA lists, in-CTA bounds, candidate logs, at the
+// offsets pass_lists / pass_logs / pass_streams): written by scan_kernel, read by filter_kernel.  The Works rotate so that the
+// filters of launch i (filter stream) overlap the scan of launch i+1.
 struct Work {
     DeviceBuf<float> d_lists, d_tlocal;
     DeviceBuf<uint2> d_logs;
@@ -167,6 +168,15 @@ struct PairList {
     long long h_cap = 0;
 };
 
+// Single-query submissions held to share one pass of the column (vsb_scan_submit, DESIGN §3.2): one metric and k; query[j] is
+// what the pass reads (a host query was staged into its slot's buffer on ss when it was submitted)
+struct HeldPass {
+    int nq = 0, metric = 0, k = 0;
+    cudaStream_t ss = nullptr;
+    const uint8_t *query[kMaxPass] = {};
+    int slot[kMaxPass] = {};
+};
+
 struct BatchWs;   // batch_host.inc
 struct SetsState;   // batch_host.inc
 
@@ -200,8 +210,8 @@ struct vsb_index {
     long long st_stream_bytes = 0, st_stream_us = 0;
     int snext = 0;
     std::unique_ptr<Exchange> xch;    // peer-memory exchange (multi-GPU), see exchange.inc
-    // scan workspaces
-    int ws_kcap = 0, ws_logcap = 0, ws_streams = 0, ws_next = 0;
+    // scan workspaces, for passes of up to ws_width queries (grown to the widest pass launched so far)
+    int ws_kcap = 0, ws_logcap = 0, ws_streams = 0, ws_width = 0, ws_next = 0;
     Work work[kWorks];
     Slot slot[kSlots];
     // the allocations behind the result slots (a Slot holds views into them)
@@ -215,6 +225,10 @@ struct vsb_index {
     bool slots_ready = false;
     DeviceBuf<float> d_dist_all;
     int last_slot = -1, last_metric = 0;
+    HeldPass held;                    // vsb_scan_submit's queries waiting for a pass
+    uint32_t uncollected = 0;         // slots of vsb_scan_submit (fetch != 0) not collected yet: bit s = slot s
+    long long st_scan_passes = 0, st_pass_queries = 0;   // top-k passes and the queries they scored
+    int last_kcap = 0;                // kcap of the most recent top-k pass (vsb_index_stat "plan_pass_max")
     // optional per-kernel event timing (vsb_profile_read)
     std::vector<Event> prof_ev;         // quadruples: before scan, after scan (scan stream), before filter, after filter (filter stream)
     std::vector<int> prof_kind;         // 1 = scan only, 2 = scan + filter
@@ -271,21 +285,23 @@ namespace {
 
 // ------------------------------------------------------------------ kernel dispatch
 using ScanFn = void (*)(const ScanParams);
-template <int VT, int MC, bool D, bool R>
+// R: range mode; M: pass width (top-k and all distances)
+template <int VT, int MC, bool D, bool R, int M>
 ScanFn fn_of() {
     if constexpr (R) return scan_range_kernel<VT, MC, D>;
-    else return scan_kernel<VT, MC, D>;
+    else if constexpr (M == 1) return scan_kernel<VT, MC, D>;
+    else return scan_pass_kernel<VT, MC, D, M>;
 }
 
-template <bool R>
+template <bool R, int M>
 ScanFn pick_kernel_of(int vtype, int mc, bool direct) {
 #define ROW(VT)                                                                                                   \
     case VT:                                                                                                      \
         switch (mc) {                                                                                             \
-        case MC_L2: return direct ? fn_of<VT, MC_L2, true, R>() : fn_of<VT, MC_L2, false, R>();                   \
-        case MC_COS: return direct ? fn_of<VT, MC_COS, true, R>() : fn_of<VT, MC_COS, false, R>();                \
-        case MC_DOT: return direct ? fn_of<VT, MC_DOT, true, R>() : fn_of<VT, MC_DOT, false, R>();                \
-        case MC_L1: return direct ? fn_of<VT, MC_L1, true, R>() : fn_of<VT, MC_L1, false, R>();                   \
+        case MC_L2: return direct ? fn_of<VT, MC_L2, true, R, M>() : fn_of<VT, MC_L2, false, R, M>();             \
+        case MC_COS: return direct ? fn_of<VT, MC_COS, true, R, M>() : fn_of<VT, MC_COS, false, R, M>();          \
+        case MC_DOT: return direct ? fn_of<VT, MC_DOT, true, R, M>() : fn_of<VT, MC_DOT, false, R, M>();          \
+        case MC_L1: return direct ? fn_of<VT, MC_L1, true, R, M>() : fn_of<VT, MC_L1, false, R, M>();             \
         }                                                                                                         \
         break;
     switch (vtype) {
@@ -294,9 +310,14 @@ ScanFn pick_kernel_of(int vtype, int mc, bool direct) {
 #undef ROW
     return nullptr;
 }
-// range: the range-mode instantiation (vsb_scan_range)
-ScanFn pick_kernel(int vtype, int mc, bool direct, bool range = false) {
-    return range ? pick_kernel_of<true>(vtype, mc, direct) : pick_kernel_of<false>(vtype, mc, direct);
+// range: the range-mode instantiation (vsb_scan_range); nq: the queries of a top-k pass, which runs the narrowest width that
+// holds them
+ScanFn pick_kernel(int vtype, int mc, bool direct, bool range = false, int nq = 1) {
+    if (range) return pick_kernel_of<true, 1>(vtype, mc, direct);
+    if (nq <= 1) return pick_kernel_of<false, 1>(vtype, mc, direct);
+    if (nq <= 2) return pick_kernel_of<false, 2>(vtype, mc, direct);
+    if (nq <= 4) return pick_kernel_of<false, 4>(vtype, mc, direct);
+    return pick_kernel_of<false, 8>(vtype, mc, direct);
 }
 
 int metric_class(int metric, int *root) {
@@ -314,24 +335,27 @@ int metric_class(int metric, int *root) {
 struct Plan {
     bool direct;
     int log2P, wtile_bytes, nsw;
+    bool reserved;      // the filter reserve was left free
     size_t smem;
 };
 
-// choose lanes-per-row, ring depth and shared-memory size for (pitch, kcap)
-Plan make_plan(const vsb_index *ix, int kcap) {
+// choose lanes-per-row, ring depth and shared-memory size for (pitch, kcap) and a pass of nq queries
+Plan make_plan(const vsb_index *ix, int kcap, int nq = 1) {
     Plan pl{};
     const int pitch = ix->pitch;
     int log2P = 0;
     while (log2P < 5 && (32 >> log2P) * (long long)pitch > g_opt_stage_bytes) ++log2P;
-    // Room for 2 query + 2 list buffers, although scan_kernel uses one of each.  Giving the ring that room would change the
-    // plan at many shapes (some dims would turn from DIRECT to staged) and needs its own measurement (DESIGN §8).
-    const size_t fixed = kBarrierBytes + (((size_t)2 * pitch + (size_t)2 * kWarps * kcap * 4 + 127) & ~(size_t)127);
+    // Room for max(2, nq) query + list buffers.  A one-query pass uses one of each: the room of the second is what lets a
+    // pass of two keep the plan of one (pass_max); giving it to the ring instead would change the plan at many shapes.
+    const size_t nbuf = (size_t)std::max(2, nq);
+    const size_t fixed = kBarrierBytes + ((nbuf * pitch + nbuf * kWarps * kcap * 4 + 127) & ~(size_t)127);
     size_t avail = (size_t)ix->max_smem > fixed ? (size_t)ix->max_smem - fixed : 0;
     if (g_opt_ring_bytes > 0 && (size_t)g_opt_ring_bytes < avail) avail = (size_t)g_opt_ring_bytes;
     const size_t wtile = (size_t)(32 >> log2P) * pitch;
     // leave room on the SM for one filter block of the previous query (it runs beside the scan CTA, see launch_scan)
     const size_t reserve = filter_fast_smem(ix->num_sms) + 3072;
-    if (kcap > 0 && kcap <= 32 && avail > reserve && (avail - reserve) / kWarps / (wtile ? wtile : 1) >= 2) avail -= reserve;
+    pl.reserved = kcap > 0 && kcap <= 32 && avail > reserve && (avail - reserve) / kWarps / (wtile ? wtile : 1) >= 2;
+    if (pl.reserved) avail -= reserve;
     int nsw = (int)(avail / kWarps / (wtile ? wtile : 1));
     if (nsw > kMaxStages) nsw = kMaxStages;
     pl.direct = g_opt_direct || nsw < 2;
@@ -347,6 +371,21 @@ Plan make_plan(const vsb_index *ix, int kcap) {
         pl.smem = fixed + (size_t)kWarps * nsw * wtile;
     }
     return pl;
+}
+
+// the widest pass of a shape: the largest width whose query and list buffers fit beside the one-query plan left as it is
+// (the same lanes per row, ring depth, DIRECT and filter reserve), so that sharing a pass never slows the scan of a row
+int pass_max(const vsb_index *ix, int kcap) {
+    const Plan one = make_plan(ix, kcap);
+    int w = 1;
+    for (int m = 2; m <= kMaxPass; m *= 2) {
+        const Plan pl = make_plan(ix, kcap, m);
+        if (pl.direct != one.direct || pl.log2P != one.log2P || pl.nsw != one.nsw || pl.reserved != one.reserved ||
+            pl.smem > (size_t)ix->max_smem)
+            break;
+        w = m;
+    }
+    return w;
 }
 
 // the result slots, built on first need
@@ -387,28 +426,34 @@ int ensure_slots(vsb_index *ix) {
     return VSB_OK;
 }
 
-// waits for the scan streams and the filter stream of ix
+int flush_held(vsb_index *ix);
+
+// waits for the scan streams and the filter stream of ix (after launching the held pass)
 int drain(vsb_index *ix) {
+    const int rc = flush_held(ix);
+    if (rc) return rc;
     CU(cudaStreamSynchronize(ix->stream));
     CU(cudaStreamSynchronize(ix->stream2));
     CU(cudaStreamSynchronize(ix->fstream));
     return VSB_OK;
 }
 
-int ensure_workspace(vsb_index *ix, int k) {
-    const int kcap = (k + 31) & ~31;
-    const int logcap = std::max(256, 12 * k);
+// the workspaces hold passes of `width` queries with this k (never shrunk: a caller who never shares a pass keeps width 1)
+int ensure_workspace(vsb_index *ix, int k, int width = 1) {
+    const int kcap = std::max((k + 31) & ~31, ix->ws_kcap);
+    const int logcap = std::max(std::max(256, 12 * k), ix->ws_logcap);
+    width = std::max(width, ix->ws_width);
     const int streams = ix->num_sms * kWarps;
-    if (ix->ws_kcap >= kcap && ix->ws_logcap >= logcap && ix->ws_streams == streams) return VSB_OK;
+    if (ix->ws_kcap >= kcap && ix->ws_logcap >= logcap && ix->ws_width >= width && ix->ws_streams == streams) return VSB_OK;
     const int rc = drain(ix);       // queries in flight still use the old workspaces
     if (rc) return rc;
     Work fresh[kWorks];
     for (int i = 0; i < kWorks; ++i) {
         Work &w = fresh[i], &old = ix->work[i];
-        CU(w.d_lists.alloc(sizeof(float) * (size_t)streams * kcap));
-        CU(w.d_logs.alloc(sizeof(uint2) * (size_t)streams * logcap));
-        CU(w.d_counts.alloc(sizeof(int) * (size_t)streams));
-        CU(w.d_tlocal.alloc(sizeof(float) * (size_t)streams));
+        CU(w.d_lists.alloc(sizeof(float) * (size_t)width * streams * kcap));
+        CU(w.d_logs.alloc(sizeof(uint2) * (size_t)width * streams * logcap));
+        CU(w.d_counts.alloc(sizeof(int) * (size_t)width * streams));
+        CU(w.d_tlocal.alloc(sizeof(float) * (size_t)width * streams));
         CU(w.d_bounds.alloc(sizeof(long long) * (size_t)(ix->num_sms + 1)));
         CU(w.d_cta_time.alloc(sizeof(unsigned) * (size_t)ix->num_sms));
         if (!old.scanned) CU(old.scanned.create(cudaEventDisableTiming));
@@ -419,12 +464,12 @@ int ensure_workspace(vsb_index *ix, int k) {
         fresh[i].drained = std::move(ix->work[i].drained);
         ix->work[i] = std::move(fresh[i]);
     }
-    ix->ws_kcap = kcap; ix->ws_logcap = logcap; ix->ws_streams = streams;
+    ix->ws_kcap = kcap; ix->ws_logcap = logcap; ix->ws_width = width; ix->ws_streams = streams;
     return VSB_OK;
 }
 
 // the ScanParams of a top-k and a range launch alike: rows [0, n) of vec, whose first row is shard row r0 (the row filter is
-// indexed by shard rows), scanned with plan pl for the query at d_query
+// indexed by shard rows), scanned with plan pl for the query at d_query (the first of a pass's queries)
 ScanParams scan_params(const vsb_index *ix, const Plan &pl, int root, const uint8_t *d_query, const uint8_t *vec, long long n, long long r0) {
     ScanParams p{};
     p.vec = vec;
@@ -435,7 +480,8 @@ ScanParams scan_params(const vsb_index *ix, const Plan &pl, int root, const uint
     p.wtile_bytes = pl.wtile_bytes;
     p.nsw = pl.nsw;
     p.root = root;
-    p.query = d_query;
+    p.nq = 1;
+    p.query[0] = d_query;
     p.allow = ix->flt_d;
     p.allow_base = r0;
     return p;
@@ -452,15 +498,15 @@ unsigned exchange_next_seq(vsb_index *ix, int slot);
 int merge_blocks_strided(const uint8_t *blocks, int world, size_t stride, const int64_t *first_seq, int k, int64_t *out_rowids, double *out_dist);
 int exchange_fill_push(vsb_index *ix, PushParams *pp);
 
-// launches the scan kernel for one query (device pointer, pitch bytes) on ss and, when k > 0, the filter on ix->fstream;
-// slot receives the result.
-// fetch: copy the slot's head to pinned host memory afterwards (false when the heads are all-gathered on the device)
-// ss: the scan stream of this launch (next_scan_stream); push: the head is labelled for the exchange (shard index and
-// exchange sequence number); push_heads_kernel moves it (exchange_push)
+// launches one pass of the scan kernel for nq <= pass_max queries (device pointers queries[j], pitch bytes each) on ss and, when
+// k > 0, one filter per query on ix->fstream; slots[j] receives query j's result.  nq > 1 needs k > 0.
+// fetch: copy each slot's head to pinned host memory afterwards (false when the heads are all-gathered on the device)
+// ss: the scan stream of this launch (next_scan_stream); push: the heads are labelled for the exchange (shard index and
+// exchange sequence number); push_heads_kernel moves them (exchange_push)
 // view_vec / view_n: scan these rows instead of the resident column (the windows of a streamed index)
 // view_r0: the shard row of view_vec's first row (the row filter is indexed by shard rows)
-int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *slot, float *d_dist_all, bool fetch, cudaStream_t ss,
-                bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1, long long view_r0 = 0) {
+int launch_scan(vsb_index *ix, int metric, const uint8_t *const *queries, Slot *const *slots, int nq, int k, float *d_dist_all, bool fetch,
+                cudaStream_t ss, bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1, long long view_r0 = 0) {
     const uint8_t *scan_vec = view_vec ? view_vec : ix->d_vec;
     const long long scan_n = view_vec ? view_n : ix->n;
     if (!scan_vec) return fail(VSB_EINVAL, "this entry point needs a resident (not streamed) index");
@@ -471,16 +517,18 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
     // the scan's list layout, the filter's FAST/generic choice and its shared-memory layout all follow THIS query's k
     const int kcap = k > 0 ? ((k + 31) & ~31) : 0;
     if (kcap > ix->ws_kcap) return fail(VSB_EINVAL, "scan workspace too small for k = %d", k);
-    const Plan pl = make_plan(ix, kcap);
-    ScanFn fn = pick_kernel(ix->vtype, mc, pl.direct);
+    if (nq < 1 || (nq > 1 && (k <= 0 || nq > ix->ws_width || nq > pass_max(ix, kcap))))
+        return fail(VSB_EINVAL, "bad pass of %d queries", nq);
+    const Plan pl = make_plan(ix, kcap, nq);
+    ScanFn fn = pick_kernel(ix->vtype, mc, pl.direct, false, nq);
     if (!fn) return fail(VSB_EINVAL, "unsupported vector type %d", ix->vtype);
     // max-shared carve-out for the scan AND the filter kernel: kernels that want different L1/shared splits cannot share
     // an SM, and the filter blocks of launch i are meant to run beside the scan CTAs of launch i+1
     CU((cudaError_t)set_smem_limit((const void *)fn, pl.smem));
 
-    // the scan runs on its scan stream (ss), the filter (+ result copy) on ix->fstream: while the filters of this launch walk the
-    // k-lists and compact the candidate logs, the scan of the next launch is already streaming the shard (the filter
-    // blocks are small enough to sit on the SMs beside the scan CTAs).  The two workspaces alternate.
+    // the scan runs on its scan stream (ss), the filters (+ result copies) on ix->fstream: while the filters of this launch walk
+    // the k-lists and compact the candidate logs, the scan of the next launch is already streaming the shard (the filter
+    // blocks are small enough to sit on the SMs beside the scan CTAs).  The workspaces rotate.
     Work *wk = nullptr;
     if (k > 0) {
         wk = &ix->work[ix->ws_next];
@@ -498,7 +546,12 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
         CU(cudaMemsetAsync(wk->d_cta_time, 0, sizeof(unsigned) * (size_t)ix->num_sms, ss));
         wk->bounds_tiles = total_tiles;
     }
-    ScanParams p = scan_params(ix, pl, root, d_query, scan_vec, scan_n, view_r0);
+    ScanParams p = scan_params(ix, pl, root, queries[0], scan_vec, scan_n, view_r0);
+    p.nq = nq;
+    for (int j = 0; j < nq; ++j) {
+        p.query[j] = queries[j];
+        p.ctrl[j] = slots[j] ? slots[j]->d_ctrl : nullptr;
+    }
     p.k = k;
     p.kcap = kcap;
     p.logcap = ix->ws_logcap;
@@ -506,7 +559,6 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
     p.tlocal = wk ? wk->d_tlocal.get() : nullptr;
     p.logs = wk ? wk->d_logs.get() : nullptr;
     p.counts = wk ? wk->d_counts.get() : nullptr;
-    p.ctrl = slot ? slot->d_ctrl : nullptr;
     p.dist_all = d_dist_all;
     p.bounds = balance ? wk->d_bounds.get() : nullptr;
     p.cta_time = balance ? wk->d_cta_time.get() : nullptr;
@@ -528,58 +580,69 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *d_query, int k, Slot *
     CU(cudaGetLastError());
     ++g_launches;
     note_plan(ix, pl);
+    if (k > 0) {
+        ix->st_scan_passes++;
+        ix->st_pass_queries += nq;
+        ix->last_kcap = kcap;
+    }
     if (pev) CU(cudaEventRecord(pev[1], ss));
     if (k > 0) {
         CU(cudaEventRecord(wk->scanned, ss));
         CU(cudaStreamWaitEvent(ix->fstream, wk->scanned, 0));
-        FilterParams f{};
+        PushParams pp{};
         if (push) {
-            PushParams pp{};
             const int rc = exchange_fill_push(ix, &pp);
             if (rc) return rc;
-            f.src = pp.src;
         }
-        f.S = ix->ws_streams;
-        f.k = k;
-        f.kcap = kcap;
-        f.logcap = ix->ws_logcap;
-        f.headcap = kFirstFetch;
-        f.outcap = kOutCap;
-        const bool fast = (kcap == 32) && filter_fast_smem(f.S / kWarps) + 2048 <= (size_t)ix->max_smem;
+        const int S = ix->ws_streams;
+        const bool fast = (kcap == 32) && filter_fast_smem(S / kWarps) + 2048 <= (size_t)ix->max_smem;
         const int fw = filter_warps(fast);
-        const int nblocks = (f.S + fw - 1) / fw;
+        const int nblocks = (S + fw - 1) / fw;
         if (nblocks > kTableCap) return fail(VSB_ERANGE, "too many filter blocks (%d)", nblocks);
-        f.lists = wk->d_lists;
-        f.tlocal = wk->d_tlocal;
-        f.logs = wk->d_logs;
-        f.counts = wk->d_counts;
-        f.out = head_survivors(slot->d_head);
-        f.out_tail = slot->d_tail;
-        f.table = head_table(slot->d_head);
-        f.hdr = slot->d_head;
-        f.ctrl = slot->d_ctrl;
-        f.seqno = ++slot->seq;
-        f.xseq = push ? exchange_next_seq(ix, (int)(slot - ix->slot)) : 0u;
-        f.bounds = balance ? wk->d_bounds.get() : nullptr;
-        f.cta_time = wk->d_cta_time;
-        f.total_tiles = total_tiles;
         if (pev) CU(cudaEventRecord(pev[2], ix->fstream));
-        if (fast) {
-            const size_t fsm = filter_fast_smem(f.S / kWarps);
-            CU((cudaError_t)set_smem_limit((const void *)filter_kernel<true>, fsm));
-            filter_kernel<true><<<nblocks, fw * 32, fsm, ix->fstream>>>(f);
-        } else {
-            const size_t fsm = sizeof(float) * ((size_t)2 * kFilterWarps * kcap + (size_t)f.S + 32);
-            CU((cudaError_t)set_smem_limit((const void *)filter_kernel<false>, fsm));
-            filter_kernel<false><<<nblocks, fw * 32, fsm, ix->fstream>>>(f);
+        for (int j = 0; j < nq; ++j) {
+            Slot *slot = slots[j];
+            FilterParams f{};
+            f.src = pp.src;
+            f.S = S;
+            f.k = k;
+            f.kcap = kcap;
+            f.logcap = ix->ws_logcap;
+            f.headcap = kFirstFetch;
+            f.outcap = kOutCap;
+            f.lists = wk->d_lists + pass_lists(j, S, kcap);
+            f.tlocal = wk->d_tlocal + pass_streams(j, S);
+            f.logs = wk->d_logs + pass_logs(j, S, ix->ws_logcap);
+            f.counts = wk->d_counts + pass_streams(j, S);
+            f.out = head_survivors(slot->d_head);
+            f.out_tail = slot->d_tail;
+            f.table = head_table(slot->d_head);
+            f.hdr = slot->d_head;
+            f.ctrl = slot->d_ctrl;
+            f.seqno = ++slot->seq;
+            f.xseq = push ? exchange_next_seq(ix, (int)(slot - ix->slot)) : 0u;
+            f.bounds = (balance && j == 0) ? wk->d_bounds.get() : nullptr;   // the partition follows the CTA times once per pass
+            f.cta_time = wk->d_cta_time;
+            f.total_tiles = total_tiles;
+            if (fast) {
+                const size_t fsm = filter_fast_smem(S / kWarps);
+                CU((cudaError_t)set_smem_limit((const void *)filter_kernel<true>, fsm));
+                filter_kernel<true><<<nblocks, fw * 32, fsm, ix->fstream>>>(f);
+            } else {
+                const size_t fsm = sizeof(float) * ((size_t)2 * kFilterWarps * kcap + (size_t)S + 32);
+                CU((cudaError_t)set_smem_limit((const void *)filter_kernel<false>, fsm));
+                filter_kernel<false><<<nblocks, fw * 32, fsm, ix->fstream>>>(f);
+            }
+            CU(cudaGetLastError());
+            ++g_launches;
+            if (j == nq - 1) {                       // the pass's filters are the last readers of the workspace
+                if (pev) CU(cudaEventRecord(pev[3], ix->fstream));
+                CU(cudaEventRecord(wk->drained, ix->fstream));
+                wk->in_use = true;
+            }
+            if (fetch) CU(cudaMemcpyAsync(slot->h_head, slot->d_head, kHeadBytes, cudaMemcpyDeviceToHost, ix->fstream));
+            CU(cudaEventRecord(slot->done, ix->fstream));
         }
-        CU(cudaGetLastError());
-        ++g_launches;
-        if (pev) CU(cudaEventRecord(pev[3], ix->fstream));
-        CU(cudaEventRecord(wk->drained, ix->fstream));
-        wk->in_use = true;
-        if (fetch) CU(cudaMemcpyAsync(slot->h_head, slot->d_head, kHeadBytes, cudaMemcpyDeviceToHost, ix->fstream));
-        CU(cudaEventRecord(slot->done, ix->fstream));
     }
     return VSB_OK;
 }
@@ -817,7 +880,8 @@ int scan_all_into(vsb_index *ix, int metric, const uint8_t *d_query, std::vector
     dist.resize((size_t)ix->n);
     return for_each_view(ix, 2,
         [&](const View &v) {
-            return launch_scan(ix, metric, d_query, 0, nullptr, ix->d_dist_all + (size_t)v.buf * ix->win_rows, false, ix->stream, false, v.vec, v.rows, v.r0);
+            Slot *none = nullptr;
+            return launch_scan(ix, metric, &d_query, &none, 1, 0, ix->d_dist_all + (size_t)v.buf * ix->win_rows, false, ix->stream, false, v.vec, v.rows, v.r0);
         },
         [&](const View &v) {
             CU(cudaMemcpyAsync(dist.data() + v.r0, ix->d_dist_all + (size_t)v.buf * ix->win_rows, sizeof(float) * (size_t)v.rows, cudaMemcpyDeviceToHost, ix->stream));
@@ -904,7 +968,9 @@ void rows_of_rowids(vsb_index *ix, const int64_t *rowids, int64_t n, Mark mark) 
 // the query is parked in the last one)
 int stage_host_query(vsb_index *ix, const void *query, Slot **slot) {
     CU(cudaSetDevice(ix->device));
-    const int rc = ensure_slots(ix);
+    int rc = flush_held(ix);                       // a held query may sit in this slot
+    if (rc) return rc;
+    rc = ensure_slots(ix);
     if (rc) return rc;
     *slot = &ix->slot[ix->streamed ? kSlots - 1 : 0];
     return stage_query(ix, *slot, query, ix->stream);
@@ -926,7 +992,11 @@ int query_candidates(vsb_index *ix, int metric, const void *query, int k, std::v
     if (rc) return rc;
     // every view's survivors in scan order, rows made column-global; a streamed index rotates result slots 0..3 over its windows
     rc = for_each_view(ix, ix->streamed ? 4 : 1,
-        [&](const View &v) { return launch_scan(ix, metric, slot->d_query, k, &ix->slot[v.slot], nullptr, true, ix->stream, false, v.vec, v.rows, v.r0); },
+        [&](const View &v) {
+            const uint8_t *q = slot->d_query;
+            Slot *vs = &ix->slot[v.slot];
+            return launch_scan(ix, metric, &q, &vs, 1, k, nullptr, true, ix->stream, false, v.vec, v.rows, v.r0);
+        },
         [&](const View &v) {
             bool ovf = false;
             const int r = visit_survivors(ix, &ix->slot[v.slot], &ovf, [&](uint2 c) { cands.push_back(make_uint2(c.x, c.y + (uint32_t)v.r0)); });
@@ -937,36 +1007,61 @@ int query_candidates(vsb_index *ix, int metric, const void *query, int k, std::v
     return overflow ? all_candidates(ix, metric, slot->d_query, cands) : VSB_OK;
 }
 
-int check_index(const vsb_index *ix) {
-    if (!ix) return fail(VSB_EINVAL, "null index");
-    return VSB_OK;
+// launches the held pass (vsb_scan_submit), if any
+int flush_held(vsb_index *ix) {
+    if (ix->held.nq == 0) return VSB_OK;
+    const HeldPass h = ix->held;
+    ix->held.nq = 0;
+    CU(cudaSetDevice(ix->device));
+    Slot *slots[kMaxPass];
+    for (int j = 0; j < h.nq; ++j) slots[j] = &ix->slot[h.slot[j]];
+    const int rc = ensure_workspace(ix, h.k, h.nq);
+    return rc ? rc : launch_scan(ix, h.metric, h.query, slots, h.nq, h.k, nullptr, true, h.ss);
 }
 
-// one scan + filter launch per query of a group of independent queries (query j at queries + j * query_stride; slots
+// every entry point on an index but vsb_scan_submit and vsb_collect: launches the held pass first, so that no other call
+// waits behind a query the caller has already submitted
+int check_index(vsb_index *ix) {
+    if (!ix) return fail(VSB_EINVAL, "null index");
+    return flush_held(ix);
+}
+
+bool scan_args_ok(const void *queries, int k) {
+    return queries != nullptr && k > 0 && k <= kMaxK;
+}
+
+// one pass of the column per pass_max queries of a group of independent queries (query j at queries + j * query_stride; slots
 // first_slot ..).  push: the heads are labelled for the exchange targets (peer memory), see exchange.inc
 int submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device, int k, int fetch,
                  int first_slot, bool push) {
     if (check_index(ix)) return VSB_EINVAL;
-    if (!queries || k <= 0 || k > kMaxK) return fail(VSB_EINVAL, "bad scan arguments (k must be 1..%d)", kMaxK);
+    if (!scan_args_ok(queries, k)) return fail(VSB_EINVAL, "bad scan arguments (k must be 1..%d)", kMaxK);
     if (nq <= 0 || first_slot < 0 || first_slot + nq > kSlots) return fail(VSB_EINVAL, "bad slot group [%d, %d)", first_slot, first_slot + nq);
     CU(cudaSetDevice(ix->device));
     int rc = ensure_slots(ix);
     if (rc) return rc;
-    rc = ensure_workspace(ix, k);
+    const int width = std::min(nq, pass_max(ix, (k + 31) & ~31));
+    rc = ensure_workspace(ix, k, width);
     if (rc) return rc;
-    for (int j = 0; j < nq; ++j) {
-        Slot *slot = &ix->slot[first_slot + j];
-        const uint8_t *q = (const uint8_t *)queries + (size_t)j * (size_t)query_stride;
+    for (int j0 = 0; j0 < nq; j0 += width) {
+        const int m = std::min(width, nq - j0);
         cudaStream_t ss = next_scan_stream(ix);
-        if (!query_on_device) {
-            if (slot->seq > 0) CU(cudaEventSynchronize(slot->done));   // the slot's pinned staging buffer is free again
-            rc = stage_query(ix, slot, q, ss);
-            if (rc) return rc;
-            q = slot->d_query;
+        const uint8_t *q[kMaxPass];
+        Slot *slots[kMaxPass];
+        for (int j = 0; j < m; ++j) {
+            Slot *slot = slots[j] = &ix->slot[first_slot + j0 + j];
+            ix->uncollected &= ~(1u << (first_slot + j0 + j));     // a query left in this slot is given up
+            q[j] = (const uint8_t *)queries + (size_t)(j0 + j) * (size_t)query_stride;
+            if (!query_on_device) {
+                if (slot->seq > 0) CU(cudaEventSynchronize(slot->done));   // the slot's pinned staging buffer is free again
+                rc = stage_query(ix, slot, q[j], ss);
+                if (rc) return rc;
+                q[j] = slot->d_query;
+            }
         }
-        rc = launch_scan(ix, metric, q, k, slot, nullptr, fetch != 0, ss, push);
+        rc = launch_scan(ix, metric, q, slots, m, k, nullptr, fetch != 0, ss, push);
         if (rc) return rc;
-        ix->last_slot = first_slot + j;
+        ix->last_slot = first_slot + j0 + m - 1;
         ix->last_metric = metric;
     }
     return VSB_OK;
@@ -1214,7 +1309,8 @@ int large_k_candidates(vsb_index *ix, int metric, const uint8_t *d_query, int k,
         return for_each_view(ix, 2,
             [&](const View &v) {
                 float *dist = ix->d_dist_all + (size_t)v.buf * ix->win_rows;
-                const int r = launch_scan(ix, metric, d_query, 0, nullptr, dist, false, ix->stream, false, v.vec, v.rows, v.r0);
+                Slot *none = nullptr;
+                const int r = launch_scan(ix, metric, &d_query, &none, 1, 0, dist, false, ix->stream, false, v.vec, v.rows, v.r0);
                 return r ? r : large_k_view(ix, dist, v.rows, v.r0, k);
             },
             no_visit);
@@ -1508,6 +1604,9 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "filter_blocks")) return (ix->num_sms * kWarps + kFilterWarpsFast - 1) / kFilterWarpsFast;
     if (!strcmp(name, "sms")) return ix->num_sms;
     if (!strcmp(name, "plan_log2p")) return ix->last_log2p;
+    if (!strcmp(name, "plan_pass_max")) return pass_max(ix, ix->last_kcap > 0 ? ix->last_kcap : 32);   // for the k of the last top-k pass
+    if (!strcmp(name, "scan_passes")) return ix->st_scan_passes;
+    if (!strcmp(name, "pass_queries")) return ix->st_pass_queries;
     if (!strcmp(name, "plan_nsw")) return ix->last_nsw;
     if (!strcmp(name, "plan_direct")) return ix->last_direct;
     if (!strcmp(name, "range_pairs")) return ix->st_range_pairs;
@@ -1706,12 +1805,52 @@ int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double 
     return VSB_OK;
 }
 
+// The hold rule (DESIGN §3.2): while the caller has an uncollected query on this index, a new submission waits to share a pass
+// with the next ones; the held pass is launched when it is full, when one of its queries is collected, when a submission with
+// another metric or k (or for one of its slots) arrives, and by any other call on the index (check_index).  A submission with
+// nothing outstanding launches at once.  fetch == 0 submissions are read on the device, where their collection cannot be seen:
+// they launch at once and never count as outstanding.
 int vsb_scan_submit(vsb_index *ix, int metric, const void *query, int query_on_device, int k, int fetch, int want_slot) {
-    if (check_index(ix)) return VSB_EINVAL;
+    if (!ix) return fail(VSB_EINVAL, "null index");
     if (want_slot >= kSlots) return fail(VSB_EINVAL, "slot %d out of range (have %d)", want_slot, kSlots);
     const int si = want_slot >= 0 ? want_slot : (ix->last_slot + 1) % kSlots;
-    const int rc = submit_group(ix, metric, query, 0, 1, query_on_device, k, fetch, si, false);
-    return rc ? rc : si;   // slot id (>= 0) for vsb_collect / vsb_result_block
+    HeldPass &h = ix->held;
+    bool in_pass = false;
+    for (int j = 0; j < h.nq; ++j) in_pass |= h.slot[j] == si;
+    int rc = VSB_OK;
+    if (h.nq > 0 && (in_pass || h.metric != metric || h.k != k)) rc = flush_held(ix);
+    if (rc) return rc;
+    ix->uncollected &= ~(1u << si);                 // a query left uncollected in this slot is given up
+    if (fetch == 0 || ix->uncollected == 0) {
+        rc = submit_group(ix, metric, query, 0, 1, query_on_device, k, fetch, si, false);
+    } else {
+        if (!scan_args_ok(query, k)) return fail(VSB_EINVAL, "bad scan arguments (k must be 1..%d)", kMaxK);
+        CU(cudaSetDevice(ix->device));
+        rc = ensure_slots(ix);
+        if (rc) return rc;
+        if (h.nq == 0) {
+            h.metric = metric;
+            h.k = k;
+            h.ss = next_scan_stream(ix);
+        }
+        Slot *slot = &ix->slot[si];
+        const uint8_t *q = (const uint8_t *)query;
+        if (!query_on_device) {
+            if (slot->seq > 0) CU(cudaEventSynchronize(slot->done));   // the slot's pinned staging buffer is free again
+            rc = stage_query(ix, slot, q, h.ss);
+            if (rc) return rc;
+            q = slot->d_query;
+        }
+        h.query[h.nq] = q;
+        h.slot[h.nq] = si;
+        ++h.nq;
+        ix->last_slot = si;
+        ix->last_metric = metric;
+        if (h.nq >= pass_max(ix, (k + 31) & ~31)) rc = flush_held(ix);
+    }
+    if (rc) return rc;
+    if (fetch != 0) ix->uncollected |= 1u << si;
+    return si;   // slot id (>= 0) for vsb_collect / vsb_result_block
 }
 
 int vsb_scan_submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device, int k,
@@ -1798,8 +1937,14 @@ int vsb_collect_last(vsb_index *ix, int k, int64_t *out_rowids, double *out_dist
 }
 
 int vsb_collect(vsb_index *ix, int slot_id, int k, int64_t *out_rowids, double *out_dist, int *out_count) {
-    if (check_index(ix)) return VSB_EINVAL;
+    if (!ix) return fail(VSB_EINVAL, "null index");
     if (slot_id < 0 || slot_id >= kSlots || !ix->slots_ready) return fail(VSB_EINVAL, "bad slot");
+    for (int j = 0; j < ix->held.nq; ++j)            // collecting a held query launches its pass; collecting another does not
+        if (ix->held.slot[j] == slot_id) {
+            const int rc = flush_held(ix);
+            if (rc) return rc;
+        }
+    ix->uncollected &= ~(1u << slot_id);
     CU(cudaSetDevice(ix->device));
     bool overflow = false;
     const int cnt = slots_replay(k, nullptr, out_dist, out_rowids, [&](SlotState &s) {   // waits for this query only; a later launch may still run

@@ -34,7 +34,11 @@ enum { T_F32 = 1, T_F16 = 2, T_BF16 = 3, T_U8 = 4, T_I8 = 5 };
 enum { MC_L2 = 0, MC_COS = 1, MC_DOT = 2, MC_L1 = 3 };  // L2 and SQUARED_L2 share a kernel (root flag)
 
 constexpr int kMaxGroup = 8;          // queries of one exchange group (vsb_exchange_submit): heads waited for and pushed together
+constexpr int kMaxPass = 8;           // queries scored in one pass of the column (scan_pass_kernel's widest compile-time width)
 
+// One scan launch is a pass: it reads every row of the column once and scores it against nq <= M queries.  Query j
+// has its own k-lists, logs, counts and in-CTA bounds at j times the per-query stride of each workspace array (pass_lists
+// and friends), and its own overflow flag ctrl[j][1].
 struct ScanParams {
     const uint8_t *vec;   // [n][pitch]
     long long n;
@@ -47,13 +51,14 @@ struct ScanParams {
     int k;                // 0 => no top-k (dist_all only)
     int kcap;             // k rounded up to 32
     int logcap;
-    const uint8_t *query; // device, pitch bytes, zero padded
+    int nq;               // queries of the pass (1 .. the kernel's M)
+    const uint8_t *query[kMaxPass]; // device, pitch bytes each, zero padded
     float *lists;         // k <= 32: [CTAs][32] the k smallest distances of each CTA's rows, sorted ascending, +INF padded;
                           // k > 32:  [streams][kcap] k smallest distances of each stream (unsorted)
     float *tlocal;        // k <= 32: [streams] k-th smallest distance over the EARLIER streams of the same CTA (+INF if < k rows)
     uint2 *logs;          // [streams][logcap] (dist bits, local row)
     int *counts;          // [streams] log entries written (may exceed logcap => overflow)
-    int *ctrl;            // ctrl[1] = overflow flag
+    int *ctrl[kMaxPass];  // ctrl[j][1] = overflow flag of query j
     float *dist_all;      // optional [n]
     // adaptive row partition (optional): bounds[c] .. bounds[c+1] are the warp-tiles of CTA c (contiguous, ascending, any
     // sizes: the exactness argument only needs streams to be contiguous row ranges in scan order).  Each CTA reports the
@@ -74,6 +79,11 @@ struct ScanParams {
     long long range_cap;
     unsigned range_row_base;   // shard row of vec's first row, added to the rows written (the windows of a streamed index)
 };
+
+// query j's part of the pass workspaces (streams = scan CTAs x kWarps; the filter of query j gets the same offsets)
+__host__ __device__ inline size_t pass_lists(int j, long long streams, int kcap) { return (size_t)j * streams * kcap; }
+__host__ __device__ inline size_t pass_logs(int j, long long streams, int logcap) { return (size_t)j * streams * logcap; }
+__host__ __device__ inline size_t pass_streams(int j, long long streams) { return (size_t)j * streams; }
 
 // bit `row` of a row bitmap (bit row & 31 of word row >> 5); nullptr: every row is eligible
 __device__ __forceinline__ bool row_allowed(const uint32_t *allow, long long row) {
@@ -155,8 +165,9 @@ __device__ __forceinline__ void unpack8(const uint4 v, float (&o)[8]) {
     }
 }
 
-// one 16-byte chunk of the row (r) against the same chunk of the query (q)
-template <int VT, int MC>
+// one 16-byte chunk of the row (r) against the same chunk of the query (q).  NORM = false leaves out the row's own terms (its
+// norm, A.ib / A.ny), which a pass accumulates once for all its queries
+template <int VT, int MC, bool NORM = true>
 __device__ __forceinline__ void accum16(Accum &A, const uint4 r, const uint4 q) {
     if constexpr (VT == T_U8 || VT == T_I8) {
         const uint32_t rw[4] = {r.x, r.y, r.z, r.w}, qw[4] = {q.x, q.y, q.z, q.w};
@@ -169,10 +180,10 @@ __device__ __forceinline__ void accum16(Accum &A, const uint4 r, const uint4 q) 
             } else {
                 if constexpr (VT == T_U8) {
                     A.ia = (int)__dp4a(rw[j], qw[j], (uint32_t)A.ia);
-                    if constexpr (MC != MC_DOT) A.ib = (int)__dp4a(rw[j], rw[j], (uint32_t)A.ib);
+                    if constexpr (MC != MC_DOT && NORM) A.ib = (int)__dp4a(rw[j], rw[j], (uint32_t)A.ib);
                 } else {
                     A.ia = __dp4a((int)rw[j], (int)qw[j], A.ia);
-                    if constexpr (MC != MC_DOT) A.ib = __dp4a((int)rw[j], (int)rw[j], A.ib);
+                    if constexpr (MC != MC_DOT && NORM) A.ib = __dp4a((int)rw[j], (int)rw[j], A.ib);
                 }
             }
         }
@@ -197,10 +208,21 @@ __device__ __forceinline__ void accum16(Accum &A, const uint4 r, const uint4 q) 
                 s = fmaf(x[j], y[j], s);
             } else {  // cosine
                 s = fmaf(x[j], y[j], s);
-                A.ny = fmaf(y[j], y[j], A.ny);
+                if constexpr (NORM) A.ny = fmaf(y[j], y[j], A.ny);
             }
         }
     }
+}
+
+// one 16-byte chunk of the row against the same chunk of each of the pass's nq queries (query m's chunk at q + m * qstride).
+// The row's norm goes to A[0] only; every accumulator sees its terms in the order of a lone query, so each query's distance
+// is bit for bit the one a pass of its own computes.
+template <int VT, int MC, int M>
+__device__ __forceinline__ void accum16_pass(Accum (&A)[M], const uint4 r, const uint8_t *q, int qstride, int nq) {
+    accum16<VT, MC>(A[0], r, *reinterpret_cast<const uint4 *>(q));
+#pragma unroll
+    for (int m = 1; m < M; ++m)
+        if (m < nq) accum16<VT, MC, false>(A[m], r, *reinterpret_cast<const uint4 *>(q + (size_t)m * qstride));
 }
 
 struct QueryNorm {
@@ -349,13 +371,14 @@ __device__ __noinline__ float special_row_distance(const uint8_t *row, const uin
     return special_row_distance_body<VT, MC>(row, query, nelem, root);
 }
 
+template <bool NORM = true>
 __device__ __forceinline__ void accum_reduce(Accum &A, int P) {
     for (int off = P >> 1; off >= 1; off >>= 1) {
         A.s0 += __shfl_xor_sync(0xFFFFFFFFu, A.s0, off);
         A.s1 += __shfl_xor_sync(0xFFFFFFFFu, A.s1, off);
-        A.ny += __shfl_xor_sync(0xFFFFFFFFu, A.ny, off);
+        if constexpr (NORM) A.ny += __shfl_xor_sync(0xFFFFFFFFu, A.ny, off);
         A.ia += __shfl_xor_sync(0xFFFFFFFFu, A.ia, off);
-        A.ib += __shfl_xor_sync(0xFFFFFFFFu, A.ib, off);
+        if constexpr (NORM) A.ib += __shfl_xor_sync(0xFFFFFFFFu, A.ib, off);
     }
 }
 
@@ -440,32 +463,40 @@ struct SortedList {
 };
 
 // ------------------------------------------------------------------ the scan kernel
-// One launch scans the shard for one query: scan_kernel (top-k, all distances) and scan_range_kernel (range search) share this
-// body.  RANGE: the fixed threshold prm.range_t instead of the k-lists, hits appended to prm.range_pairs (no log, no lists, no
+// One launch is one pass over the shard: scan_kernel (one query: top-k, all distances), scan_pass_kernel (top-k for nq <= M
+// queries scored against every staged row) and scan_range_kernel (range search, one query) share this body.  Each query keeps its own running k-th value, k-list, log and counts; the streams are the same contiguous
+// row ranges for every query, so the exactness argument of a lone query (DESIGN §3.1) holds for each one unchanged.
+// RANGE: the fixed threshold prm.range_t instead of the k-lists, hits appended to prm.range_pairs (no log, no lists, no
 // filter_kernel afterwards).
-template <int VT, int MC, bool DIRECT, bool RANGE>
+template <int VT, int MC, bool DIRECT, bool RANGE, int M>
 __device__ __forceinline__ void scan_body(const ScanParams &prm) {
+    static_assert(M >= 1 && M <= kMaxPass && (!RANGE || M == 1), "range search scans one query per pass");
     extern __shared__ __align__(1024) uint8_t smem[];
+    const int nq = (M == 1) ? 1 : prm.nq;
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem);                    // [kWarps][kMaxStages]
-    uint8_t *qs = smem + kBarrierBytes;                                      // [pitch] the query
-    float *lists_s = reinterpret_cast<float *>(qs + prm.pitch);              // [kWarps][kcap]
-    uint8_t *ring = qs + ((prm.pitch + kWarps * prm.kcap * 4 + 127) & ~127); // [kWarps][nsw][wtile_bytes]
+    uint8_t *qs = smem + kBarrierBytes;                                      // [nq][pitch] the queries
+    float *lists_s = reinterpret_cast<float *>(qs + nq * prm.pitch);         // [kWarps][nq][kcap]
+    uint8_t *ring = qs + ((nq * (prm.pitch + kWarps * prm.kcap * 4) + 127) & ~127); // [kWarps][nsw][wtile_bytes]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int P = 1 << prm.log2P, rpw = 32 >> prm.log2P;
     const int nsw = prm.nsw;
     const long long clk0 = clock64();
 
-    // ---- prologue: barriers, query
+    // ---- prologue: barriers, queries
     if (tid == 0) {
         for (int i = 0; i < kWarps * kMaxStages; ++i) mbar_init(&bars[i], 1);
         fence_barrier_init();
     }
-    for (int i = tid; i < prm.nc; i += kThreads)
-        reinterpret_cast<uint4 *>(qs)[i] = reinterpret_cast<const uint4 *>(prm.query)[i];
+#pragma unroll
+    for (int m = 0; m < M; ++m)
+        if (m < nq)
+            for (int i = tid; i < prm.nc; i += kThreads)
+                reinterpret_cast<uint4 *>(qs + m * prm.pitch)[i] = reinterpret_cast<const uint4 *>(prm.query[m])[i];
     __syncthreads();
 
     // ---- this warp's stream: a contiguous range of warp-tiles (rpw rows each)
+    const long long S = (long long)gridDim.x * kWarps;
     const long long sidx = (long long)blockIdx.x * kWarps + warp;
     const long long T = (prm.n + rpw - 1) / rpw;
     long long c0, c1;                                                        // this CTA's warp-tiles
@@ -504,15 +535,15 @@ __device__ __forceinline__ void scan_body(const ScanParams &prm) {
     const uint8_t *fix_row = nullptr;
     int fix_stage = 0;
 
-    float *mylist = lists_s + (size_t)warp * prm.kcap;
-
-    // query norm (every warp computes it the same way: lane-strided chunks, butterfly sum)
-    QueryNorm qn;
-    {
+    // query norms (every warp computes them the same way: lane-strided chunks, butterfly sum)
+    QueryNorm qn[M];
+#pragma unroll
+    for (int m = 0; m < M; ++m) {
         float f = 0.0f;
         int iq = 0;
-        for (int c = lane; c < prm.nc; c += 32) {
-            const uint4 q = reinterpret_cast<const uint4 *>(qs)[c];
+        const uint8_t *qm = qs + m * prm.pitch;
+        for (int c = lane; c < prm.nc && m < nq; c += 32) {
+            const uint4 q = reinterpret_cast<const uint4 *>(qm)[c];
             if constexpr (VT == T_U8) {
                 iq = (int)__dp4a(q.x, q.x, (uint32_t)iq); iq = (int)__dp4a(q.y, q.y, (uint32_t)iq);
                 iq = (int)__dp4a(q.z, q.z, (uint32_t)iq); iq = (int)__dp4a(q.w, q.w, (uint32_t)iq);
@@ -531,19 +562,26 @@ __device__ __forceinline__ void scan_body(const ScanParams &prm) {
             f += __shfl_xor_sync(0xFFFFFFFFu, f, off);
             iq += __shfl_xor_sync(0xFFFFFFFFu, iq, off);
         }
-        qn.f = f; qn.i = iq;
+        qn[m].f = f; qn[m].i = iq;
     }
-    for (int j = lane; j < prm.kcap; j += 32) mylist[j] = (j < prm.k) ? INFINITY : -INFINITY;
+    // query m's k-list of this warp, its log
+    auto mylist = [&](int m) { return lists_s + ((size_t)warp * nq + m) * prm.kcap; };
+    for (int m = 0; m < nq; ++m)
+        for (int j = lane; j < prm.kcap; j += 32) mylist(m)[j] = (j < prm.k) ? INFINITY : -INFINITY;
     __syncwarp();
 
-    float thr = INFINITY;
-    int pos = 0, logged = 0;
+    float thr[M];
+    int pos[M], logged[M];
+#pragma unroll
+    for (int m = 0; m < M; ++m) { thr[m] = INFINITY; pos[m] = 0; logged[m] = 0; }
     uint2 *mylog = prm.logs + (size_t)sidx * prm.logcap;
 
     for (int it = 0; it < ntiles; ++it) {
         const long long row0 = (t0 + it) * rpw;
         const bool valid = (row0 + r) < prm.n;
-        Accum A = {0.f, 0.f, 0.f, 0, 0};
+        Accum A[M];
+#pragma unroll
+        for (int m = 0; m < M; ++m) A[m] = {0.f, 0.f, 0.f, 0, 0};
         if constexpr (!DIRECT) {
             const int s = stage;
             mbar_wait(&mybars[s], parity);
@@ -556,8 +594,7 @@ __device__ __forceinline__ void scan_body(const ScanParams &prm) {
                     if (ii >= cnt) ii -= cnt;
                     const int c = p + (ii << prm.log2P);
                     const uint4 rv = *reinterpret_cast<const uint4 *>(rowp + (size_t)c * 16);
-                    const uint4 qv = *reinterpret_cast<const uint4 *>(qs + (size_t)c * 16);
-                    accum16<VT, MC>(A, rv, qv);
+                    accum16_pass<VT, MC, M>(A, rv, qs + (size_t)c * 16, prm.pitch, nq);
                 }
             }
             __syncwarp();
@@ -574,17 +611,30 @@ __device__ __forceinline__ void scan_body(const ScanParams &prm) {
                 for (int i = 0; i < cnt; ++i) {
                     const int c = p + (i << prm.log2P);
                     const uint4 rv = ldg_stream(reinterpret_cast<const uint4 *>(rowp) + c);
-                    const uint4 qv = *reinterpret_cast<const uint4 *>(qs + (size_t)c * 16);
-                    accum16<VT, MC>(A, rv, qv);
+                    accum16_pass<VT, MC, M>(A, rv, qs + (size_t)c * 16, prm.pitch, nq);
                 }
             }
         }
-        accum_reduce(A, P);
-        float d = finalize<VT, MC>(A, qn, prm.root);
+        accum_reduce(A[0], P);
+        float d[M];
+#pragma unroll
+        for (int m = 0; m < M; ++m) {
+            if (m >= nq) break;
+            if (m > 0) {
+                accum_reduce<false>(A[m], P);
+                A[m].ny = A[0].ny;
+                A[m].ib = A[0].ib;
+            }
+            d[m] = finalize<VT, MC>(A[m], qn[m], prm.root);
+        }
         if constexpr (kFix16) {
-            if (valid && p == 0 && row_needs_exact<VT, MC>(A, qn)) {
-                if constexpr (DIRECT) fix_row = prm.vec + (size_t)(row0 + r) * prm.pitch;
-                d = special_row_distance<VT, MC>(fix_row, qs, prm.pitch / 2, prm.root);
+#pragma unroll
+            for (int m = 0; m < M; ++m) {
+                if (m >= nq) break;
+                if (valid && p == 0 && row_needs_exact<VT, MC>(A[m], qn[m])) {
+                    if constexpr (DIRECT) fix_row = prm.vec + (size_t)(row0 + r) * prm.pitch;
+                    d[m] = special_row_distance<VT, MC>(fix_row, qs + m * prm.pitch, prm.pitch / 2, prm.root);
+                }
             }
             if constexpr (!DIRECT) {
                 __syncwarp();
@@ -593,74 +643,87 @@ __device__ __forceinline__ void scan_body(const ScanParams &prm) {
         }
         if constexpr (RANGE) {
             // one reservation per ballot; hit lanes write at their rank among the hits (slots are ordered later, range_sort_kernel)
-            const bool hit = valid && p == 0 && d < prm.range_t && row_allowed(prm.allow, prm.allow_base + row0 + r);
-            const unsigned m = __ballot_sync(0xFFFFFFFFu, hit);
-            if (m != 0u) {
+            const bool hit = valid && p == 0 && d[0] < prm.range_t && row_allowed(prm.allow, prm.allow_base + row0 + r);
+            const unsigned msk = __ballot_sync(0xFFFFFFFFu, hit);
+            if (msk != 0u) {
                 unsigned base = 0;
-                if (lane == 0) base = atomicAdd(prm.range_count, (unsigned)__popc(m));
+                if (lane == 0) base = atomicAdd(prm.range_count, (unsigned)__popc(msk));
                 base = __shfl_sync(0xFFFFFFFFu, base, 0);
-                const unsigned at = base + (unsigned)__popc(m & ((1u << lane) - 1u));
+                const unsigned at = base + (unsigned)__popc(msk & ((1u << lane) - 1u));
                 if (hit && (long long)at < prm.range_cap)
-                    prm.range_pairs[at] = make_uint2(prm.range_row_base + (unsigned)(row0 + r), __float_as_uint(d));
+                    prm.range_pairs[at] = make_uint2(prm.range_row_base + (unsigned)(row0 + r), __float_as_uint(d[0]));
             }
             continue;
         }
-        if (prm.dist_all != nullptr && valid && p == 0) prm.dist_all[row0 + r] = d;
+        if (prm.dist_all != nullptr && valid && p == 0) prm.dist_all[row0 + r] = d[0];
         if (topk) {
-            // rows are visited in scan order (lane order); strict '<' like the reference (:2102, :2145)
-            unsigned m = __ballot_sync(0xFFFFFFFFu, valid && p == 0 && d < thr && row_allowed(prm.allow, prm.allow_base + row0 + r));
-            while (m) {
-                const int src = __ffs(m) - 1;
-                m &= m - 1;
-                const float dv = __shfl_sync(0xFFFFFFFFu, d, src);
-                if (dv < thr) {
-                    if (lane == 0) {
-                        if (logged < prm.logcap) mylog[logged] = make_uint2(__float_as_uint(dv), (uint32_t)(row0 + (src >> prm.log2P)));
-                        mylist[pos] = dv;
+#pragma unroll
+            for (int m = 0; m < M; ++m) {
+                if (m >= nq) break;
+                // rows are visited in scan order (lane order); strict '<' like the reference (:2102, :2145)
+                unsigned msk = __ballot_sync(0xFFFFFFFFu, valid && p == 0 && d[m] < thr[m] && row_allowed(prm.allow, prm.allow_base + row0 + r));
+                while (msk) {
+                    const int src = __ffs(msk) - 1;
+                    msk &= msk - 1;
+                    const float dv = __shfl_sync(0xFFFFFFFFu, d[m], src);
+                    if (dv < thr[m]) {
+                        if (lane == 0) {
+                            if (logged[m] < prm.logcap)
+                                mylog[pass_logs(m, S, prm.logcap) + logged[m]] = make_uint2(__float_as_uint(dv), (uint32_t)(row0 + (src >> prm.log2P)));
+                            mylist(m)[pos[m]] = dv;
+                        }
+                        ++logged[m];
+                        __syncwarp();
+                        list_argmax(mylist(m), prm.kcap, lane, thr[m], pos[m]);
                     }
-                    ++logged;
-                    __syncwarp();
-                    list_argmax(mylist, prm.kcap, lane, thr, pos);
                 }
             }
         }
     }
     if (topk) {
         __syncwarp();
-        if (lane == 0) {
-            prm.counts[sidx] = logged;
-            if (logged > prm.logcap) atomicExch(&prm.ctrl[1], 1);
-        }
-        if (prm.kcap == 32) {
-            // k <= 32: the CTA's 8 streams are consecutive in scan order.  Sort each stream's list, then one warp merges
-            // them in stream order, recording the running k-th value BEFORE each stream (its in-CTA prefix bound), and
-            // publishes ONE sorted list per CTA: filter_kernel then walks one list per CTA instead of one per stream.
-            float v = (lane < prm.k) ? mylist[lane] : INFINITY;
-            v = warp_sort_asc(v, lane);
-            mylist[lane] = v;
-        } else {
-            float *gl = prm.lists + (size_t)sidx * prm.kcap;
-            for (int j = lane; j < prm.kcap; j += 32) gl[j] = mylist[j];
+#pragma unroll
+        for (int m = 0; m < M; ++m) {
+            if (m >= nq) break;
+            if (lane == 0) {
+                prm.counts[pass_streams(m, S) + sidx] = logged[m];
+                if (logged[m] > prm.logcap) atomicExch(&prm.ctrl[m][1], 1);
+            }
+            if (prm.kcap == 32) {
+                // k <= 32: the CTA's 8 streams are consecutive in scan order.  Sort each stream's list, then one warp per query
+                // merges them in stream order, recording the running k-th value BEFORE each stream (its in-CTA prefix bound), and
+                // publishes ONE sorted list per CTA: filter_kernel then walks one list per CTA instead of one per stream.
+                float v = (lane < prm.k) ? mylist(m)[lane] : INFINITY;
+                v = warp_sort_asc(v, lane);
+                mylist(m)[lane] = v;
+            } else {
+                float *gl = prm.lists + pass_lists(m, S, prm.kcap) + (size_t)sidx * prm.kcap;
+                for (int j = lane; j < prm.kcap; j += 32) gl[j] = mylist(m)[j];
+            }
         }
     }
-    if (topk && prm.kcap == 32) __syncthreads();                             // every stream's sorted list is in lists_s
+    if (topk && prm.kcap == 32) __syncthreads();                             // every stream's sorted lists are in lists_s
     if (tid == 0 && prm.cta_time != nullptr)
         prm.cta_time[blockIdx.x] = (unsigned)min((long long)0xFFFFFFFFll, (clock64() - clk0) >> 6);   // units of 64 cycles
-    if (topk && prm.kcap == 32 && warp == 0) {
+    if (topk && prm.kcap == 32 && warp < nq) {                               // warp m merges query m's lists (nq <= kWarps)
+        const int m = warp;
         SortedList Lm;
         Lm.init(lane, prm.k);
         for (int w = 0; w < kWarps; ++w) {
-            if (lane == 0) prm.tlocal[(size_t)blockIdx.x * kWarps + w] = Lm.thr;
-            Lm.offer_sorted(lane, lists_s[w * 32 + lane]);
+            if (lane == 0) prm.tlocal[pass_streams(m, S) + (size_t)blockIdx.x * kWarps + w] = Lm.thr;
+            Lm.offer_sorted(lane, lists_s[((size_t)w * nq + m) * 32 + lane]);
         }
-        prm.lists[(size_t)blockIdx.x * 32 + lane] = Lm.v;
+        prm.lists[pass_lists(m, S, 32) + (size_t)blockIdx.x * 32 + lane] = Lm.v;
     }
 }
 
 template <int VT, int MC, bool DIRECT>
-__global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm) { scan_body<VT, MC, DIRECT, false>(prm); }
+__global__ void __launch_bounds__(kThreads, 1) scan_kernel(const ScanParams prm) { scan_body<VT, MC, DIRECT, false, 1>(prm); }
+// a pass of 2 <= nq <= M queries
+template <int VT, int MC, bool DIRECT, int M>
+__global__ void __launch_bounds__(kThreads, 1) scan_pass_kernel(const ScanParams prm) { scan_body<VT, MC, DIRECT, false, M>(prm); }
 template <int VT, int MC, bool DIRECT>
-__global__ void __launch_bounds__(kThreads, 1) scan_range_kernel(const ScanParams prm) { scan_body<VT, MC, DIRECT, true>(prm); }
+__global__ void __launch_bounds__(kThreads, 1) scan_range_kernel(const ScanParams prm) { scan_body<VT, MC, DIRECT, true, 1>(prm); }
 
 // ------------------------------------------------------------------ range search: result order
 // One block per query orders that query's (row, distance bits) pairs by (distance, row), in place: a bitonic sort of 64-bit keys

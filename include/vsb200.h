@@ -209,7 +209,9 @@ VSB_API int vsb_scan_device_query(vsb_index *ix, int metric, const void *d_query
  * (or for a held query's slot) arrives, any other call on the index (vsb_collect_last, vsb_result_block, vsb_scan_topk*,
  * range, batch, profile or debug calls, close).  A submission with nothing outstanding, or with fetch == 0, launches at
  * once.  So "submit i+1, collect i" pairs the queries; a caller who submits a second query and then does host work before
- * collecting the first leaves the second waiting until it does.  Sharing a pass never changes a result. */
+ * collecting the first leaves the second waiting until it does.  Sharing a pass never changes a result.
+ * A submission is checked before it is held or launched: VSB_EINVAL, with no slot taken and nothing launched, for an
+ * unknown metric, k outside 1..256, a null query, or a device query that is not 16-byte aligned. */
 VSB_API int vsb_scan_submit(vsb_index *ix, int metric, const void *query, int query_on_device, int k, int fetch, int slot);
 /* blocks until the engine stream is idle and converts the last device-side result into top-k. */
 VSB_API int vsb_collect_last(vsb_index *ix, int k, int64_t *out_rowids, double *out_dist, int *out_count);
@@ -227,7 +229,9 @@ VSB_API int vsb_merge_result_blocks(const void *blocks, int world, int64_t block
 /* the same for a GROUP of nq independent queries in one call (query j at queries + j * query_stride; slots first_slot ..
  * first_slot + nq - 1): what the sharded launcher uses so that its per-query host cost stays far below one shard scan.
  * The queries are launched at once, as passes of up to vsb_index_stat("plan_pass_max") queries (one read of the column per
- * pass, one filter launch per query); each query's result is what it gets alone. */
+ * pass, one filter launch per query); each query's result is what it gets alone.  Device queries (query_on_device != 0) are
+ * read as 16-byte vectors over the pitch: `queries` must be 16-byte aligned and, for nq > 1, query_stride a multiple of 16
+ * and at least vsb_index_query_pitch, each query zero-padded to the pitch; else VSB_EINVAL before anything is launched. */
 VSB_API int vsb_scan_submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device,
                                   int k, int fetch, int first_slot);
 /* vsb_merge_result_blocks for a gathered group: query j's block of shard r is at blocks + r * rank_stride + j * block_stride;
@@ -373,6 +377,11 @@ VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t b
  * workspace of a resident index, so that the next single-query scans with k <= 32 use it instead of equal shares (the filter
  * then rewrites it as usual).  Rejects an index too small for the adaptive partition.  Returns 0 or < 0. */
 VSB_API int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t bytes);
+/* diagnostics: the survivors of a result slot (fetch != 0) exactly as vsb_collect replays them: (uint32 distance bits, uint32
+ * local row) pairs in block-table order, the head's then the tail's, which is scan order.  Waits for the slot's query; a
+ * held query's pass is launched first, as vsb_collect does.  Writes the first `cap` pairs to out_pairs and the head's flags
+ * to *flags (non-zero: the candidates overflowed, and no pair is returned).  Returns the survivor count or < 0. */
+VSB_API int64_t vsb_debug_survivors(vsb_index *ix, int slot, uint32_t *out_pairs, int64_t cap, int *flags);
 /* diagnostics: ONE tensor-core level of the batch path (tc_scan_kernel; metric VSB_L1: l1_batch_kernel, any column type) over
  * rows [r0, r1) of a finalized resident index (r0 a multiple of 128), for nq HOST queries whose exact distance bounds U[nq] are
  * given instead of found by earlier levels; the per-query constants are the batch path's own (conservative_qc).  N: queries

@@ -105,6 +105,7 @@ _SIGNATURES = {
     "vsb_profile_read": (_i, [_vp, _vp, _vp, _vp, _vp]),
     "vsb_debug_read": (_i, [_vp, C.c_char_p, _vp, _i64]),
     "vsb_debug_write": (_i, [_vp, C.c_char_p, _vp, _i64]),
+    "vsb_debug_survivors": (_i64, [_vp, _i, _vp, _i64, C.POINTER(_i)]),
     "vsb_debug_tc_level": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i64, _i, _i, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
     "vsb_debug_refine": (_i, [_vp, _i, _vp, _i, _vp, _i64, _vp, _i64, _vp, _vp, _vp]),
     "vsb_debug_replay": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
@@ -513,6 +514,18 @@ class Index(_Column):
         """plant an internal buffer (vsb_debug_write); "bounds": int64 [stat("sms") + 1] tile boundaries"""
         a = np.ascontiguousarray(data, dtype=np.int64)
         self.eng.check(self.eng.lib.vsb_debug_write(self.h, name.encode(), _ptr(a), a.nbytes))
+
+    def debug_survivors(self, slot: int, cap: int = 1 << 16):
+        """(pairs uint32 [n, 2] of (distance bits, local row) in scan order, head flags) of a result slot: what collect(slot)
+        replays (vsb_debug_survivors); no pairs when the flags report an overflow"""
+        pairs = np.zeros((cap, 2), dtype=np.uint32)
+        flags = _i(0)
+        n = self.eng.lib.vsb_debug_survivors(self.h, slot, _ptr(pairs), cap, C.byref(flags))
+        if n < 0:
+            self.eng.check(n)
+        if n > cap:
+            raise VsbError(f"slot {slot} holds {n} survivors, more than cap = {cap}")
+        return pairs[:n].copy(), flags.value
 
     def debug_tc_level(self, metric: int, queries: np.ndarray, U: np.ndarray, r0: int, r1: int, N: int = 0, scores: bool = False,
                        cap: int = 1 << 22):

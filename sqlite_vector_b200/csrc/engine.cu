@@ -1026,8 +1026,18 @@ int check_index(vsb_index *ix) {
     return flush_held(ix);
 }
 
-bool scan_args_ok(const void *queries, int k) {
-    return queries != nullptr && k > 0 && k <= kMaxK;
+// what launch_scan would reject, checked before a submission stages, holds or launches anything.  A device query is read as
+// 16-byte vectors over its pitch: query j of a group at queries + j * query_stride must be 16-byte aligned and hold the
+// zero-padded pitch bytes before the next query begins.
+int check_submission(const vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device, int k) {
+    int root = 0;
+    if (!queries || k <= 0 || k > kMaxK) return fail(VSB_EINVAL, "bad scan arguments (k must be 1..%d)", kMaxK);
+    if (metric_class(metric, &root) < 0) return fail(VSB_EINVAL, "unknown distance metric %d", metric);
+    if (!query_on_device) return VSB_OK;
+    if ((uintptr_t)queries % 16 != 0) return fail(VSB_EINVAL, "device queries must be 16-byte aligned");
+    if (nq > 1 && (query_stride % 16 != 0 || query_stride < ix->pitch))
+        return fail(VSB_EINVAL, "device query stride %lld: a multiple of 16 and at least the pitch (%d) expected", (long long)query_stride, ix->pitch);
+    return VSB_OK;
 }
 
 // one pass of the column per pass_max queries of a group of independent queries (query j at queries + j * query_stride; slots
@@ -1035,10 +1045,11 @@ bool scan_args_ok(const void *queries, int k) {
 int submit_group(vsb_index *ix, int metric, const void *queries, int64_t query_stride, int nq, int query_on_device, int k, int fetch,
                  int first_slot, bool push) {
     if (check_index(ix)) return VSB_EINVAL;
-    if (!scan_args_ok(queries, k)) return fail(VSB_EINVAL, "bad scan arguments (k must be 1..%d)", kMaxK);
     if (nq <= 0 || first_slot < 0 || first_slot + nq > kSlots) return fail(VSB_EINVAL, "bad slot group [%d, %d)", first_slot, first_slot + nq);
+    int rc = check_submission(ix, metric, queries, query_stride, nq, query_on_device, k);
+    if (rc) return rc;
     CU(cudaSetDevice(ix->device));
-    int rc = ensure_slots(ix);
+    rc = ensure_slots(ix);
     if (rc) return rc;
     const int width = std::min(nq, pass_max(ix, (k + 31) & ~31));
     rc = ensure_workspace(ix, k, width);
@@ -1757,6 +1768,28 @@ int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t b
     return VSB_OK;
 }
 
+int64_t vsb_debug_survivors(vsb_index *ix, int slot_id, uint32_t *out_pairs, int64_t cap, int *flags) {
+    if (!ix) return fail(VSB_EINVAL, "null index");
+    if (slot_id < 0 || slot_id >= kSlots || !ix->slots_ready || (!out_pairs && cap > 0) || cap < 0 || !flags)
+        return fail(VSB_EINVAL, "bad debug survivors arguments");
+    for (int j = 0; j < ix->held.nq; ++j)            // as vsb_collect: reading a held query launches its pass
+        if (ix->held.slot[j] == slot_id) {
+            const int rc = flush_held(ix);
+            if (rc) return rc;
+        }
+    CU(cudaSetDevice(ix->device));
+    Slot *slot = &ix->slot[slot_id];
+    bool overflow = false;
+    int64_t n = 0;
+    const int rc = visit_survivors(ix, slot, &overflow, [&](uint2 c) {
+        if (n < cap) { out_pairs[2 * n] = c.x; out_pairs[2 * n + 1] = c.y; }
+        ++n;
+    });
+    if (rc) return rc;
+    *flags = slot->h_head->flags;
+    return n;
+}
+
 int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1, int N, int mode,
                        void *out, int64_t out_cap, void *out_qc, void *out_norms, int64_t *out_count) {
     if (check_index(ix)) return VSB_EINVAL;
@@ -1813,18 +1846,18 @@ int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches, double 
 int vsb_scan_submit(vsb_index *ix, int metric, const void *query, int query_on_device, int k, int fetch, int want_slot) {
     if (!ix) return fail(VSB_EINVAL, "null index");
     if (want_slot >= kSlots) return fail(VSB_EINVAL, "slot %d out of range (have %d)", want_slot, kSlots);
+    int rc = check_submission(ix, metric, query, 0, 1, query_on_device, k);   // before a held query could take a slot
+    if (rc) return rc;
     const int si = want_slot >= 0 ? want_slot : (ix->last_slot + 1) % kSlots;
     HeldPass &h = ix->held;
     bool in_pass = false;
     for (int j = 0; j < h.nq; ++j) in_pass |= h.slot[j] == si;
-    int rc = VSB_OK;
     if (h.nq > 0 && (in_pass || h.metric != metric || h.k != k)) rc = flush_held(ix);
     if (rc) return rc;
     ix->uncollected &= ~(1u << si);                 // a query left uncollected in this slot is given up
     if (fetch == 0 || ix->uncollected == 0) {
         rc = submit_group(ix, metric, query, 0, 1, query_on_device, k, fetch, si, false);
     } else {
-        if (!scan_args_ok(query, k)) return fail(VSB_EINVAL, "bad scan arguments (k must be 1..%d)", kMaxK);
         CU(cudaSetDevice(ix->device));
         rc = ensure_slots(ix);
         if (rc) return rc;

@@ -154,6 +154,31 @@ VSB_API int vsb_scan_topk_sets(vsb_index *ix, int metric, const void *queries, i
 VSB_API int vsb_scan_topk_rows(vsb_index *ix, int metric, const void *queries, int nq, int k, const int64_t *rowids,
                                const int64_t *offsets, int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
 
+/* ---- grouped top-k: each key's k nearest rows for the best keys, from one scan of the column per query (no counterpart in the
+ * reference, whose stream modules answer it with row_number() OVER (PARTITION BY key ORDER BY distance)) ---------------------------
+ * Key g's rowids are rowids[offsets[g], offsets[g + 1]) (offsets: nkeys + 1 non-decreasing values from 0; rowids may be NULL when
+ * there are none).  Rowids not in the column are ignored, a duplicate inside one key counts once, and keys may share rows.  For
+ * query q and key g the rows are bit for bit what vsb_scan_topk_filtered returns for that one query (nq = 1, max_index NULL) under
+ * the bitmap of g's rows: the same rowids, order and distances, exchange sort and INF trim, for every element type and metric.
+ * Keys with at least one row are ranked by their first row's distance (ascending, -INF first), then that row's scan position,
+ * then the key index; limit > 0 keeps the first limit keys, limit 0 every key with a row.  0 <= k <= 256 (k = 0: no keys; larger
+ * k is VSB_EINVAL); nkeys >= 0; limit >= 0.  Queries are answered one after another, each from a fresh cursor.  Each shard lays
+ * out its rows of every key once per call (more than 2^32 - 1 (key, row) pairs on one shard: VSB_ERANGE), then per query scans
+ * every distance, walks every key in pieces of 1024 rows on the device, and copies to the host only the candidates of the keys
+ * whose smallest distance over all shards is at or below the limit-th smallest (DESIGN §3.15).  A streamed index keeps the
+ * distances of all its windows on the device (4 bytes per row, in vsb_index_device_bytes).  Counters: "grouped_queries",
+ * "grouped_pairs" (the (key, row) pairs of the last layout), "grouped_cands" (candidates replayed), "grouped_keys_replayed" (on a
+ * group's first shard), "grouped_regrows", "grouped_layout_us", and the device times "grouped_scan_us" (scans) and
+ * "grouped_walk_us" (walk, bounds and compaction) and the host time "grouped_replay_us" (on a group's first shard).  *out receives
+ * a result owned by the caller (vsb_grouped_free); vsb_grouped_get borrows query q's arrays from it: nkeys_out keys in rank
+ * order, key i's rows at [row_offsets[i], row_offsets[i + 1]) of rowids and dist. */
+typedef struct vsb_grouped vsb_grouped;
+VSB_API int vsb_scan_topk_grouped(vsb_index *ix, int metric, const void *queries, int nq, int k, const int64_t *rowids,
+                                  const int64_t *offsets, int nkeys, int limit, vsb_grouped **out);
+VSB_API int vsb_grouped_get(const vsb_grouped *r, int q, int *nkeys_out, const int32_t **keys, const int64_t **row_offsets /* nkeys_out + 1 */,
+                            const int64_t **rowids, const double **dist); /* borrowed until free */
+VSB_API void vsb_grouped_free(vsb_grouped *r);
+
 /* ---- range search: every row closer than a radius (no counterpart in the reference, whose stream modules answer it as
  * SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < r ORDER BY distance) --------------------------------------
  * For query b (nq HOST queries, as for vsb_scan_topk) the result is every row with (double)d < radius[b], d being the distance
@@ -309,6 +334,10 @@ VSB_API int vsb_group_scan_topk_sets(vsb_group *g, int metric, const void *queri
 /* vsb_scan_topk_rows over the group's global scan order: every shard computes the distances of its own listed rows */
 VSB_API int vsb_group_scan_topk_rows(vsb_group *g, int metric, const void *queries, int nq, int k, const int64_t *rowids,
                                      const int64_t *offsets, int64_t *out_rowids, double *out_dist, int *out_counts, int *max_index);
+/* vsb_scan_topk_grouped over the group's global scan order: every shard lays out and walks its own rows of every key; the limit's
+ * bound is taken from each key's minimum over all shards, and each key replays the shards' candidates in shard order */
+VSB_API int vsb_group_scan_topk_grouped(vsb_group *g, int metric, const void *queries, int nq, int k, const int64_t *rowids,
+                                        const int64_t *offsets, int nkeys, int limit, vsb_grouped **out);
 /* vsb_scan_range over the group's global scan order (nbits = vsb_group_rows): every shard scans its rows, the shards' lists are
  * merged by (distance, global scan row) */
 VSB_API int vsb_group_scan_range(vsb_group *g, int metric, const void *queries, int nq, const double *radius, const uint32_t *allow,
@@ -350,7 +379,7 @@ VSB_API int vsb_index_query_pitch(const vsb_index *ix); /* bytes per query row o
  * per query), "rows_host_bytes" (bytes a streamed index's listed-rows kernel read from pinned host memory: pitch bytes per pair),
  * "sets_batches", "sets_fallbacks", "sets_levels", "sets_plan_us" (see vsb_scan_topk_sets), "scan_passes" (top-k passes of
  * the single-query scan kernel), "pass_queries" (the queries they scored: pass_queries / scan_passes queries per read of the
- * column)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
+ * column), "grouped_*" (see vsb_scan_topk_grouped)}, and the plan of the most recent single-query scan launch: "plan_log2p" (log2 of the lanes per
  * row), "plan_nsw" (ring stages per warp), "plan_direct" (1: no staging), "plan_pass_max" (the widest pass of the shape at the k
  * of the most recent top-k pass, k <= 32 before any); -1 if unknown (or, for plan_*, before any scan) */
 VSB_API int64_t vsb_index_stat(const vsb_index *ix, const char *name);

@@ -52,6 +52,9 @@ _SIGNATURES = {
     "vsb_index_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
     "vsb_scan_topk_rows": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vsb_scan_topk_sets": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "vsb_scan_topk_grouped": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, C.POINTER(_vp)]),
+    "vsb_grouped_get": (_i, [_vp, _i, C.POINTER(_i), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp)]),
+    "vsb_grouped_free": (None, [_vp]),
     "vsb_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_range_get": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_i64)]),
     "vsb_range_free": (None, [_vp]),
@@ -85,6 +88,7 @@ _SIGNATURES = {
     "vsb_group_rowid_bitmap": (_i64, [_vp, _vp, _i64, _vp]),
     "vsb_group_scan_topk_rows": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vsb_group_scan_topk_sets": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "vsb_group_scan_topk_grouped": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, C.POINTER(_vp)]),
     "vsb_group_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_group_gpus": (_i, [_vp]),
     "vsb_group_rows": (_i64, [_vp]),
@@ -275,6 +279,37 @@ def _range(eng: "Engine", fn, h, rows: int, metric: int, queries: np.ndarray, ra
     return out
 
 
+def _grouped(eng: "Engine", fn, h, metric: int, queries: np.ndarray, k: int, key_lists, limit: int):
+    """the grouped entry points: fn(handle, metric, queries, nq, k, rowids, offsets, nkeys, limit, &result) -> rc; per query a list
+    of (key index, rowids, distances), keys in rank order"""
+    q = np.ascontiguousarray(queries)
+    q2 = q.reshape(-1, q.shape[-1]) if q.ndim > 1 else q.reshape(1, -1)
+    nq = q2.shape[0]
+    lists = [np.asarray(r, dtype=np.int64).reshape(-1) for r in key_lists]
+    offsets = np.zeros(len(lists) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([len(r) for r in lists])
+    flat = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.int64))
+    res = _vp()
+    eng.check(fn(h, metric, _ptr(q2), nq, k, _ptr(flat), _ptr(offsets), len(lists), limit, C.byref(res)))
+    out = []
+    try:
+        for b in range(nq):
+            n, keys, offs, ids, dist = _i(), _vp(), _vp(), _vp(), _vp()
+            eng.check(eng.lib.vsb_grouped_get(res, b, C.byref(n), C.byref(keys), C.byref(offs), C.byref(ids), C.byref(dist)))
+            nk = n.value
+            if nk == 0:
+                out.append([])
+                continue
+            o = np.ctypeslib.as_array(C.cast(offs, C.POINTER(C.c_int64)), (nk + 1,))
+            kk = np.ctypeslib.as_array(C.cast(keys, C.POINTER(C.c_int32)), (nk,))
+            rid = np.ctypeslib.as_array(C.cast(ids, C.POINTER(C.c_int64)), (int(o[-1]),))
+            dd = np.ctypeslib.as_array(C.cast(dist, C.POINTER(C.c_double)), (int(o[-1]),))
+            out.append([(int(kk[i]), rid[o[i]:o[i + 1]].copy(), dd[o[i]:o[i + 1]].copy()) for i in range(nk)])
+    finally:
+        eng.lib.vsb_grouped_free(res)
+    return out
+
+
 def _rowid_bitmap(eng: "Engine", fn, h, rows: int, rowids) -> tuple[np.ndarray, int]:
     rid = np.ascontiguousarray(rowids, dtype=np.int64).reshape(-1)
     bits = np.zeros(max((rows + 31) // 32, 1), dtype=np.uint32)
@@ -328,6 +363,12 @@ class _Column:
         `sets` is a list of boolean masks over the scan-order rows or of uint32 row bitmaps, set_of_query[b] the index of query
         b's set (None: query b uses set b); each query's result equals scan_topk_filtered with its set"""
         return _sets_topk(self.eng, self._fn("scan_topk_sets"), self.h, self.rows, metric, queries, k, sets, set_of_query, as_arrays)
+
+    def scan_topk_grouped(self, metric: int, queries: np.ndarray, k: int, key_lists, limit: int = 0):
+        """each key's k nearest rows for the best keys (vsb_scan_topk_grouped): key_lists holds one sequence of rowids per key.
+        Returns per query a list of (key index, rowids, distances), keys ranked by their first distance (then its scan row, then
+        the key index) and cut to `limit` (0: every key with a row); each key's rows equal scan_topk_filtered with its rowids"""
+        return _grouped(self.eng, self._fn("scan_topk_grouped"), self.h, metric, queries, k, key_lists, limit)
 
     def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
         """every row with distance < radius (vsb_scan_range), for one query or a batch; radius: one value or one per query, allow:

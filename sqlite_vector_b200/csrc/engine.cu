@@ -273,12 +273,30 @@ struct vsb_index {
     // null outside such a call
     const SetsState *sets = nullptr;
     long long st_sets_batches = 0, st_sets_fallbacks = 0, st_sets_levels = 0, st_sets_plan_us = 0;
+    // grouped top-k (vsb_scan_topk_grouped, DESIGN §3.15): one device area for the layout and the per-query arrays of a call, and
+    // a streamed index's distances of every window (4 bytes per row), both grown never shrunk
+    DeviceBuf<uint8_t> d_grouped;
+    DeviceBuf<float> d_grouped_dist;
+    long long grouped_cap = 0, grouped_dist_cap = 0;
+    long long st_grouped_queries = 0, st_grouped_pairs = 0, st_grouped_cands = 0, st_grouped_keys_replayed = 0;
+    long long st_grouped_regrows = 0, st_grouped_layout_us = 0, st_grouped_scan_us = 0, st_grouped_walk_us = 0, st_grouped_replay_us = 0;
 };
 
 // result of a range call (vsb_scan_range): per query, rowids and distances in result order
 struct vsb_range {
     std::vector<std::vector<int64_t>> ids;
     std::vector<std::vector<double>> dist;
+};
+
+// result of a grouped call (vsb_scan_topk_grouped): per query, the keys in rank order and each key's rows in result order
+struct vsb_grouped {
+    struct Query {
+        std::vector<int32_t> keys;
+        std::vector<int64_t> offsets{0};
+        std::vector<int64_t> ids;
+        std::vector<double> dist;
+    };
+    std::vector<Query> q;
 };
 
 namespace {
@@ -505,8 +523,11 @@ int exchange_fill_push(vsb_index *ix, PushParams *pp);
 // exchange sequence number); push_heads_kernel moves them (exchange_push)
 // view_vec / view_n: scan these rows instead of the resident column (the windows of a streamed index)
 // view_r0: the shard row of view_vec's first row (the row filter is indexed by shard rows)
+// plan_kcap >= 0 (k == 0 only): scan with the plan of that kcap instead of k's, for all-distances scans whose distances must have
+// the bits of a top-k scan at that k (grouped top-k)
 int launch_scan(vsb_index *ix, int metric, const uint8_t *const *queries, Slot *const *slots, int nq, int k, float *d_dist_all, bool fetch,
-                cudaStream_t ss, bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1, long long view_r0 = 0) {
+                cudaStream_t ss, bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1, long long view_r0 = 0,
+                int plan_kcap = -1) {
     const uint8_t *scan_vec = view_vec ? view_vec : ix->d_vec;
     const long long scan_n = view_vec ? view_n : ix->n;
     if (!scan_vec) return fail(VSB_EINVAL, "this entry point needs a resident (not streamed) index");
@@ -519,7 +540,7 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *const *queries, Slot *
     if (kcap > ix->ws_kcap) return fail(VSB_EINVAL, "scan workspace too small for k = %d", k);
     if (nq < 1 || (nq > 1 && (k <= 0 || nq > ix->ws_width || nq > pass_max(ix, kcap))))
         return fail(VSB_EINVAL, "bad pass of %d queries", nq);
-    const Plan pl = make_plan(ix, kcap, nq);
+    const Plan pl = make_plan(ix, k == 0 && plan_kcap >= 0 ? plan_kcap : kcap, nq);
     ScanFn fn = pick_kernel(ix->vtype, mc, pl.direct, false, nq);
     if (!fn) return fail(VSB_EINVAL, "unsupported vector type %d", ix->vtype);
     // max-shared carve-out for the scan AND the filter kernel: kernels that want different L1/shared splits cannot share
@@ -1638,6 +1659,15 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "rows_queries")) return ix->st_rows_queries;
     if (!strcmp(name, "rows_pairs")) return ix->st_rows_pairs;
     if (!strcmp(name, "rows_host_bytes")) return ix->st_rows_host_bytes;
+    if (!strcmp(name, "grouped_queries")) return ix->st_grouped_queries;
+    if (!strcmp(name, "grouped_pairs")) return ix->st_grouped_pairs;
+    if (!strcmp(name, "grouped_cands")) return ix->st_grouped_cands;
+    if (!strcmp(name, "grouped_keys_replayed")) return ix->st_grouped_keys_replayed;
+    if (!strcmp(name, "grouped_regrows")) return ix->st_grouped_regrows;
+    if (!strcmp(name, "grouped_layout_us")) return ix->st_grouped_layout_us;
+    if (!strcmp(name, "grouped_scan_us")) return ix->st_grouped_scan_us;
+    if (!strcmp(name, "grouped_walk_us")) return ix->st_grouped_walk_us;
+    if (!strcmp(name, "grouped_replay_us")) return ix->st_grouped_replay_us;
     if (!strcmp(name, "sets_batches")) return ix->st_sets_batches;
     if (!strcmp(name, "sets_fallbacks")) return ix->st_sets_fallbacks;
     if (!strcmp(name, "sets_levels")) return ix->st_sets_levels;

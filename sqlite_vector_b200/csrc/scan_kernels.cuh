@@ -1064,6 +1064,191 @@ __global__ void __launch_bounds__(kLkThreads) lk_write_kernel(const LkParams p) 
     }
 }
 
+// ------------------------------------------------------------------ grouped top-k (DESIGN §3.15)
+// The keys' rows of one shard are laid out as positions in (key, scan order) order; every key's run is cut into pieces of at
+// most kGroupedPiece positions, and no piece crosses a key.  The distances of one query are already in dist (the all-distances
+// scan with the plan of the filtered call at this k).
+//   grouped_walk_kernel: one warp per piece reads d[row] in piece order and keeps the piece's k smallest.  A position is logged
+//   when d < the piece's running k-th value (+INF until k rows were seen, strict, as scan_kernel's ballot: NaN and +INF never
+//   log); pd[pos] is d for a logged position and NaN otherwise.  The piece publishes its k smallest, ascending, +INF padded.
+//   grouped_bounds_kernel: one warp per key merges its pieces' lists in piece order; a piece's bound is the k-th smallest of the
+//   earlier pieces of its key (+INF for the first), the key's minimum the smallest value of all of them (+INF: empty key).
+//   grouped_count_kernel, lk_offsets_kernel, grouped_write_kernel: the ordered compaction of the positions with pd < their
+//   piece's bound, of the selected keys only, into the pair list as (distance bits, position).
+constexpr int kGroupedPiece = 1024;  // positions of a piece
+constexpr int kGroupedWarps = 8;     // warps of a block: one piece or key each
+
+struct GroupedParams {
+    const float *dist;               // [shard rows] the query's distances
+    const uint32_t *rows;            // [positions] shard row of each position
+    const uint32_t *pstart;          // [npieces + 1] first position of each piece
+    const uint32_t *pkey;            // [npieces] key of each piece
+    const uint32_t *kpiece;          // [nkeys + 1] first piece of each key
+    float *pd;                       // [positions] d of a logged position, NaN otherwise
+    float *lists;                    // [npieces][k] each piece's k smallest, ascending, +INF padded
+    float *bound;                    // [npieces]
+    float *kmin;                     // [nkeys]
+    const uint8_t *ksel;             // [nkeys] keys to compact (nullptr: every key)
+    unsigned *pcount;                // [npieces] survivors of each piece, then where they start (lk_offsets_kernel)
+    uint2 *out;                      // pair list; positions at or past cap are not written
+    long long cap;
+    long long npieces;
+    int nkeys, k;
+};
+
+// the k smallest values (k <= kcap, entries >= k of list hold -INF) of a warp's shared list, ascending, into out[0, k)
+__device__ __forceinline__ void grouped_sorted_out(const float *list, int k, int lane, float *out) {
+    for (int j = lane; j < k; j += 32) {
+        const float v = list[j];
+        int rank = 0;
+        for (int i = 0; i < k; ++i) {
+            const float u = list[i];
+            rank += (u < v || (u == v && i < j)) ? 1 : 0;
+        }
+        out[rank] = v;
+    }
+}
+
+// SMALL: k <= 32, the running list in registers (SortedList); otherwise a shared list of kMaxK entries per warp (list_argmax)
+template <bool SMALL>
+__global__ void __launch_bounds__(kGroupedWarps * 32) grouped_walk_kernel(const GroupedParams p) {
+    __shared__ float sl[SMALL ? 1 : kGroupedWarps * 256];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp;
+    if (pc >= p.npieces) return;
+    const uint32_t a = p.pstart[pc], b = p.pstart[pc + 1];
+    const int k = p.k, kcap = (k + 31) & ~31;
+    SortedList L;
+    float *list = sl + (SMALL ? 0 : warp * 256);
+    float thr = INFINITY;
+    int pos = 0;
+    if constexpr (SMALL) {
+        L.init(lane, k);
+    } else {
+        for (int j = lane; j < kcap; j += 32) list[j] = (j < k) ? INFINITY : -INFINITY;
+        __syncwarp();
+        list_argmax(list, kcap, lane, thr, pos);
+    }
+    for (uint32_t c0 = a; c0 < b; c0 += 32) {
+        const uint32_t at = c0 + (uint32_t)lane;
+        const bool valid = at < b;
+        const float d = valid ? p.dist[p.rows[at]] : __int_as_float(0x7FC00000);
+        unsigned msk = __ballot_sync(0xFFFFFFFFu, valid && d < (SMALL ? L.thr : thr));
+        unsigned logged = 0u;
+        while (msk) {
+            const int src = __ffs(msk) - 1;
+            msk &= msk - 1;
+            const float dv = __shfl_sync(0xFFFFFFFFu, d, src);
+            if constexpr (SMALL) {
+                if (dv < L.thr) {
+                    L.insert(lane, dv);
+                    logged |= 1u << src;
+                }
+            } else if (dv < thr) {
+                if (lane == 0) list[pos] = dv;
+                __syncwarp();
+                list_argmax(list, kcap, lane, thr, pos);
+                logged |= 1u << src;
+            }
+        }
+        if (valid) p.pd[at] = ((logged >> lane) & 1u) ? d : __int_as_float(0x7FC00000);
+    }
+    float *out = p.lists + (size_t)pc * k;
+    if constexpr (SMALL) {
+        if (lane < k) out[lane] = L.v;
+    } else {
+        __syncwarp();
+        grouped_sorted_out(list, k, lane, out);
+    }
+}
+
+// one warp per key: its pieces' bounds and its minimum
+template <bool SMALL>
+__global__ void __launch_bounds__(kGroupedWarps * 32) grouped_bounds_kernel(const GroupedParams p) {
+    __shared__ float sl[SMALL ? 1 : kGroupedWarps * 256];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int g = blockIdx.x * kGroupedWarps + warp;
+    if (g >= p.nkeys) return;
+    const int k = p.k, kcap = (k + 31) & ~31;
+    const uint32_t q0 = p.kpiece[g], q1 = p.kpiece[g + 1];
+    SortedList L;
+    float *list = sl + (SMALL ? 0 : warp * 256);
+    float thr = INFINITY, mn = INFINITY;
+    int pos = 0;
+    if constexpr (SMALL) {
+        L.init(lane, k);
+    } else {
+        for (int j = lane; j < kcap; j += 32) list[j] = (j < k) ? INFINITY : -INFINITY;
+        __syncwarp();
+        list_argmax(list, kcap, lane, thr, pos);
+    }
+    for (uint32_t pc = q0; pc < q1; ++pc) {
+        const float *src = p.lists + (size_t)pc * k;
+        if (lane == 0) p.bound[pc] = SMALL ? L.thr : thr;
+        mn = fminf(mn, src[0]);
+        if constexpr (SMALL) {
+            L.offer_sorted(lane, lane < k ? src[lane] : INFINITY);
+        } else {
+            // the list is ascending: once a value is not below the running k-th value, none after it is
+            for (int j0 = 0; j0 < k; j0 += 32) {
+                const float v = j0 + lane < k ? src[j0 + lane] : INFINITY;
+                unsigned msk = __ballot_sync(0xFFFFFFFFu, v < thr);
+                if (!msk) break;
+                while (msk) {
+                    const int s = __ffs(msk) - 1;
+                    msk &= msk - 1;
+                    const float dv = __shfl_sync(0xFFFFFFFFu, v, s);
+                    if (dv < thr) {
+                        if (lane == 0) list[pos] = dv;
+                        __syncwarp();
+                        list_argmax(list, kcap, lane, thr, pos);
+                    }
+                }
+            }
+        }
+    }
+    if (lane == 0) p.kmin[g] = mn;
+}
+
+__device__ __forceinline__ bool grouped_selected(const GroupedParams &p, long long pc) {
+    return p.ksel == nullptr || p.ksel[p.pkey[pc]] != 0;
+}
+
+// one warp per piece: its survivors
+__global__ void __launch_bounds__(kGroupedWarps * 32) grouped_count_kernel(const GroupedParams p) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp;
+    if (pc >= p.npieces) return;
+    unsigned c = 0;
+    if (grouped_selected(p, pc)) {
+        const uint32_t a = p.pstart[pc], b = p.pstart[pc + 1];
+        const float bd = p.bound[pc];
+        for (uint32_t at = a + (uint32_t)lane; at < b; at += 32) c += p.pd[at] < bd ? 1u : 0u;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, o);
+    }
+    if (lane == 0) p.pcount[pc] = c;
+}
+
+// one warp per piece: its survivors in position order from the piece's offset on
+__global__ void __launch_bounds__(kGroupedWarps * 32) grouped_write_kernel(const GroupedParams p) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp;
+    if (pc >= p.npieces || !grouped_selected(p, pc)) return;
+    const uint32_t a = p.pstart[pc], b = p.pstart[pc + 1];
+    const float bd = p.bound[pc];
+    unsigned w = p.pcount[pc];
+    for (uint32_t c0 = a; c0 < b; c0 += 32) {
+        const uint32_t at = c0 + (uint32_t)lane;
+        const float d = at < b ? p.pd[at] : __int_as_float(0x7FC00000);
+        const bool hit = d < bd;
+        const unsigned m = __ballot_sync(0xFFFFFFFFu, hit);
+        const unsigned o = w + (unsigned)__popc(m & ((1u << lane) - 1u));
+        if (hit && (long long)o < p.cap) p.out[o] = make_uint2(__float_as_uint(d), at);
+        w += (unsigned)__popc(m);
+    }
+}
+
 // ------------------------------------------------------------------ candidate filter
 // One warp per stream.  thresholds: a row of stream s can only enter the reference's slots if its distance
 // is below the k-th smallest distance among ALL earlier rows; any subset of earlier rows gives a valid upper

@@ -9,6 +9,7 @@
  * additions: vector_*_scan_batch (tbl, col, vectors, k); vector_*_scan_filtered (tbl, col, vector, k, rowids),
  *            vector_*_scan_batch_filtered (tbl, col, vectors, k, rowids) and the aggregate vector_rowid_set(x) that builds rowids;
  *            vector_*_scan_batch_sets (tbl, col, vectors, k, sets, query_sets) and the aggregate vector_rowid_sets(set, rowid);
+ *            vector_*_scan_grouped (tbl, col, vector, k, groups, limit);
  *            vector_*_scan_range (tbl, col, vector, radius), vector_*_scan_range_filtered (tbl, col, vector, radius, rowids);
  *            vector_quantize_scan_rerank (tbl, col, vector, k, candidates), vector_quantize_scan_rerank_batch (tbl, col, vectors, k,
  *            candidates)
@@ -88,6 +89,7 @@ typedef struct {
     /* batch mode (vector_*_scan_batch): ids/dist hold bnq x bk results, bcounts[b] valid rows of query b */
     int batch, bnq, bk, bq, bj;
     int *bcounts;
+    sqlite3_int64 *bkeys;          /* grouped mode (vector_*_scan_grouped): the key of each result group, emitted as its first column */
 } scan_cursor;
 
 /* ------------------------------------------------------------------------------------------------ helpers */
@@ -1180,6 +1182,7 @@ static int vt_open(sqlite3_vtab *t, sqlite3_vtab_cursor **out) {
 static int vt_close(sqlite3_vtab_cursor *cur) {
     scan_cursor *c = (scan_cursor *)cur;
     sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->sdist); sqlite3_free(c->sids); sqlite3_free(c->bcounts);
+    sqlite3_free(c->bkeys);
     sqlite3_free(c);
     return SQLITE_OK;
 }
@@ -1504,7 +1507,8 @@ static int vt_column_batch(sqlite3_vtab_cursor *cur, sqlite3_context *ctx, int c
     scan_cursor *c = (scan_cursor *)cur;
     const size_t at = (size_t)c->bq * (size_t)c->bk + (size_t)c->bj;
     col -= ((scan_vtab *)cur->pVtab)->filtered;
-    if (col == BCOL_QUERY) sqlite3_result_int(ctx, c->bq);
+    if (col == BCOL_QUERY && c->bkeys) sqlite3_result_int64(ctx, c->bkeys[c->bq]);
+    else if (col == BCOL_QUERY) sqlite3_result_int(ctx, c->bq);
     else if (col == BCOL_ID) sqlite3_result_int64(ctx, c->ids[at]);
     else if (col == BCOL_DISTANCE) sqlite3_result_double(ctx, c->dist[at]);
     return SQLITE_OK;
@@ -1627,6 +1631,127 @@ static sqlite3_module mod_full_batch_sets = {0, 0, vt_connect_batch_sets, vt_bes
                                              vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 static sqlite3_module mod_quant_batch_sets = {0, 0, vt_connect_batch_sets, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch_sets,
                                               vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+
+/* ------------------------------------------------------------------------------------------------ grouped scans
+ * vector_*_scan_grouped(tbl, col, vector, k, groups, limit): each key's k nearest rows for the `limit` best keys (NULL or 0: every
+ * key with a row), keys ranked by their first row's distance, then its scan position, then the key.  `groups` is a BLOB of
+ * little-endian (int64 key, int64 rowid) pairs (vector_rowid_sets builds it); keys may be sparse.  Rows are (key, id, distance),
+ * keys in rank order and each key's rows exactly those of vector_*_scan_filtered with that key's rowids (vsb_group_scan_topk_grouped,
+ * DESIGN §3.15).  No counterpart in the reference, which answers it with row_number() OVER (PARTITION BY key ORDER BY distance)
+ * over vector_*_scan_stream. */
+static int vt_connect_grouped(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
+    (void)argc; (void)argv; (void)err;
+    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, groups hidden, \"limit\" hidden, key, id, distance);", 2, out);
+}
+
+static int filter_grouped(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized) {
+    scan_cursor *c = (scan_cursor *)cur;
+    scan_vtab *vt = (scan_vtab *)cur->pVtab;
+    c->batch = 1;
+    c->bnq = 0; c->bq = 0; c->bj = 0;
+    if (argc != 6) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, 6, argc);
+    for (int i = 0; i < argc; ++i) {
+        int t = sqlite3_value_type(argv[i]);
+        if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
+        if (i == 4 && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument 5 must be of type BLOB (got %s).", fname, sql_type_name(t));
+        if (i == 4 && sqlite3_value_bytes(argv[4]) % 16 != 0)
+            return vtab_error(&vt->base, "%s: groups has %d bytes, expected a multiple of 16 (int64 key, int64 rowid pairs).", fname, sqlite3_value_bytes(argv[4]));
+        if (i == 5 && t != SQLITE_INTEGER && t != SQLITE_NULL) return vtab_error(&vt->base, "%s: argument 6 must be of type INTEGER or NULL (got %s).", fname, sql_type_name(t));
+        if (i == 5 && t == SQLITE_INTEGER && sqlite3_value_int64(argv[5]) < 0) return vtab_error(&vt->base, "%s: limit must not be negative.", fname);
+    }
+    const char *tbl = (const char *)sqlite3_value_text(argv[0]);
+    const char *col = (const char *)sqlite3_value_text(argv[1]);
+    vcolumn *v = ctx_find(vt->ctx, tbl, col);
+    if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
+    const int need = v->dim * elem_size(v->vtype);
+    void *owned = 0;
+    const void *query = 0;
+    if (sqlite3_value_type(argv[2]) == SQLITE_TEXT) {
+        int sz = 0;
+        owned = json_to_blob(0, &vt->base, v->vtype, (const char *)sqlite3_value_text(argv[2]), &sz, v->dim);
+        if (!owned) return SQLITE_ERROR;
+        query = owned;
+    } else {
+        query = sqlite3_value_blob(argv[2]);
+        if (!query) return vtab_error(&vt->base, "%s: input vector cannot be NULL.", fname);
+        if (sqlite3_value_bytes(argv[2]) < need) return vtab_error(&vt->base, "%s: input vector has %d bytes, expected %d.", fname, sqlite3_value_bytes(argv[2]), need);
+    }
+    const sqlite3_int64 npairs = sqlite3_value_bytes(argv[4]) / 16, lim64 = sqlite3_value_type(argv[5]) == SQLITE_NULL ? 0 : sqlite3_value_int64(argv[5]);
+    const int limit = lim64 > 0x7FFFFFFF ? 0 : (int)lim64;     /* a limit above every possible key count keeps every key */
+    int rc = SQLITE_OK, nkeys = 0;
+    uint8_t *qq = 0;
+    int64_t *pairs = 0, *rowids = 0, *offsets = 0, *keys = 0;
+    vsb_group *ix = 0;
+    vsb_grouped *res = 0;
+    const int k = sqlite3_value_int(argv[3]);
+    if (k < 0) { rc = vtab_error(&vt->base, "%s: k must not be negative.", fname); goto out; }
+    rc = resident_index(vt, v, tbl, col, fname, quantized, &ix);
+    if (rc != SQLITE_OK) goto out;
+    if (quantized) {
+        qq = (uint8_t *)sqlite3_malloc(v->dim);
+        if (!qq) { rc = SQLITE_NOMEM; goto out; }
+        quantize_vec(v->vtype, query, qq, v->offset, v->scale, v->dim, v->qtype);
+        query = qq;
+    }
+    if (k == 0) goto out;                                                /* empty result, like k = 0 of the top-k functions */
+    pairs = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * 16);
+    rowids = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * sizeof(int64_t));
+    offsets = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs + 1) * sizeof(int64_t));
+    keys = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * sizeof(int64_t));
+    if (!pairs || !rowids || !offsets || !keys) { rc = SQLITE_NOMEM; goto out; }
+    if (npairs > 0) memcpy(pairs, sqlite3_value_blob(argv[4]), (size_t)npairs * 16);   /* little-endian host */
+    qsort(pairs, (size_t)npairs, 16, cmp_pair);
+    offsets[0] = 0;
+    for (sqlite3_int64 i = 0; i < npairs; ++i) {                          /* distinct keys -> dense 0 .. nkeys-1, rowids in CSR form */
+        if (nkeys == 0 || keys[nkeys - 1] != pairs[2 * i]) {
+            if (nkeys > 0) offsets[nkeys] = i;
+            keys[nkeys++] = pairs[2 * i];
+        }
+        rowids[i] = pairs[2 * i + 1];
+    }
+    offsets[nkeys] = npairs;
+    if (vsb_group_scan_topk_grouped(ix, v->metric, query, 1, k, rowids, offsets, nkeys, limit, &res) != VSB_OK) {
+        rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
+        goto out;
+    }
+    {
+        int nk = 0;
+        const int32_t *gk = 0;
+        const int64_t *go = 0, *gi = 0;
+        const double *gd = 0;
+        vsb_grouped_get(res, 0, &nk, &gk, &go, &gi, &gd);
+        sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->bcounts); sqlite3_free(c->bkeys);
+        c->k_alloc = 0;
+        c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * (sqlite3_uint64)k * sizeof(sqlite3_int64));
+        c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * (sqlite3_uint64)k * sizeof(double));
+        c->bcounts = (int *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * sizeof(int));
+        c->bkeys = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * sizeof(sqlite3_int64));
+        if (!c->ids || !c->dist || !c->bcounts || !c->bkeys) { rc = SQLITE_NOMEM; goto out; }
+        for (int i = 0; i < nk; ++i) {
+            const int n = (int)(go[i + 1] - go[i]);
+            c->bcounts[i] = n;
+            c->bkeys[i] = keys[gk[i]];
+            memcpy(c->ids + (size_t)i * k, gi + go[i], (size_t)n * sizeof(int64_t));
+            memcpy(c->dist + (size_t)i * k, gd + go[i], (size_t)n * sizeof(double));
+        }
+        c->bnq = nk;
+        c->bk = k;
+        batch_skip_empty(c);
+    }
+out:
+    vsb_grouped_free(res);
+    sqlite3_free(owned); sqlite3_free(qq);
+    sqlite3_free(pairs); sqlite3_free(rowids); sqlite3_free(offsets); sqlite3_free(keys);
+    return rc;
+}
+static int vt_filter_full_grouped(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_grouped(c, argc, argv, "vector_full_scan_grouped", 0); }
+static int vt_filter_quant_grouped(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_grouped(c, argc, argv, "vector_quantize_scan_grouped", 1); }
+static sqlite3_module mod_full_grouped = {0, 0, vt_connect_grouped, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_full_grouped,
+                                          vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+static sqlite3_module mod_quant_grouped = {0, 0, vt_connect_grouped, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_grouped,
+                                           vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 
 #define SCAN_MODULE(NAME, CONNECT, BEST, FILTER)                                                                          \
     static sqlite3_module NAME = {0, 0, CONNECT, BEST, vt_disconnect, 0, vt_open, vt_close, FILTER, vt_next, vt_eof, \
@@ -1880,6 +2005,8 @@ __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char
     if ((rc = sqlite3_create_module(db, "vector_full_scan_batch_sets", &mod_full_batch_sets, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch_sets", &mod_quant_batch_sets, ctx)) != SQLITE_OK) return rc;
     /* additions: range scans */
+    if ((rc = sqlite3_create_module(db, "vector_full_scan_grouped", &mod_full_grouped, ctx)) != SQLITE_OK) return rc;
+    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_grouped", &mod_quant_grouped, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_full_scan_range", &mod_full_range, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range", &mod_quant_range, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_module(db, "vector_full_scan_range_filtered", &mod_full_range_filtered, ctx)) != SQLITE_OK) return rc;

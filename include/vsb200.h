@@ -399,12 +399,21 @@ VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches,
  * large-k batch on this index: int64 piece count P, int64 query count Q, int64 [P][3] each piece's shard rows [first, end) and
  * level, float [P][Q] the bound each piece was refined against, +INF for level 0), "large_k_batch_cands" (the same batch's
  * candidates: int64 query count Q, int64 [Q] each query's count (-1: answered alone), then the queries' (uint32 distance bits,
- * uint32 shard row) pairs in scan order, query after query)}.  Returns the bytes copied or < 0. */
+ * uint32 shard row) pairs in scan order, query after query), "grouped" (this shard's state after the most recent
+ * vsb_scan_topk_grouped or group call with k > 0, keys and queries, for its last query (DESIGN §3.15): int64 [7] {P positions,
+ * N pieces, G keys, k, D distances (the shard's rows; 0 without positions), S (1: the limit selected keys), C survivor pairs},
+ * then uint32 rows [P] (shard row of each position), koff [G + 1], pstart [N + 1], pkey [N], kpiece [G + 1], float dist [D] (the
+ * query's distances), pd [P] (d where the walk logged, NaN otherwise), lists [N][k], bound [N], kmin [G], uint32 [C][2]
+ * survivors (distance bits, position) in position order, and with S = 1 uint8 ksel [G] (1: the key was compacted))}.  Returns
+ * the bytes copied or < 0. */
 VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes);
 /* diagnostics: the counterpart of vsb_debug_read for name "bounds": plants a row partition (int64 tile boundaries, one per scan
  * CTA plus one, non-decreasing from 0 to the tile count of the k <= 32 plan; vsb_index_stat "sms" CTAs) into every scan
  * workspace of a resident index, so that the next single-query scans with k <= 32 use it instead of equal shares (the filter
- * then rewrites it as usual).  Rejects an index too small for the adaptive partition.  Returns 0 or < 0. */
+ * then rewrites it as usual).  Rejects an index too small for the adaptive partition.  Name "grouped_dist": float32 [shard
+ * rows], the distances every query of the next grouped call on this index (resident or streamed, or a shard of a group through
+ * vsb_group_shard) uses instead of its scans; everything after the scans runs as usual, and the call drops the plant when it
+ * ends, however it ends.  Returns 0 or < 0. */
 VSB_API int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t bytes);
 /* diagnostics: the survivors of a result slot (fetch != 0) exactly as vsb_collect replays them: (uint32 distance bits, uint32
  * local row) pairs in block-table order, the head's then the tail's, which is scan order.  Waits for the slot's query; a

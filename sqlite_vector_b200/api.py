@@ -552,9 +552,31 @@ class Index(_Column):
         return out[: got // out.itemsize]
 
     def debug_write(self, name: str, data: np.ndarray):
-        """plant an internal buffer (vsb_debug_write); "bounds": int64 [stat("sms") + 1] tile boundaries"""
-        a = np.ascontiguousarray(data, dtype=np.int64)
+        """plant an internal buffer (vsb_debug_write); "bounds": int64 [stat("sms") + 1] tile boundaries; "grouped_dist":
+        float32 [rows], the distances of the next grouped call instead of its scans"""
+        a = np.ascontiguousarray(data, dtype=np.float32 if name == "grouped_dist" else np.int64)
         self.eng.check(self.eng.lib.vsb_debug_write(self.h, name.encode(), _ptr(a), a.nbytes))
+
+    def debug_grouped(self) -> dict:
+        """this shard's state after the last grouped call, for its last query (vsb_debug_read "grouped"): numpy arrays "rows",
+        "koff", "pstart", "pkey", "kpiece" (uint32 layout), "dist", "pd", "lists" [npieces, k], "bound", "kmin" (float32),
+        "pairs" (uint32 [n, 2] of (distance bits, position)), "ksel" (uint8 per key, None when every key was compacted), and "k" """
+        head = self.debug_read("grouped", np.int64, 7)
+        P, N, G, k, D, S, Cn = (int(v) for v in head)
+        sizes = [("rows", "<u4", P), ("koff", "<u4", G + 1), ("pstart", "<u4", N + 1), ("pkey", "<u4", N), ("kpiece", "<u4", G + 1),
+                 ("dist", "<f4", D), ("pd", "<f4", P), ("lists", "<f4", N * k), ("bound", "<f4", N), ("kmin", "<f4", G),
+                 ("pairs", "<u4", 2 * Cn), ("ksel", "u1", G if S else 0)]
+        raw = self.debug_read("grouped", np.uint8, 56 + sum(np.dtype(t).itemsize * c for _, t, c in sizes))
+        out, at = {"k": k}, 56
+        for name, t, c in sizes:
+            nb = np.dtype(t).itemsize * c
+            out[name] = raw[at:at + nb].view(t).copy()
+            at += nb
+        out["lists"] = out["lists"].reshape(N, k)
+        out["pairs"] = out["pairs"].reshape(Cn, 2)
+        if not S:
+            out["ksel"] = None
+        return out
 
     def debug_survivors(self, slot: int, cap: int = 1 << 16):
         """(pairs uint32 [n, 2] of (distance bits, local row) in scan order, head flags) of a result slot: what collect(slot)

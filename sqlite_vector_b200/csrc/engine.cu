@@ -179,6 +179,7 @@ struct HeldPass {
 
 struct BatchWs;   // batch_host.inc
 struct SetsState;   // batch_host.inc
+struct GroupedShard;   // batch_host.inc
 
 }  // namespace
 
@@ -278,6 +279,10 @@ struct vsb_index {
     DeviceBuf<uint8_t> d_grouped;
     DeviceBuf<float> d_grouped_dist;
     long long grouped_cap = 0, grouped_dist_cap = 0;
+    // this shard's layout and last query's host state of the most recent grouped call (vsb_debug_read "grouped"), kept until the
+    // next one; and the distances planted by vsb_debug_write "grouped_dist" for the next call (empty: scan them)
+    std::unique_ptr<GroupedShard> grouped;
+    std::vector<float> grouped_plant;
     long long st_grouped_queries = 0, st_grouped_pairs = 0, st_grouped_cands = 0, st_grouped_keys_replayed = 0;
     long long st_grouped_regrows = 0, st_grouped_layout_us = 0, st_grouped_scan_us = 0, st_grouped_walk_us = 0, st_grouped_replay_us = 0;
 };
@@ -1764,6 +1769,42 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
         memcpy(out, d.data(), n);
         return (int)n;
     }
+    else if (!strcmp(name, "grouped")) {                                // the layout and last query of the last grouped call
+        if (!ix->grouped) return fail(VSB_EINVAL, "no grouped call has run yet");
+        const GroupedShard &gs = *ix->grouped;
+        const GroupedParams &p = gs.p;
+        const size_t npos = gs.rows.size(), np = gs.pkey.size(), nk = gs.kmin.size(), kk = (size_t)p.k;
+        const size_t ndist = npos ? (size_t)ix->n : 0;
+        const long long head[7] = {(long long)npos, (long long)np, (long long)nk, (long long)kk, (long long)ndist, gs.ksel_used ? 1 : 0,
+                                   (long long)gs.pairs.size()};
+        std::vector<uint8_t> d(sizeof head);
+        memcpy(d.data(), head, sizeof head);
+        const auto host = [&](const void *src, size_t n) {
+            d.insert(d.end(), (const uint8_t *)src, (const uint8_t *)src + n);
+        };
+        const auto dev = [&](const void *src, size_t n) {
+            const size_t at = d.size();
+            d.resize(at + n);
+            if (n) CU(cudaMemcpy(d.data() + at, src, n, cudaMemcpyDeviceToHost));
+            return (int)VSB_OK;
+        };
+        host(gs.rows.data(), 4 * npos);
+        host(gs.koff.data(), 4 * (nk + 1));
+        host(gs.pstart.data(), 4 * (np + 1));
+        host(gs.pkey.data(), 4 * np);
+        host(gs.kpiece.data(), 4 * (nk + 1));
+        int rc2 = dev(gs.d_dist, 4 * ndist);
+        if (rc2 == VSB_OK) rc2 = dev(p.pd, 4 * npos);
+        if (rc2 == VSB_OK) rc2 = dev(p.lists, 4 * np * kk);
+        if (rc2 == VSB_OK) rc2 = dev(p.bound, 4 * np);
+        if (rc2) return rc2;
+        host(gs.kmin.data(), 4 * nk);
+        host(gs.pairs.data(), sizeof(uint2) * gs.pairs.size());
+        if (gs.ksel_used && (rc2 = dev(gs.d_ksel, nk))) return rc2;
+        const size_t n = std::min<size_t>({d.size(), (size_t)bytes, (size_t)INT32_MAX});
+        memcpy(out, d.data(), n);
+        return (int)n;
+    }
     else return fail(VSB_EINVAL, "unknown debug buffer %s", name);
     if (!src) return fail(VSB_EINVAL, "no %s has run yet", strcmp(name, "topk_bounds") ? "scan" : "large-k query");
     CU(cudaMemcpy(out, src, std::min<size_t>(have, (size_t)bytes), cudaMemcpyDeviceToHost));
@@ -1773,6 +1814,12 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
 int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t bytes) {
     if (check_index(ix)) return VSB_EINVAL;
     if (!name || !data) return fail(VSB_EINVAL, "bad debug write arguments");
+    if (!strcmp(name, "grouped_dist")) {       // the distances of every shard row for the next grouped call, instead of its scans
+        if (bytes != (int64_t)sizeof(float) * ix->n || ix->n == 0)
+            return fail(VSB_EINVAL, "grouped_dist: %lld bytes expected (float32 x %lld)", (long long)sizeof(float) * ix->n, ix->n);
+        ix->grouped_plant.assign((const float *)data, (const float *)data + ix->n);
+        return VSB_OK;
+    }
     if (strcmp(name, "bounds") != 0) return fail(VSB_EINVAL, "unknown debug buffer %s", name);
     if (ix->streamed || !ix->d_vec) return fail(VSB_EINVAL, "the row partition belongs to a resident index");
     const size_t want = sizeof(long long) * (size_t)(ix->num_sms + 1);

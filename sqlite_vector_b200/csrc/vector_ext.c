@@ -42,8 +42,9 @@ const sqlite3_api_routines *vsq_api = 0;
 #define MAX_COLUMNS 128                        /* MAX_TABLES, src/sqlite-vector.c:72 */
 #define DEFAULT_MAX_MEMORY (30 * 1024 * 1024)  /* src/sqlite-vector.c:71 */
 
-/* hidden / visible columns of the table-valued functions (src/sqlite-vector.c:98-103, :1830) */
-enum { COL_TBL = 0, COL_VECTOR = 1, COL_K = 2, COL_MEMIDX = 3, COL_ID = 4, COL_DISTANCE = 5 };
+/* the hidden columns every table-valued function starts with (src/sqlite-vector.c:98-103, :1830) */
+enum { COL_TBL = 0, COL_VECTOR = 1, COL_K = 2, COL_MEMIDX = 3 };
+#define N_MODULES 20                           /* rows of `modules`, the table-valued functions */
 
 /* ------------------------------------------------------------------------------------------------ state */
 typedef struct {
@@ -63,33 +64,36 @@ typedef struct {
     int fix_tainted;               /* staged inside an open transaction: never reused */
 } vcolumn;
 
+typedef struct module_def module_def;         /* one table-valued function: a row of `modules` */
+typedef struct vcontext vcontext;
 typedef struct {
+    const module_def *def;
+    vcontext *ctx;
+} vmodule;                                     /* a module's pAux: its row and the connection's columns */
+struct vcontext {
     vcolumn cols[MAX_COLUMNS];
     int ncols;
-} vcontext;
+    vmodule mods[N_MODULES];
+};
 
 typedef struct {
     sqlite3_vtab base;
     sqlite3 *db;
     vcontext *ctx;
-    int filtered;                  /* hidden columns before the visible ones beyond memidx: 1 for *_filtered (rowids), 2 for *_sets (sets, query_sets) */
+    const module_def *def;
 } scan_vtab;
 
+/* a result is ngroups groups of rows: group g has count[g] rows at ids / dist + g * stride and, for grouped scans, the key
+ * key[g].  One group for the one-query modules, one per query for the many-query modules, one per returned key for grouped. */
 typedef struct {
     sqlite3_vtab_cursor base;
-    int streaming;
-    /* top-k mode */
-    sqlite3_int64 *ids;
+    int64_t *ids;
     double *dist;
-    int k_alloc, row_count, row_index, max_index;
-    /* stream mode */
-    float *sdist;
-    sqlite3_int64 *sids;
-    sqlite3_int64 sn, spos;
-    /* batch mode (vector_*_scan_batch): ids/dist hold bnq x bk results, bcounts[b] valid rows of query b */
-    int batch, bnq, bk, bq, bj;
-    int *bcounts;
-    sqlite3_int64 *bkeys;          /* grouped mode (vector_*_scan_grouped): the key of each result group, emitted as its first column */
+    float *fdist;                  /* a stream's distances, in place of dist: every row of the column is one result row */
+    sqlite3_int64 *count, *key;
+    sqlite3_int64 ngroups, stride;
+    sqlite3_int64 g, j;            /* the current row: row j of group g; a stream starts at j = -1, the reference's (0, 0.0) row */
+    int max_index;                 /* carried from one xFilter to the next, as the reference's cursor does (:1808-1813) */
 } scan_cursor;
 
 /* ------------------------------------------------------------------------------------------------ helpers */
@@ -1123,31 +1127,101 @@ static int stage_full_column(scan_vtab *vt, vcolumn *v) {
     return SQLITE_OK;
 }
 
-/* ------------------------------------------------------------------------------------------------ virtual tables */
-static int connect_vtab(sqlite3 *db, void *aux, const char *schema, int filtered, sqlite3_vtab **out) {
-    int rc = sqlite3_declare_vtab(db, schema);
+/* ------------------------------------------------------------------------------------------------ virtual tables
+ * Every table-valued function is one row of `modules`: the column it scans, one query or many, its hidden arguments after
+ * memidx and its operation.  One xConnect, xFilter and cursor serve them all (vCursorFilterCommon, :1723-1826).  The reference
+ * has vector_full_scan / vector_quantize_scan (tbl, col, vector, k) and their *_stream twins (tbl, col, vector); the rest are
+ * additions without a counterpart there:
+ *
+ * vector_*_scan_batch(tbl, col, vectors, k): B queries in one call.  `vectors` is a BLOB of B x dimension elements of the column's
+ *   type back to back, or a flat JSON array of B x dimension numbers.  Rows are (query, id, distance) with query = 0 .. B-1, each
+ *   query's rows exactly those of the single-query function in the same order.  B >= 16 on F16/BF16/INT8/UINT8 data is scored on
+ *   the tensor cores, except L1, which is batched on the CUDA cores for every column type (FLOAT32 too).
+ * vector_*_scan_filtered(tbl, col, vector, k, rowids) / vector_*_scan_batch_filtered(tbl, col, vectors, k, rowids): the k nearest
+ *   among the rows whose rowid is in `rowids`, a BLOB of little-endian int64 (vector_rowid_set builds it): the results of the
+ *   unfiltered function over a table holding only those rows (vsb_group_scan_topk_filtered).
+ * vector_*_scan_batch_sets(tbl, col, vectors, k, sets, query_sets): query b's k nearest among the rows of its own set.  `sets` is a
+ *   BLOB of little-endian (int64 set, int64 rowid) pairs (vector_rowid_sets builds it); `query_sets` a BLOB of nq int64 set indexes
+ *   (vector_rowid_set builds it), or NULL: query b uses set b.  Set indexes may be sparse; one that no pair names is an empty set.
+ *   Each query's rows equal vector_*_scan_batch_filtered with that query's set (vsb_group_scan_topk_sets, DESIGN §3.14).
+ * vector_*_scan_grouped(tbl, col, vector, k, groups, limit): each key's k nearest rows for the `limit` best keys (NULL or 0: every
+ *   key with a row), keys ranked by their first row's distance, then its scan position, then the key.  `groups` is a BLOB of
+ *   little-endian (int64 key, int64 rowid) pairs (vector_rowid_sets builds it); keys may be sparse.  Rows are (key, id, distance),
+ *   keys in rank order and each key's rows exactly those of vector_*_scan_filtered with that key's rowids
+ *   (vsb_group_scan_topk_grouped, DESIGN §3.15).  The reference answers it with row_number() OVER (PARTITION BY key ORDER BY
+ *   distance) over vector_*_scan_stream.
+ * vector_*_scan_range(tbl, col, vector, radius) and the *_range_filtered twins (+ rowids): every row with distance < radius,
+ *   ordered by distance, equal distances in scan order (vsb_group_scan_range).  The reference answers this only as
+ *   SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < radius ORDER BY distance: the same rows, here without a
+ *   pass of every row through the VM.  For vector_quantize_scan_range the radius is in the units vector_quantize_scan reports.
+ *   The radius takes the hidden column `k`.
+ * vector_quantize_scan_rerank(tbl, col, vector, k, candidates) / vector_quantize_scan_rerank_batch(tbl, col, vectors, k,
+ *   candidates): the top `candidates` rows of the quantized column, reranked by their raw-column distance.  The single function
+ *   returns row for row what
+ *     SELECT id, distance FROM vector_full_scan_filtered(tbl, col, vector, k,
+ *         (SELECT vector_rowid_set(id) FROM vector_quantize_scan(tbl, col, vector, candidates)))
+ *   returns, but the rerank reads only the candidate rows of the raw column (vsb_group_scan_topk_rows) instead of all of it.  The
+ *   batch function returns (query, id, distance), each query's rows those of the single function.  Distances are raw-column
+ *   distances.  candidates may be smaller than k (fewer rows come back) or 0 (no rows). */
+enum { OP_TOPK, OP_STREAM, OP_RANGE, OP_SETS, OP_GROUPED, OP_RERANK };
+enum { ARG_NONE, ARG_TEXT, ARG_VECTOR, ARG_K, ARG_RADIUS, ARG_ROWIDS, ARG_SETS, ARG_QUERY_SETS, ARG_GROUPS, ARG_LIMIT, ARG_CANDIDATES };
+
+struct module_def {
+    const char *name, *schema;
+    int quantized;                 /* scans the quantized column (rerank: for its candidates, then the raw column) */
+    int many;                      /* `vector` holds B x dimension queries: one group of result rows per query */
+    int hidden[2];                 /* the arguments after memidx (ARG_NONE: none) */
+    int op;                        /* top-k (filtered: with rowids, batch: many), stream, range, sets, grouped or rerank */
+};
+
+#define SCHEMA(cols) "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, " cols ");"
+static const module_def modules[] = {
+    {"vector_full_scan", SCHEMA("id, distance"), 0, 0, {ARG_NONE}, OP_TOPK},
+    {"vector_quantize_scan", SCHEMA("id, distance"), 1, 0, {ARG_NONE}, OP_TOPK},
+    {"vector_full_scan_stream", SCHEMA("id, distance"), 0, 0, {ARG_NONE}, OP_STREAM},
+    {"vector_quantize_scan_stream", SCHEMA("id, distance"), 1, 0, {ARG_NONE}, OP_STREAM},
+    {"vector_full_scan_batch", SCHEMA("query, id, distance"), 0, 1, {ARG_NONE}, OP_TOPK},
+    {"vector_quantize_scan_batch", SCHEMA("query, id, distance"), 1, 1, {ARG_NONE}, OP_TOPK},
+    {"vector_full_scan_filtered", SCHEMA("rowids hidden, id, distance"), 0, 0, {ARG_ROWIDS}, OP_TOPK},
+    {"vector_quantize_scan_filtered", SCHEMA("rowids hidden, id, distance"), 1, 0, {ARG_ROWIDS}, OP_TOPK},
+    {"vector_full_scan_batch_filtered", SCHEMA("rowids hidden, query, id, distance"), 0, 1, {ARG_ROWIDS}, OP_TOPK},
+    {"vector_quantize_scan_batch_filtered", SCHEMA("rowids hidden, query, id, distance"), 1, 1, {ARG_ROWIDS}, OP_TOPK},
+    {"vector_full_scan_batch_sets", SCHEMA("sets hidden, query_sets hidden, query, id, distance"), 0, 1, {ARG_SETS, ARG_QUERY_SETS}, OP_SETS},
+    {"vector_quantize_scan_batch_sets", SCHEMA("sets hidden, query_sets hidden, query, id, distance"), 1, 1, {ARG_SETS, ARG_QUERY_SETS}, OP_SETS},
+    {"vector_full_scan_grouped", SCHEMA("groups hidden, \"limit\" hidden, key, id, distance"), 0, 0, {ARG_GROUPS, ARG_LIMIT}, OP_GROUPED},
+    {"vector_quantize_scan_grouped", SCHEMA("groups hidden, \"limit\" hidden, key, id, distance"), 1, 0, {ARG_GROUPS, ARG_LIMIT}, OP_GROUPED},
+    {"vector_full_scan_range", SCHEMA("id, distance"), 0, 0, {ARG_NONE}, OP_RANGE},
+    {"vector_quantize_scan_range", SCHEMA("id, distance"), 1, 0, {ARG_NONE}, OP_RANGE},
+    {"vector_full_scan_range_filtered", SCHEMA("rowids hidden, id, distance"), 0, 0, {ARG_ROWIDS}, OP_RANGE},
+    {"vector_quantize_scan_range_filtered", SCHEMA("rowids hidden, id, distance"), 1, 0, {ARG_ROWIDS}, OP_RANGE},
+    {"vector_quantize_scan_rerank", SCHEMA("candidates hidden, id, distance"), 1, 0, {ARG_CANDIDATES}, OP_RERANK},
+    {"vector_quantize_scan_rerank_batch", SCHEMA("candidates hidden, query, id, distance"), 1, 1, {ARG_CANDIDATES}, OP_RERANK},
+};
+#undef SCHEMA
+_Static_assert(sizeof modules / sizeof modules[0] == N_MODULES, "N_MODULES counts the rows of modules");
+
+static int nhidden(const module_def *m) { return (m->hidden[0] != ARG_NONE) + (m->hidden[1] != ARG_NONE); }
+/* many-query and grouped results lead each row with its query or key, and number the rows by their position in the result */
+static int leads_group(const module_def *m) { return m->many || m->op == OP_GROUPED; }
+
+static int vt_connect(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) { /* :1828-1842 */
+    (void)argc; (void)argv; (void)err;
+    const vmodule *mod = (const vmodule *)aux;
+    int rc = sqlite3_declare_vtab(db, mod->def->schema);
     if (rc != SQLITE_OK) return rc;
     scan_vtab *vt = (scan_vtab *)sqlite3_malloc((int)sizeof *vt);
     if (!vt) return SQLITE_NOMEM;
     memset(vt, 0, sizeof *vt);
     vt->db = db;
-    vt->ctx = (vcontext *)aux;
-    vt->filtered = filtered;
+    vt->ctx = mod->ctx;
+    vt->def = mod->def;
     *out = &vt->base;
     return SQLITE_OK;
-}
-static int vt_connect(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) { /* :1828-1842 */
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, id, distance);", 0, out);
-}
-static int vt_connect_filtered(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, rowids hidden, id, distance);", 1, out);
 }
 static int vt_disconnect(sqlite3_vtab *p) { sqlite3_free(p); return SQLITE_OK; }
 
 static void map_constraints(sqlite3_vtab *t, sqlite3_index_info *ii) { /* hidden column N -> argv[N] (:1856-1878) */
-    const int last_hidden = COL_MEMIDX + ((scan_vtab *)t)->filtered;
+    const int last_hidden = COL_MEMIDX + nhidden(((scan_vtab *)t)->def);
     for (int i = 0; i < ii->nConstraint; ++i) {
         const struct sqlite3_index_constraint *c = &ii->aConstraint[i];
         if (!c->usable || c->op != SQLITE_INDEX_CONSTRAINT_EQ) continue;
@@ -1157,7 +1231,14 @@ static void map_constraints(sqlite3_vtab *t, sqlite3_index_info *ii) { /* hidden
         }
     }
 }
+static int vt_best_index_stream(sqlite3_vtab *t, sqlite3_index_info *ii) { /* :2245-2275 */
+    ii->estimatedCost = 1e8;
+    ii->estimatedRows = 100000;
+    map_constraints(t, ii);
+    return SQLITE_OK;
+}
 static int vt_best_index(sqlite3_vtab *t, sqlite3_index_info *ii) { /* :1850-1880 */
+    if (((scan_vtab *)t)->def->op == OP_STREAM) return vt_best_index_stream(t, ii);
     ii->estimatedCost = 1.0;
     ii->estimatedRows = 100;
     ii->orderByConsumed = 1;
@@ -1165,12 +1246,7 @@ static int vt_best_index(sqlite3_vtab *t, sqlite3_index_info *ii) { /* :1850-188
     map_constraints(t, ii);
     return SQLITE_OK;
 }
-static int vt_best_index_stream(sqlite3_vtab *t, sqlite3_index_info *ii) { /* :2245-2275 */
-    ii->estimatedCost = 1e8;
-    ii->estimatedRows = 100000;
-    map_constraints(t, ii);
-    return SQLITE_OK;
-}
+
 static int vt_open(sqlite3_vtab *t, sqlite3_vtab_cursor **out) {
     (void)t;
     scan_cursor *c = (scan_cursor *)sqlite3_malloc((int)sizeof *c);
@@ -1179,34 +1255,56 @@ static int vt_open(sqlite3_vtab *t, sqlite3_vtab_cursor **out) {
     *out = &c->base;
     return SQLITE_OK;
 }
+static void cursor_free_result(scan_cursor *c) {
+    sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->fdist); sqlite3_free(c->count); sqlite3_free(c->key);
+    c->ids = 0; c->dist = 0; c->fdist = 0; c->count = 0; c->key = 0;
+}
 static int vt_close(sqlite3_vtab_cursor *cur) {
-    scan_cursor *c = (scan_cursor *)cur;
-    sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->sdist); sqlite3_free(c->sids); sqlite3_free(c->bcounts);
-    sqlite3_free(c->bkeys);
-    sqlite3_free(c);
+    cursor_free_result((scan_cursor *)cur);
+    sqlite3_free(cur);
     return SQLITE_OK;
+}
+/* the cursor's result arrays for `groups` groups of up to `stride` rows: float distances for a stream, a key per group for grouped */
+static int cursor_alloc(scan_cursor *c, sqlite3_int64 groups, sqlite3_int64 stride, int op) {
+    const sqlite3_uint64 ng = (sqlite3_uint64)(groups > 0 ? groups : 1), nr = ng * (sqlite3_uint64)(stride > 0 ? stride : 1);
+    cursor_free_result(c);
+    c->ids = (int64_t *)sqlite3_malloc64(nr * sizeof(int64_t));
+    if (op == OP_STREAM) c->fdist = (float *)sqlite3_malloc64(nr * sizeof(float));
+    else c->dist = (double *)sqlite3_malloc64(nr * sizeof(double));
+    c->count = (sqlite3_int64 *)sqlite3_malloc64(ng * sizeof(sqlite3_int64));
+    if (op == OP_GROUPED) c->key = (sqlite3_int64 *)sqlite3_malloc64(ng * sizeof(sqlite3_int64));
+    c->stride = stride;
+    return c->ids && (c->dist || c->fdist) && c->count && (c->key || op != OP_GROUPED) ? SQLITE_OK : SQLITE_NOMEM;
+}
+static void skip_empty(scan_cursor *c) {
+    while (c->g < c->ngroups && c->j >= c->count[c->g]) { ++c->g; c->j = 0; }
 }
 static int vt_next(sqlite3_vtab_cursor *cur) {
     scan_cursor *c = (scan_cursor *)cur;
-    if (c->streaming) ++c->spos; else ++c->row_index;
+    ++c->j;
+    skip_empty(c);
     return SQLITE_OK;
 }
 static int vt_eof(sqlite3_vtab_cursor *cur) {
-    scan_cursor *c = (scan_cursor *)cur;
-    return c->streaming ? (c->spos >= c->sn) : (c->row_index >= c->row_count);
+    const scan_cursor *c = (const scan_cursor *)cur;
+    return c->g >= c->ngroups;
 }
-static sqlite3_int64 cur_id(const scan_cursor *c) {
-    if (!c->streaming) return c->ids[c->row_index];
-    return c->spos < 0 ? 0 : c->sids[c->spos];          /* the reference's stream cursors emit (0, 0.0) first (SURVEY B.5) */
-}
+static sqlite3_int64 cur_id(const scan_cursor *c) { return c->j < 0 ? 0 : c->ids[c->g * c->stride + c->j]; }
 static int vt_column(sqlite3_vtab_cursor *cur, sqlite3_context *ctx, int col) { /* :2006-2014 */
-    scan_cursor *c = (scan_cursor *)cur;
-    col -= ((scan_vtab *)cur->pVtab)->filtered;
-    if (col == COL_ID) sqlite3_result_int64(ctx, cur_id(c));
-    else if (col == COL_DISTANCE) sqlite3_result_double(ctx, c->streaming ? (c->spos < 0 ? 0.0 : (double)c->sdist[c->spos]) : c->dist[c->row_index]);
+    const scan_cursor *c = (const scan_cursor *)cur;
+    const module_def *m = ((scan_vtab *)cur->pVtab)->def;
+    const sqlite3_int64 at = c->g * c->stride + c->j;
+    const int first = COL_MEMIDX + 1 + nhidden(m), lead = leads_group(m);     /* the visible columns: [query | key,] id, distance */
+    if (lead && col == first) sqlite3_result_int64(ctx, c->key ? c->key[c->g] : c->g);
+    else if (col == first + lead) sqlite3_result_int64(ctx, cur_id(c));
+    else if (col == first + lead + 1) sqlite3_result_double(ctx, c->j < 0 ? 0.0 : c->fdist ? (double)c->fdist[at] : c->dist[at]);
     return SQLITE_OK;
 }
-static int vt_rowid(sqlite3_vtab_cursor *cur, sqlite3_int64 *out) { *out = cur_id((scan_cursor *)cur); return SQLITE_OK; }
+static int vt_rowid(sqlite3_vtab_cursor *cur, sqlite3_int64 *out) {
+    const scan_cursor *c = (const scan_cursor *)cur;
+    *out = leads_group(((scan_vtab *)cur->pVtab)->def) ? c->g * c->stride + c->j : cur_id(c);
+    return SQLITE_OK;
+}
 
 /* the resident shard a scan runs on: the quantized column (staged from the shadow table on first use) or the raw column */
 static int resident_index(scan_vtab *vt, vcolumn *v, const char *tbl, const char *col, const char *fname, int quantized, vsb_group **out) {
@@ -1248,15 +1346,107 @@ static int resident_index(scan_vtab *vt, vcolumn *v, const char *tbl, const char
     return SQLITE_OK;
 }
 
-/* ------------------------------------------------------------------------------------------------ filtered scans
- * vector_*_scan_filtered(tbl, col, vector, k, rowids) / vector_*_scan_batch_filtered(tbl, col, vectors, k, rowids): the k nearest
- * among the rows whose rowid is in `rowids`, a BLOB of little-endian int64 (vector_rowid_set builds it).  No counterpart in the
- * reference; the results are those of the unfiltered function over a table holding only those rows (vsb_group_scan_topk_filtered). */
-static int check_rowids_arg(scan_vtab *vt, const char *fname, sqlite3_value *arg) {
-    const int t = sqlite3_value_type(arg);
-    if (t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument 5 must be of type BLOB (got %s).", fname, sql_type_name(t));
-    if (sqlite3_value_bytes(arg) % 8 != 0)
-        return vtab_error(&vt->base, "%s: rowids has %d bytes, expected a multiple of 8 (int64 rowids).", fname, sqlite3_value_bytes(arg));
+/* ------------------------------------------------------------------------------------------------ arguments */
+static int arg_kind(const module_def *m, int i) {
+    if (i < 2) return ARG_TEXT;
+    if (i == 2) return ARG_VECTOR;
+    if (i == 3) return m->op == OP_STREAM ? ARG_NONE : m->op == OP_RANGE ? ARG_RADIUS : ARG_K;
+    return m->hidden[i - 4];
+}
+static int check_multiple(scan_vtab *vt, const char *fname, sqlite3_value *a, const char *what, int multiple, const char *unit) {
+    if (sqlite3_value_bytes(a) % multiple == 0) return SQLITE_OK;
+    return vtab_error(&vt->base, "%s: %s has %d bytes, expected a multiple of %d (%s).", fname, what, sqlite3_value_bytes(a), multiple, unit);
+}
+/* every check of argument i that needs no other argument: its SQL type, a BLOB's size, a count's range */
+static int check_arg(scan_vtab *vt, const char *fname, int kind, int i, sqlite3_value *a) {
+#define T(t) (1 << SQLITE_##t)
+    static const struct { int types; const char *names; } accepts[] = {
+        [ARG_TEXT] = {T(TEXT), "TEXT"},          [ARG_VECTOR] = {T(TEXT) | T(BLOB), "TEXT or BLOB"},
+        [ARG_K] = {T(INTEGER), "INTEGER"},       [ARG_RADIUS] = {T(INTEGER) | T(FLOAT), "INTEGER or FLOAT"},
+        [ARG_ROWIDS] = {T(BLOB), "BLOB"},        [ARG_SETS] = {T(BLOB), "BLOB"},
+        [ARG_QUERY_SETS] = {T(BLOB) | T(NULL), "BLOB or NULL"}, [ARG_GROUPS] = {T(BLOB), "BLOB"},
+        [ARG_LIMIT] = {T(INTEGER) | T(NULL), "INTEGER or NULL"}, [ARG_CANDIDATES] = {T(INTEGER), "INTEGER"},
+    };
+#undef T
+    const int t = sqlite3_value_type(a);
+    if (!(accepts[kind].types & (1 << t)))
+        return vtab_error(&vt->base, "%s: argument %d must be of type %s (got %s).", fname, i + 1, accepts[kind].names, sql_type_name(t));
+    switch (kind) {
+    case ARG_K:
+        if (sqlite3_value_int(a) < 0) return vtab_error(&vt->base, "%s: k must not be negative.", fname);
+        break;
+    case ARG_LIMIT:
+        if (t == SQLITE_INTEGER && sqlite3_value_int64(a) < 0) return vtab_error(&vt->base, "%s: limit must not be negative.", fname);
+        break;
+    case ARG_CANDIDATES:
+        if (sqlite3_value_int64(a) < 0 || sqlite3_value_int64(a) > INT32_MAX)
+            return vtab_error(&vt->base, "%s: candidates must be between 0 and %d.", fname, INT32_MAX);
+        break;
+    case ARG_ROWIDS: return check_multiple(vt, fname, a, "rowids", 8, "int64 rowids");
+    case ARG_SETS: return check_multiple(vt, fname, a, "sets", 16, "int64 set, int64 rowid pairs");
+    case ARG_QUERY_SETS: return t == SQLITE_NULL ? SQLITE_OK : check_multiple(vt, fname, a, "query_sets", 8, "int64 set indexes");
+    case ARG_GROUPS: return check_multiple(vt, fname, a, "groups", 16, "int64 key, int64 rowid pairs");
+    }
+    return SQLITE_OK;
+}
+
+/* an xFilter call once its arguments have passed: the column, its resident copy and the queries */
+typedef struct {
+    vcolumn *v;
+    vsb_group *ix;                 /* the resident column of the module (rerank: the quantized one) */
+    const uint8_t *raw;            /* nq queries of the column's type */
+    const void *query;             /* the queries ix is scanned with: raw, or quantized for the quantized column */
+    int nq, k;
+    void *owned;                   /* queries decoded from JSON */
+    uint8_t *qq;                   /* quantized queries */
+} scan_call;
+
+/* the checks of a call in one order for every module: the argument count, each argument on its own in position order, the
+ * context, the queries against the column, query_sets against the queries, then the quantization table and staging
+ * (resident_index); then every query is quantized for a quantized column.  The caller frees owned and qq whatever this returns. */
+static int parse_call(scan_vtab *vt, const module_def *m, int argc, sqlite3_value **argv, scan_call *q) {
+    const char *fname = m->name;
+    memset(q, 0, sizeof *q);
+    const int nargs = m->op == OP_STREAM ? 3 : 4 + nhidden(m);
+    if (argc != nargs) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, nargs, argc);
+    for (int i = 0; i < argc; ++i) {
+        int rc = check_arg(vt, fname, arg_kind(m, i), i, argv[i]);
+        if (rc != SQLITE_OK) return rc;
+    }
+    const char *tbl = (const char *)sqlite3_value_text(argv[0]);
+    const char *col = (const char *)sqlite3_value_text(argv[1]);
+    vcolumn *v = q->v = ctx_find(vt->ctx, tbl, col);
+    if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
+
+    const int need = v->dim * elem_size(v->vtype);
+    int bytes = 0;
+    if (sqlite3_value_type(argv[2]) == SQLITE_TEXT) {
+        q->owned = json_to_blob(0, &vt->base, v->vtype, (const char *)sqlite3_value_text(argv[2]), &bytes, m->many ? 0 : v->dim);
+        if (!q->owned) return SQLITE_ERROR;
+        q->raw = (const uint8_t *)q->owned;
+    } else {
+        q->raw = (const uint8_t *)sqlite3_value_blob(argv[2]);
+        bytes = sqlite3_value_bytes(argv[2]);
+        if (!q->raw) return vtab_error(&vt->base, "%s: input vector%s cannot be NULL.", fname, m->many ? "s" : "");
+        /* the reference never checks the BLOB length (SURVEY B.7) and reads out of bounds; we refuse */
+        if (!m->many && bytes < need) return vtab_error(&vt->base, "%s: input vector has %d bytes, expected %d.", fname, bytes, need);
+    }
+    if (m->many && (bytes <= 0 || bytes % need != 0))
+        return vtab_error(&vt->base, "%s: input has %d bytes, expected a positive multiple of %d (dimension %d).", fname, bytes, need, v->dim);
+    const int nq = q->nq = m->many ? bytes / need : 1;
+    if (m->op == OP_SETS && sqlite3_value_type(argv[5]) == SQLITE_BLOB && sqlite3_value_bytes(argv[5]) / 8 != nq)
+        return vtab_error(&vt->base, "%s: query_sets holds %d set indexes for %d queries.", fname, sqlite3_value_bytes(argv[5]) / 8, nq);
+
+    int rc = resident_index(vt, v, tbl, col, fname, m->quantized, &q->ix);
+    if (rc != SQLITE_OK) return rc;
+    q->query = q->raw;
+    if (m->quantized) {                                                  /* quantize every query like vQuantRun does for one (:2162-2177) */
+        q->qq = (uint8_t *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)v->dim);
+        if (!q->qq) return SQLITE_NOMEM;
+        for (int b = 0; b < nq; ++b) quantize_vec(v->vtype, q->raw + (size_t)b * need, q->qq + (size_t)b * v->dim, v->offset, v->scale, v->dim, v->qtype);
+        q->query = q->qq;
+    }
+    q->k = arg_kind(m, 3) == ARG_K ? sqlite3_value_int(argv[3]) : 0;
     return SQLITE_OK;
 }
 
@@ -1274,647 +1464,206 @@ static int rowids_bitmap(scan_vtab *vt, const char *fname, sqlite3_value *arg, v
     return SQLITE_OK;
 }
 
-/* range scans (additions): vector_*_scan_range(tbl, col, vector, radius) and the *_range_filtered twins (+ rowids): every row with
- * distance < radius, ordered by distance, equal distances in scan order (vsb_group_scan_range).  The reference answers this only as
- * SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < radius ORDER BY distance: the same rows, here without a pass
- * of every row through the VM.  For vector_quantize_scan_range the radius is in the units vector_quantize_scan reports. */
-enum { SCAN_TOPK = 0, SCAN_STREAM = 1, SCAN_RANGE = 2 };
-
-/* the rows of a range scan into the cursor (its id / distance arrays, sized to the result) */
-static int range_rows(scan_vtab *vt, scan_cursor *c, const char *fname, vsb_group *ix, int metric, const void *query, double radius,
-                      const uint32_t *allow) {
-    vsb_range *res = 0;
-    if (vsb_group_scan_range(ix, metric, query, 1, &radius, allow, allow ? vsb_group_rows(ix) : 0, &res) != VSB_OK)
-        return vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
-    const int64_t *ids = 0;
-    const double *dist = 0;
-    int64_t n = 0;
-    vsb_range_get(res, 0, &ids, &dist, &n);
-    sqlite3_free(c->ids); sqlite3_free(c->dist);
-    c->k_alloc = 0;                                                      /* a later top-k call on this cursor allocates its own */
-    c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(sqlite3_int64));
-    c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(double));
-    const int rc = (c->ids && c->dist) ? SQLITE_OK : SQLITE_NOMEM;
-    if (rc == SQLITE_OK && n > 0) {
-        memcpy(c->ids, ids, (size_t)n * sizeof(int64_t));
-        memcpy(c->dist, dist, (size_t)n * sizeof(double));
-    }
-    c->row_count = rc == SQLITE_OK ? (int)n : 0;
-    vsb_range_free(res);
-    return rc;
-}
-
-/* common xFilter (vCursorFilterCommon, :1723-1826); filtered: the *_filtered twin, whose 5th argument is the rowid set */
-static int filter_common(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized, int mode) {
-    scan_cursor *c = (scan_cursor *)cur;
-    scan_vtab *vt = (scan_vtab *)cur->pVtab;
-    const int filtered = vt->filtered;
-    c->streaming = mode == SCAN_STREAM;
-    const int nargs = mode == SCAN_STREAM ? 3 : 4 + filtered;
-    if (argc != nargs) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, nargs, argc);
-    for (int i = 0; i < argc; ++i) {
-        int t = sqlite3_value_type(argv[i]);
-        if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 3 && mode == SCAN_RANGE && t != SQLITE_INTEGER && t != SQLITE_FLOAT)
-            return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER or FLOAT (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 3 && mode != SCAN_RANGE && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 4) { int rc = check_rowids_arg(vt, fname, argv[4]); if (rc != SQLITE_OK) return rc; }
-    }
-    const char *tbl = (const char *)sqlite3_value_text(argv[0]);
-    const char *col = (const char *)sqlite3_value_text(argv[1]);
-    vcolumn *v = ctx_find(vt->ctx, tbl, col);
-    if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
-
-    const int need = v->dim * elem_size(v->vtype);
-    void *owned = 0;
-    const void *query = 0;
-    if (sqlite3_value_type(argv[2]) == SQLITE_TEXT) {
-        int sz = 0;
-        owned = json_to_blob(0, &vt->base, v->vtype, (const char *)sqlite3_value_text(argv[2]), &sz, v->dim);
-        if (!owned) return SQLITE_ERROR;
-        query = owned;
-    } else {
-        query = sqlite3_value_blob(argv[2]);
-        if (!query) return vtab_error(&vt->base, "%s: input vector cannot be NULL.", fname);
-        /* the reference never checks the BLOB length (SURVEY B.7) and reads out of bounds; we refuse */
-        if (sqlite3_value_bytes(argv[2]) < need) return vtab_error(&vt->base, "%s: input vector has %d bytes, expected %d.", fname, sqlite3_value_bytes(argv[2]), need);
-    }
-    int rc = SQLITE_OK;
-    vsb_group *ix = 0;
-    uint8_t *qq = 0;
-    uint32_t *allow = 0;
-    rc = resident_index(vt, v, tbl, col, fname, quantized, &ix);
-    if (rc != SQLITE_OK) goto out;
-    if (quantized) {
-        qq = (uint8_t *)sqlite3_malloc(v->dim);                         /* quantize the query (:2162-2177) */
-        if (!qq) { rc = SQLITE_NOMEM; goto out; }
-        quantize_vec(v->vtype, query, qq, v->offset, v->scale, v->dim, v->qtype);
-        query = qq;
-    }
-
-    if (mode == SCAN_RANGE) {
-        c->row_index = 0;
-        c->row_count = 0;
-        if (filtered && (rc = rowids_bitmap(vt, fname, argv[4], ix, &allow)) != SQLITE_OK) goto out;
-        rc = range_rows(vt, c, fname, ix, v->metric, query, sqlite3_value_double(argv[3]), allow);
-        goto out;
-    }
-    if (mode == SCAN_STREAM) {
-        sqlite3_int64 n = vsb_group_rows(ix);
-        sqlite3_free(c->sdist); sqlite3_free(c->sids);
-        c->sdist = (float *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(float));
-        c->sids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * sizeof(sqlite3_int64));
-        if (!c->sdist || !c->sids) { rc = SQLITE_NOMEM; goto out; }
-        if (n > 0 && vsb_group_scan_all(ix, v->metric, query, c->sdist, (int64_t *)c->sids) != VSB_OK) { rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error()); goto out; }
-        c->sn = n;
-        c->spos = -1;
-        goto out;
-    }
-    {
-        int k = sqlite3_value_int(argv[3]);
-        if (k == 0) { rc = SQLITE_DONE; goto out; }                     /* :1795-1796 */
-        if (k < 0) { rc = vtab_error(&vt->base, "%s: k must not be negative.", fname); goto out; }
-        if (c->k_alloc != k) {                                          /* :1798-1806 */
-            sqlite3_free(c->ids); sqlite3_free(c->dist);
-            c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)k * sizeof(sqlite3_int64));
-            c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)k * sizeof(double));
-            if (!c->ids || !c->dist) { c->k_alloc = 0; rc = SQLITE_NOMEM; goto out; }
-            c->k_alloc = k;
-        }
-        c->row_index = 0;
-        c->row_count = 0;
-        int count = 0, src;
-        if (filtered) {
-            rc = rowids_bitmap(vt, fname, argv[4], ix, &allow);
-            if (rc != SQLITE_OK) goto out;
-            src = vsb_group_scan_topk_filtered(ix, v->metric, query, 1, k, allow, vsb_group_rows(ix), (int64_t *)c->ids, c->dist, &count, &c->max_index);
-        } else {
-            src = vsb_group_scan_topk(ix, v->metric, query, 1, k, (int64_t *)c->ids, c->dist, &count, &c->max_index);
-        }
-        if (src != VSB_OK) {
-            rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
-            goto out;
-        }
-        c->row_count = count;
-    }
-out:
-    sqlite3_free(owned);
-    sqlite3_free(qq);
-    sqlite3_free(allow);
-    return rc;
-}
-static int vt_filter_full(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan", 0, 0); }
-static int vt_filter_quant(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan", 1, 0); }
-static int vt_filter_full_stream(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan_stream", 0, 1); }
-static int vt_filter_quant_stream(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan_stream", 1, 1); }
-
-/* ------------------------------------------------------------------------------------------------ batched table-valued functions
- * vector_full_scan_batch(tbl, col, vectors, k) / vector_quantize_scan_batch(tbl, col, vectors, k): B query vectors in ONE call.
- * No counterpart in the reference (one vector per xFilter, :1774-1776); this is the SQL door to vsb_scan_topk's batch path:
- * `vectors` is a BLOB of B x dimension elements of the column's type back to back, or a flat JSON array of B x dimension
- * numbers.  Rows are (query, id, distance) with query = 0 .. B-1, each query's rows exactly those of the single-query function
- * in the same order.  B >= 16 on F16/BF16/INT8/UINT8 data is scored on the tensor cores, except L1, which is batched on the
- * CUDA cores for every column type (FLOAT32 too). */
-enum { BCOL_QUERY = 4, BCOL_ID = 5, BCOL_DISTANCE = 6 };
-
-static int vt_connect_batch(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, query, id, distance);", 0, out);
-}
-static int vt_connect_batch_filtered(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, rowids hidden, query, id, distance);", 1, out);
-}
-static int vt_connect_batch_sets(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, sets hidden, query_sets hidden, query, id, distance);", 2, out);
-}
-
-/* ------------------------------------------------------------------------------------------------ per-query sets
- * vector_*_scan_batch_sets(tbl, col, vectors, k, sets, query_sets): query b's k nearest among the rows of its own set.  `sets` is a
- * BLOB of little-endian (int64 set, int64 rowid) pairs (vector_rowid_sets builds it); `query_sets` a BLOB of nq int64 set indexes
- * (vector_rowid_set builds it), or NULL: query b uses set b.  Set indexes may be sparse; one that no pair names is an empty set.
- * Each query's rows equal vector_*_scan_batch_filtered with that query's set (vsb_group_scan_topk_sets, DESIGN §3.14). */
-static int check_sets_args(scan_vtab *vt, const char *fname, sqlite3_value *sets, sqlite3_value *qsets) {
-    int t = sqlite3_value_type(sets);
-    if (t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument 5 must be of type BLOB (got %s).", fname, sql_type_name(t));
-    if (sqlite3_value_bytes(sets) % 16 != 0)
-        return vtab_error(&vt->base, "%s: sets has %d bytes, expected a multiple of 16 (int64 set, int64 rowid pairs).", fname, sqlite3_value_bytes(sets));
-    t = sqlite3_value_type(qsets);
-    if (t != SQLITE_BLOB && t != SQLITE_NULL)
-        return vtab_error(&vt->base, "%s: argument 6 must be of type BLOB or NULL (got %s).", fname, sql_type_name(t));
-    if (t == SQLITE_BLOB && sqlite3_value_bytes(qsets) % 8 != 0)
-        return vtab_error(&vt->base, "%s: query_sets has %d bytes, expected a multiple of 8 (int64 set indexes).", fname, sqlite3_value_bytes(qsets));
-    return SQLITE_OK;
-}
-
 static int cmp_i64(const void *a, const void *b) {
     const int64_t x = *(const int64_t *)a, y = *(const int64_t *)b;
     return x < y ? -1 : x > y;
 }
-static int cmp_pair(const void *a, const void *b) { return cmp_i64(a, b); }   /* (set, rowid) pairs by set */
+
+/* the (int64 key, int64 rowid) pairs of a (checked) sets / groups BLOB by key: its nkeys distinct keys ascending, key i's rowids at
+ * [offsets[i], offsets[i + 1]) of rowids (pair_runs_free) */
+typedef struct {
+    int64_t *keys, *offsets, *rowids;
+    sqlite3_int64 nkeys;
+} pair_runs;
+static void pair_runs_free(pair_runs *r) { sqlite3_free(r->keys); sqlite3_free(r->offsets); sqlite3_free(r->rowids); }
+static int pairs_by_key(sqlite3_value *arg, pair_runs *r) {
+    const sqlite3_int64 npairs = sqlite3_value_bytes(arg) / 16;
+    const sqlite3_uint64 room = (sqlite3_uint64)(npairs > 0 ? npairs : 1);
+    int64_t *pairs = (int64_t *)sqlite3_malloc64(room * 16);
+    r->keys = (int64_t *)sqlite3_malloc64(room * sizeof(int64_t));
+    r->offsets = (int64_t *)sqlite3_malloc64((room + 1) * sizeof(int64_t));
+    r->rowids = (int64_t *)sqlite3_malloc64(room * sizeof(int64_t));
+    r->nkeys = 0;
+    const int rc = (pairs && r->keys && r->offsets && r->rowids) ? SQLITE_OK : SQLITE_NOMEM;
+    if (rc == SQLITE_OK) {
+        if (npairs > 0) memcpy(pairs, sqlite3_value_blob(arg), (size_t)npairs * 16);   /* little-endian host */
+        qsort(pairs, (size_t)npairs, 16, cmp_i64);                                     /* by key, a pair's first int64 */
+        for (sqlite3_int64 i = 0; i < npairs; ++i) {
+            if (r->nkeys == 0 || r->keys[r->nkeys - 1] != pairs[2 * i]) {
+                r->offsets[r->nkeys] = i;
+                r->keys[r->nkeys++] = pairs[2 * i];
+            }
+            r->rowids[i] = pairs[2 * i + 1];
+        }
+        r->offsets[r->nkeys] = npairs;
+    }
+    sqlite3_free(pairs);
+    return rc;
+}
 
 /* the sets the nq queries name, as dense bitmaps over the resident column ix (*bits: nsets x (rows + 31) / 32 words) and each
- * query's dense set index (*soq); sqlite3_free both */
+ * query's dense set index (*soq); a named set without pairs is empty and pairs of unnamed sets are skipped; sqlite3_free both */
 static int sets_bitmaps(scan_vtab *vt, const char *fname, sqlite3_value *sets, sqlite3_value *qsets, int nq, vsb_group *ix,
                         uint32_t **bits, int32_t **soq, int *nsets) {
-    const sqlite3_int64 npairs = sqlite3_value_bytes(sets) / 16, rows = vsb_group_rows(ix), words = (rows + 31) / 32;
+    const sqlite3_int64 words = (vsb_group_rows(ix) + 31) / 32;
+    pair_runs r;
     int64_t *q = (int64_t *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int64_t));
     int64_t *keys = (int64_t *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int64_t));
-    int64_t *pairs = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * 16);
-    int64_t *ids = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * sizeof(int64_t));
     int32_t *dense = (int32_t *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int32_t));
     uint32_t *out = 0;
-    int rc = (q && keys && pairs && ids && dense) ? SQLITE_OK : SQLITE_NOMEM, n = 0;
+    int rc = pairs_by_key(sets, &r), n = 0;
+    if (rc == SQLITE_OK && !(q && keys && dense)) rc = SQLITE_NOMEM;
     if (rc != SQLITE_OK) goto done;
     for (int b = 0; b < nq; ++b) q[b] = sqlite3_value_type(qsets) == SQLITE_NULL ? b : ((const int64_t *)sqlite3_value_blob(qsets))[b];
     memcpy(keys, q, (size_t)nq * sizeof(int64_t));
     qsort(keys, (size_t)nq, sizeof(int64_t), cmp_i64);
     for (int b = 0; b < nq; ++b) if (n == 0 || keys[n - 1] != keys[b]) keys[n++] = keys[b];     /* distinct set indexes -> dense 0 .. n-1 */
     for (int b = 0; b < nq; ++b) dense[b] = (int32_t)((const int64_t *)bsearch(&q[b], keys, (size_t)n, sizeof(int64_t), cmp_i64) - keys);
-    if (npairs > 0) memcpy(pairs, sqlite3_value_blob(sets), (size_t)npairs * 16);   /* little-endian host */
-    qsort(pairs, (size_t)npairs, 16, cmp_pair);
     out = (uint32_t *)sqlite3_malloc64((sqlite3_uint64)(n > 0 ? n : 1) * (sqlite3_uint64)(words + 1) * sizeof(uint32_t));
     if (!out) { rc = SQLITE_NOMEM; goto done; }
-    for (sqlite3_int64 i = 0, d = 0; d < n; ++d) {                       /* pairs and keys both ascending by set */
-        while (i < npairs && pairs[2 * i] < keys[d]) ++i;
-        sqlite3_int64 m = 0;
-        for (; i < npairs && pairs[2 * i] == keys[d]; ++i) ids[m++] = pairs[2 * i + 1];
-        if (vsb_group_rowid_bitmap(ix, ids, m, out + d * words) < 0) { rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error()); goto done; }
+    for (int d = 0; d < n; ++d) {
+        const int64_t *run = (const int64_t *)bsearch(&keys[d], r.keys, (size_t)r.nkeys, sizeof(int64_t), cmp_i64);
+        const sqlite3_int64 i = run ? run - r.keys : 0, m = run ? r.offsets[i + 1] - r.offsets[i] : 0;
+        if (vsb_group_rowid_bitmap(ix, r.rowids + (run ? r.offsets[i] : 0), m, out + d * words) < 0) {
+            rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
+            goto done;
+        }
     }
 done:
-    sqlite3_free(q); sqlite3_free(keys); sqlite3_free(pairs); sqlite3_free(ids);
+    pair_runs_free(&r);
+    sqlite3_free(q); sqlite3_free(keys);
     if (rc != SQLITE_OK) { sqlite3_free(out); sqlite3_free(dense); return rc; }
     *bits = out; *soq = dense; *nsets = n;
     return SQLITE_OK;
 }
 
-static void batch_skip_empty(scan_cursor *c) {
-    while (c->bq < c->bnq && c->bj >= c->bcounts[c->bq]) { ++c->bq; c->bj = 0; }
-}
-static int vt_next_batch(sqlite3_vtab_cursor *cur) {
-    scan_cursor *c = (scan_cursor *)cur;
-    ++c->bj;
-    batch_skip_empty(c);
-    return SQLITE_OK;
-}
-static int vt_eof_batch(sqlite3_vtab_cursor *cur) {
-    scan_cursor *c = (scan_cursor *)cur;
-    return c->bq >= c->bnq;
-}
-static int vt_column_batch(sqlite3_vtab_cursor *cur, sqlite3_context *ctx, int col) {
-    scan_cursor *c = (scan_cursor *)cur;
-    const size_t at = (size_t)c->bq * (size_t)c->bk + (size_t)c->bj;
-    col -= ((scan_vtab *)cur->pVtab)->filtered;
-    if (col == BCOL_QUERY && c->bkeys) sqlite3_result_int64(ctx, c->bkeys[c->bq]);
-    else if (col == BCOL_QUERY) sqlite3_result_int(ctx, c->bq);
-    else if (col == BCOL_ID) sqlite3_result_int64(ctx, c->ids[at]);
-    else if (col == BCOL_DISTANCE) sqlite3_result_double(ctx, c->dist[at]);
-    return SQLITE_OK;
-}
-static int vt_rowid_batch(sqlite3_vtab_cursor *cur, sqlite3_int64 *out) {
-    scan_cursor *c = (scan_cursor *)cur;
-    *out = (sqlite3_int64)c->bq * (sqlite3_int64)c->bk + c->bj;     /* position in the result, unique per row */
-    return SQLITE_OK;
-}
-static int filter_batch(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized) {
+/* ------------------------------------------------------------------------------------------------ xFilter */
+static int vt_filter(sqlite3_vtab_cursor *cur, int idxnum, const char *idxstr, int argc, sqlite3_value **argv) {
+    (void)idxnum; (void)idxstr;
     scan_cursor *c = (scan_cursor *)cur;
     scan_vtab *vt = (scan_vtab *)cur->pVtab;
-    const int filtered = vt->filtered;
-    c->batch = 1;
-    c->bnq = 0; c->bq = 0; c->bj = 0;
-    if (argc != 4 + filtered) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, 4 + filtered, argc);
-    for (int i = 0; i < argc; ++i) {
-        int t = sqlite3_value_type(argv[i]);
-        if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 4 && filtered == 1) { int rc = check_rowids_arg(vt, fname, argv[4]); if (rc != SQLITE_OK) return rc; }
-        if (i == 4 && filtered == 2) { int rc = check_sets_args(vt, fname, argv[4], argv[5]); if (rc != SQLITE_OK) return rc; }
-    }
-    const char *tbl = (const char *)sqlite3_value_text(argv[0]);
-    const char *col = (const char *)sqlite3_value_text(argv[1]);
-    vcolumn *v = ctx_find(vt->ctx, tbl, col);
-    if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
-    const int need = v->dim * elem_size(v->vtype);
-    uint32_t *setbits = 0;
+    const module_def *m = vt->def;
+    const char *fname = m->name;
+    c->ngroups = 0; c->g = 0; c->j = 0;
+    scan_call q;
+    int rc = parse_call(vt, m, argc, argv, &q), src = VSB_OK, nsets = 0;
+    sqlite3_int64 ngroups = 1;
+    uint32_t *allow = 0, *setbits = 0;
     int32_t *soq = 0;
-    void *owned = 0;
-    const uint8_t *queries = 0;
-    int bytes = 0;
-    if (sqlite3_value_type(argv[2]) == SQLITE_TEXT) {
-        owned = json_to_blob(0, &vt->base, v->vtype, (const char *)sqlite3_value_text(argv[2]), &bytes, 0);
-        if (!owned) return SQLITE_ERROR;
-        queries = (const uint8_t *)owned;
-    } else {
-        queries = (const uint8_t *)sqlite3_value_blob(argv[2]);
-        bytes = sqlite3_value_bytes(argv[2]);
-        if (!queries) return vtab_error(&vt->base, "%s: input vectors cannot be NULL.", fname);
-    }
-    int rc = SQLITE_OK;
-    uint8_t *qq = 0;
-    uint32_t *allow = 0;
-    vsb_group *ix = 0;
-    if (bytes <= 0 || bytes % need != 0) {
-        rc = vtab_error(&vt->base, "%s: input has %d bytes, expected a positive multiple of %d (dimension %d).", fname, bytes, need, v->dim);
-        goto out;
-    }
-    const int nq = bytes / need;
-    if (filtered == 2 && sqlite3_value_type(argv[5]) == SQLITE_BLOB && sqlite3_value_bytes(argv[5]) / 8 != nq) {
-        rc = vtab_error(&vt->base, "%s: query_sets holds %d set indexes for %d queries.", fname, sqlite3_value_bytes(argv[5]) / 8, nq);
-        goto out;
-    }
-    rc = resident_index(vt, v, tbl, col, fname, quantized, &ix);
-    if (rc != SQLITE_OK) goto out;
-    if (quantized) {                                                     /* quantize every query like vQuantRun does for one (:2162-2177) */
-        qq = (uint8_t *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)v->dim);
-        if (!qq) { rc = SQLITE_NOMEM; goto out; }
-        for (int b = 0; b < nq; ++b) quantize_vec(v->vtype, queries + (size_t)b * need, qq + (size_t)b * v->dim, v->offset, v->scale, v->dim, v->qtype);
-        queries = qq;
-    }
-    {
-        int k = sqlite3_value_int(argv[3]);
-        if (k == 0) { rc = SQLITE_OK; goto out; }                       /* empty result, like k = 0 of the single-query functions */
-        if (k < 0) { rc = vtab_error(&vt->base, "%s: k must not be negative.", fname); goto out; }
-        sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->bcounts);
-        c->k_alloc = 0;
-        c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)k * sizeof(sqlite3_int64));
-        c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)k * sizeof(double));
-        c->bcounts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
-        if (!c->ids || !c->dist || !c->bcounts) { rc = SQLITE_NOMEM; goto out; }
-        int src;
-        if (filtered == 2) {
-            int nsets = 0;
-            rc = sets_bitmaps(vt, fname, argv[4], argv[5], nq, ix, &setbits, &soq, &nsets);
-            if (rc != SQLITE_OK) goto out;
-            src = vsb_group_scan_topk_sets(ix, v->metric, queries, nq, k, setbits, nsets, vsb_group_rows(ix), soq, (int64_t *)c->ids, c->dist,
-                                           c->bcounts, 0);
-        } else if (filtered) {
-            rc = rowids_bitmap(vt, fname, argv[4], ix, &allow);
-            if (rc != SQLITE_OK) goto out;
-            src = vsb_group_scan_topk_filtered(ix, v->metric, queries, nq, k, allow, vsb_group_rows(ix), (int64_t *)c->ids, c->dist, c->bcounts, 0);
-        } else {
-            src = vsb_group_scan_topk(ix, v->metric, queries, nq, k, (int64_t *)c->ids, c->dist, c->bcounts, 0);
-        }
-        if (src != VSB_OK) {
-            rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
-            goto out;
-        }
-        c->bnq = nq;
-        c->bk = k;
-        batch_skip_empty(c);
-    }
-out:
-    sqlite3_free(owned);
-    sqlite3_free(qq);
-    sqlite3_free(allow);
-    sqlite3_free(setbits);
-    sqlite3_free(soq);
-    return rc;
-}
-static int vt_filter_full_batch(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_full_scan_batch", 0); }
-static int vt_filter_quant_batch(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_quantize_scan_batch", 1); }
-static sqlite3_module mod_full_batch = {0, 0, vt_connect_batch, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_full_batch, vt_next_batch,
-                                        vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-static sqlite3_module mod_quant_batch = {0, 0, vt_connect_batch, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch, vt_next_batch,
-                                         vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-static int vt_filter_full_batch_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_full_scan_batch_filtered", 0); }
-static int vt_filter_quant_batch_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_quantize_scan_batch_filtered", 1); }
-static sqlite3_module mod_full_batch_filtered = {0, 0, vt_connect_batch_filtered, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_full_batch_filtered,
-                                                 vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-static sqlite3_module mod_quant_batch_filtered = {0, 0, vt_connect_batch_filtered, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch_filtered,
-                                                  vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-static int vt_filter_full_batch_sets(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_full_scan_batch_sets", 0); }
-static int vt_filter_quant_batch_sets(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_batch(c, argc, argv, "vector_quantize_scan_batch_sets", 1); }
-static sqlite3_module mod_full_batch_sets = {0, 0, vt_connect_batch_sets, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_full_batch_sets,
-                                             vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-static sqlite3_module mod_quant_batch_sets = {0, 0, vt_connect_batch_sets, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_batch_sets,
-                                              vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-
-/* ------------------------------------------------------------------------------------------------ grouped scans
- * vector_*_scan_grouped(tbl, col, vector, k, groups, limit): each key's k nearest rows for the `limit` best keys (NULL or 0: every
- * key with a row), keys ranked by their first row's distance, then its scan position, then the key.  `groups` is a BLOB of
- * little-endian (int64 key, int64 rowid) pairs (vector_rowid_sets builds it); keys may be sparse.  Rows are (key, id, distance),
- * keys in rank order and each key's rows exactly those of vector_*_scan_filtered with that key's rowids (vsb_group_scan_topk_grouped,
- * DESIGN §3.15).  No counterpart in the reference, which answers it with row_number() OVER (PARTITION BY key ORDER BY distance)
- * over vector_*_scan_stream. */
-static int vt_connect_grouped(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, groups hidden, \"limit\" hidden, key, id, distance);", 2, out);
-}
-
-static int filter_grouped(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int quantized) {
-    scan_cursor *c = (scan_cursor *)cur;
-    scan_vtab *vt = (scan_vtab *)cur->pVtab;
-    c->batch = 1;
-    c->bnq = 0; c->bq = 0; c->bj = 0;
-    if (argc != 6) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, 6, argc);
-    for (int i = 0; i < argc; ++i) {
-        int t = sqlite3_value_type(argv[i]);
-        if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 4 && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument 5 must be of type BLOB (got %s).", fname, sql_type_name(t));
-        if (i == 4 && sqlite3_value_bytes(argv[4]) % 16 != 0)
-            return vtab_error(&vt->base, "%s: groups has %d bytes, expected a multiple of 16 (int64 key, int64 rowid pairs).", fname, sqlite3_value_bytes(argv[4]));
-        if (i == 5 && t != SQLITE_INTEGER && t != SQLITE_NULL) return vtab_error(&vt->base, "%s: argument 6 must be of type INTEGER or NULL (got %s).", fname, sql_type_name(t));
-        if (i == 5 && t == SQLITE_INTEGER && sqlite3_value_int64(argv[5]) < 0) return vtab_error(&vt->base, "%s: limit must not be negative.", fname);
-    }
-    const char *tbl = (const char *)sqlite3_value_text(argv[0]);
-    const char *col = (const char *)sqlite3_value_text(argv[1]);
-    vcolumn *v = ctx_find(vt->ctx, tbl, col);
-    if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
-    const int need = v->dim * elem_size(v->vtype);
-    void *owned = 0;
-    const void *query = 0;
-    if (sqlite3_value_type(argv[2]) == SQLITE_TEXT) {
-        int sz = 0;
-        owned = json_to_blob(0, &vt->base, v->vtype, (const char *)sqlite3_value_text(argv[2]), &sz, v->dim);
-        if (!owned) return SQLITE_ERROR;
-        query = owned;
-    } else {
-        query = sqlite3_value_blob(argv[2]);
-        if (!query) return vtab_error(&vt->base, "%s: input vector cannot be NULL.", fname);
-        if (sqlite3_value_bytes(argv[2]) < need) return vtab_error(&vt->base, "%s: input vector has %d bytes, expected %d.", fname, sqlite3_value_bytes(argv[2]), need);
-    }
-    const sqlite3_int64 npairs = sqlite3_value_bytes(argv[4]) / 16, lim64 = sqlite3_value_type(argv[5]) == SQLITE_NULL ? 0 : sqlite3_value_int64(argv[5]);
-    const int limit = lim64 > 0x7FFFFFFF ? 0 : (int)lim64;     /* a limit above every possible key count keeps every key */
-    int rc = SQLITE_OK, nkeys = 0;
-    uint8_t *qq = 0;
-    int64_t *pairs = 0, *rowids = 0, *offsets = 0, *keys = 0;
-    vsb_group *ix = 0;
+    int *counts = 0;                                                     /* rows of each query, as the top-k calls return them */
+    int64_t *qids = 0, *offsets = 0;
+    double *qdist = 0;
+    pair_runs runs = {0};
+    vsb_range *range = 0;
     vsb_grouped *res = 0;
-    const int k = sqlite3_value_int(argv[3]);
-    if (k < 0) { rc = vtab_error(&vt->base, "%s: k must not be negative.", fname); goto out; }
-    rc = resident_index(vt, v, tbl, col, fname, quantized, &ix);
     if (rc != SQLITE_OK) goto out;
-    if (quantized) {
-        qq = (uint8_t *)sqlite3_malloc(v->dim);
-        if (!qq) { rc = SQLITE_NOMEM; goto out; }
-        quantize_vec(v->vtype, query, qq, v->offset, v->scale, v->dim, v->qtype);
-        query = qq;
-    }
-    if (k == 0) goto out;                                                /* empty result, like k = 0 of the top-k functions */
-    pairs = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * 16);
-    rowids = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * sizeof(int64_t));
-    offsets = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs + 1) * sizeof(int64_t));
-    keys = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(npairs > 0 ? npairs : 1) * sizeof(int64_t));
-    if (!pairs || !rowids || !offsets || !keys) { rc = SQLITE_NOMEM; goto out; }
-    if (npairs > 0) memcpy(pairs, sqlite3_value_blob(argv[4]), (size_t)npairs * 16);   /* little-endian host */
-    qsort(pairs, (size_t)npairs, 16, cmp_pair);
-    offsets[0] = 0;
-    for (sqlite3_int64 i = 0; i < npairs; ++i) {                          /* distinct keys -> dense 0 .. nkeys-1, rowids in CSR form */
-        if (nkeys == 0 || keys[nkeys - 1] != pairs[2 * i]) {
-            if (nkeys > 0) offsets[nkeys] = i;
-            keys[nkeys++] = pairs[2 * i];
+    const int nq = q.nq, k = q.k, metric = q.v->metric;
+    if (arg_kind(m, 3) == ARG_K) {
+        if (k == 0) { rc = leads_group(m) ? SQLITE_OK : SQLITE_DONE; goto out; }   /* :1795-1796; the many-query and grouped modules: no rows */
+        if (m->op != OP_GROUPED) {                                      /* nq groups of up to k rows */
+            counts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
+            if ((rc = counts ? cursor_alloc(c, nq, k, m->op) : SQLITE_NOMEM) != SQLITE_OK) goto out;
+            ngroups = nq;
         }
-        rowids[i] = pairs[2 * i + 1];
     }
-    offsets[nkeys] = npairs;
-    if (vsb_group_scan_topk_grouped(ix, v->metric, query, 1, k, rowids, offsets, nkeys, limit, &res) != VSB_OK) {
-        rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
-        goto out;
+    if (m->hidden[0] == ARG_ROWIDS && (rc = rowids_bitmap(vt, fname, argv[4], q.ix, &allow)) != SQLITE_OK) goto out;
+    int *max_index = m->many ? 0 : &c->max_index;
+
+    switch (m->op) {
+    case OP_TOPK:
+        src = allow ? vsb_group_scan_topk_filtered(q.ix, metric, q.query, nq, k, allow, vsb_group_rows(q.ix), c->ids, c->dist, counts, max_index)
+                    : vsb_group_scan_topk(q.ix, metric, q.query, nq, k, c->ids, c->dist, counts, max_index);
+        break;
+    case OP_STREAM: {
+        const sqlite3_int64 n = vsb_group_rows(q.ix);
+        if ((rc = cursor_alloc(c, 1, n, m->op)) != SQLITE_OK) goto out;
+        if (n > 0) src = vsb_group_scan_all(q.ix, metric, q.query, c->fdist, c->ids);
+        c->count[0] = n;
+        c->j = -1;
+        break;
     }
-    {
+    case OP_RANGE: {
+        const double radius = sqlite3_value_double(argv[3]);
+        src = vsb_group_scan_range(q.ix, metric, q.query, 1, &radius, allow, allow ? vsb_group_rows(q.ix) : 0, &range);
+        if (src != VSB_OK) break;
+        const int64_t *ids = 0;
+        const double *dist = 0;
+        int64_t n = 0;
+        vsb_range_get(range, 0, &ids, &dist, &n);
+        if ((rc = cursor_alloc(c, 1, n, m->op)) != SQLITE_OK) goto out;
+        if (n > 0) {
+            memcpy(c->ids, ids, (size_t)n * sizeof(int64_t));
+            memcpy(c->dist, dist, (size_t)n * sizeof(double));
+        }
+        c->count[0] = n;
+        break;
+    }
+    case OP_SETS:
+        if ((rc = sets_bitmaps(vt, fname, argv[4], argv[5], nq, q.ix, &setbits, &soq, &nsets)) != SQLITE_OK) goto out;
+        src = vsb_group_scan_topk_sets(q.ix, metric, q.query, nq, k, setbits, nsets, vsb_group_rows(q.ix), soq, c->ids, c->dist, counts, 0);
+        break;
+    case OP_GROUPED: {
+        const sqlite3_int64 lim64 = sqlite3_value_type(argv[5]) == SQLITE_NULL ? 0 : sqlite3_value_int64(argv[5]);
+        const int limit = lim64 > 0x7FFFFFFF ? 0 : (int)lim64;         /* a limit above every possible key count keeps every key */
+        if ((rc = pairs_by_key(argv[4], &runs)) != SQLITE_OK) goto out;
+        src = vsb_group_scan_topk_grouped(q.ix, metric, q.query, 1, k, runs.rowids, runs.offsets, (int)runs.nkeys, limit, &res);
+        if (src != VSB_OK) break;
         int nk = 0;
         const int32_t *gk = 0;
         const int64_t *go = 0, *gi = 0;
         const double *gd = 0;
         vsb_grouped_get(res, 0, &nk, &gk, &go, &gi, &gd);
-        sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->bcounts); sqlite3_free(c->bkeys);
-        c->k_alloc = 0;
-        c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * (sqlite3_uint64)k * sizeof(sqlite3_int64));
-        c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * (sqlite3_uint64)k * sizeof(double));
-        c->bcounts = (int *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * sizeof(int));
-        c->bkeys = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)(nk > 0 ? nk : 1) * sizeof(sqlite3_int64));
-        if (!c->ids || !c->dist || !c->bcounts || !c->bkeys) { rc = SQLITE_NOMEM; goto out; }
+        if ((rc = cursor_alloc(c, nk, k, m->op)) != SQLITE_OK) goto out;
         for (int i = 0; i < nk; ++i) {
-            const int n = (int)(go[i + 1] - go[i]);
-            c->bcounts[i] = n;
-            c->bkeys[i] = keys[gk[i]];
+            const sqlite3_int64 n = go[i + 1] - go[i];
+            c->count[i] = n;
+            c->key[i] = runs.keys[gk[i]];
             memcpy(c->ids + (size_t)i * k, gi + go[i], (size_t)n * sizeof(int64_t));
             memcpy(c->dist + (size_t)i * k, gd + go[i], (size_t)n * sizeof(double));
         }
-        c->bnq = nk;
-        c->bk = k;
-        batch_skip_empty(c);
+        ngroups = nk;
+        break;
     }
-out:
-    vsb_grouped_free(res);
-    sqlite3_free(owned); sqlite3_free(qq);
-    sqlite3_free(pairs); sqlite3_free(rowids); sqlite3_free(offsets); sqlite3_free(keys);
-    return rc;
-}
-static int vt_filter_full_grouped(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_grouped(c, argc, argv, "vector_full_scan_grouped", 0); }
-static int vt_filter_quant_grouped(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_grouped(c, argc, argv, "vector_quantize_scan_grouped", 1); }
-static sqlite3_module mod_full_grouped = {0, 0, vt_connect_grouped, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_full_grouped,
-                                          vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-static sqlite3_module mod_quant_grouped = {0, 0, vt_connect_grouped, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_quant_grouped,
-                                           vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-
-#define SCAN_MODULE(NAME, CONNECT, BEST, FILTER)                                                                          \
-    static sqlite3_module NAME = {0, 0, CONNECT, BEST, vt_disconnect, 0, vt_open, vt_close, FILTER, vt_next, vt_eof, \
-                                  vt_column, vt_rowid, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}
-static int vt_filter_full_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan_filtered", 0, 0); }
-static int vt_filter_quant_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan_filtered", 1, 0); }
-SCAN_MODULE(mod_full, vt_connect, vt_best_index, vt_filter_full);
-SCAN_MODULE(mod_quant, vt_connect, vt_best_index, vt_filter_quant);
-SCAN_MODULE(mod_full_stream, vt_connect, vt_best_index_stream, vt_filter_full_stream);
-SCAN_MODULE(mod_quant_stream, vt_connect, vt_best_index_stream, vt_filter_quant_stream);
-SCAN_MODULE(mod_full_filtered, vt_connect_filtered, vt_best_index, vt_filter_full_filtered);
-SCAN_MODULE(mod_quant_filtered, vt_connect_filtered, vt_best_index, vt_filter_quant_filtered);
-static int vt_filter_full_range(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan_range", 0, SCAN_RANGE); }
-static int vt_filter_quant_range(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan_range", 1, SCAN_RANGE); }
-static int vt_filter_full_range_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_full_scan_range_filtered", 0, SCAN_RANGE); }
-static int vt_filter_quant_range_filtered(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_common(c, argc, argv, "vector_quantize_scan_range_filtered", 1, SCAN_RANGE); }
-/* the radius takes the hidden column `k` of the top-k schema (argument 4), the rowids the `rowids` column of the filtered one */
-SCAN_MODULE(mod_full_range, vt_connect, vt_best_index, vt_filter_full_range);
-SCAN_MODULE(mod_quant_range, vt_connect, vt_best_index, vt_filter_quant_range);
-SCAN_MODULE(mod_full_range_filtered, vt_connect_filtered, vt_best_index, vt_filter_full_range_filtered);
-SCAN_MODULE(mod_quant_range_filtered, vt_connect_filtered, vt_best_index, vt_filter_quant_range_filtered);
-
-/* ------------------------------------------------------------------------------------------------ reranked quantized scans
- * vector_quantize_scan_rerank(tbl, col, vector, k, candidates) / vector_quantize_scan_rerank_batch(tbl, col, vectors, k, candidates):
- * the top `candidates` rows of the quantized column, reranked by their raw-column distance.  No counterpart in the reference; the
- * single function returns row for row what
- *   SELECT id, distance FROM vector_full_scan_filtered(tbl, col, vector, k,
- *       (SELECT vector_rowid_set(id) FROM vector_quantize_scan(tbl, col, vector, candidates)))
- * returns, but the rerank reads only the candidate rows of the raw column (vsb_group_scan_topk_rows) instead of all of it.  The
- * batch function returns (query, id, distance), each query's rows those of the single function.  Distances are raw-column
- * distances.  candidates may be smaller than k (fewer rows come back) or 0 (no rows). */
-static int vt_connect_rerank(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, candidates hidden, id, distance);", 1, out);
-}
-static int vt_connect_rerank_batch(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) {
-    (void)argc; (void)argv; (void)err;
-    return connect_vtab(db, aux, "CREATE TABLE x(tbl hidden, vector hidden, k hidden, memidx hidden, candidates hidden, query, id, distance);", 1, out);
-}
-
-static int filter_rerank(sqlite3_vtab_cursor *cur, int argc, sqlite3_value **argv, const char *fname, int batch) {
-    scan_cursor *c = (scan_cursor *)cur;
-    scan_vtab *vt = (scan_vtab *)cur->pVtab;
-    if (batch) { c->batch = 1; c->bnq = 0; c->bq = 0; c->bj = 0; }
-    else { c->streaming = 0; c->row_index = 0; c->row_count = 0; }
-    if (argc != 5) return vtab_error(&vt->base, "%s expects %d arguments, but %d were provided.", fname, 5, argc);
-    for (int i = 0; i < argc; ++i) {
-        int t = sqlite3_value_type(argv[i]);
-        if (i < 2 && t != SQLITE_TEXT) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT (got %s).", fname, i + 1, sql_type_name(t));
-        if (i == 2 && t != SQLITE_TEXT && t != SQLITE_BLOB) return vtab_error(&vt->base, "%s: argument %d must be of type TEXT or BLOB (got %s).", fname, i + 1, sql_type_name(t));
-        if (i >= 3 && t != SQLITE_INTEGER) return vtab_error(&vt->base, "%s: argument %d must be of type INTEGER (got %s).", fname, i + 1, sql_type_name(t));
-    }
-    const char *tbl = (const char *)sqlite3_value_text(argv[0]);
-    const char *col = (const char *)sqlite3_value_text(argv[1]);
-    vcolumn *v = ctx_find(vt->ctx, tbl, col);
-    if (!v) return vtab_error(&vt->base, "%s: unable to retrieve context.", fname);
-    const int need = v->dim * elem_size(v->vtype);
-    void *owned = 0;
-    const uint8_t *queries = 0;
-    int bytes = 0;
-    if (sqlite3_value_type(argv[2]) == SQLITE_TEXT) {
-        owned = json_to_blob(0, &vt->base, v->vtype, (const char *)sqlite3_value_text(argv[2]), &bytes, batch ? 0 : v->dim);
-        if (!owned) return SQLITE_ERROR;
-        queries = (const uint8_t *)owned;
-    } else {
-        queries = (const uint8_t *)sqlite3_value_blob(argv[2]);
-        bytes = sqlite3_value_bytes(argv[2]);
-        if (!queries) return vtab_error(&vt->base, "%s: input vector%s cannot be NULL.", fname, batch ? "s" : "");
-        if (!batch && bytes < need) return vtab_error(&vt->base, "%s: input vector has %d bytes, expected %d.", fname, bytes, need);
-    }
-    int rc = SQLITE_OK, nq = 1;
-    uint8_t *qq = 0;
-    int64_t *qids = 0, *offsets = 0;
-    double *qdist = 0;
-    int *qcounts = 0;
-    vsb_group *qix = 0, *fix = 0;
-    if (batch) {
-        if (bytes <= 0 || bytes % need != 0) {
-            rc = vtab_error(&vt->base, "%s: input has %d bytes, expected a positive multiple of %d (dimension %d).", fname, bytes, need, v->dim);
-            goto out;
-        }
-        nq = bytes / need;
-    }
-    rc = resident_index(vt, v, tbl, col, fname, 1, &qix);
-    if (rc != SQLITE_OK) goto out;
-    qq = (uint8_t *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)v->dim);   /* quantize every query (:2162-2177) */
-    if (!qq) { rc = SQLITE_NOMEM; goto out; }
-    for (int b = 0; b < nq; ++b) quantize_vec(v->vtype, queries + (size_t)b * need, qq + (size_t)b * v->dim, v->offset, v->scale, v->dim, v->qtype);
-    {
-        const int k = sqlite3_value_int(argv[3]);
-        const sqlite3_int64 cand64 = sqlite3_value_int64(argv[4]);
-        if (k == 0) { rc = batch ? SQLITE_OK : SQLITE_DONE; goto out; }   /* as the single- and multi-query scans (:1795-1796) */
-        if (k < 0) { rc = vtab_error(&vt->base, "%s: k must not be negative.", fname); goto out; }
-        if (cand64 < 0 || cand64 > INT32_MAX) { rc = vtab_error(&vt->base, "%s: candidates must be between 0 and %d.", fname, INT32_MAX); goto out; }
-        const int cand = (int)cand64;
-        /* 1: the top `candidates` of the quantized column, every query from a fresh cursor, as the subquery of the composed statement */
-        qcounts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
+    case OP_RERANK: {
+        const int cand = (int)sqlite3_value_int64(argv[4]);
+        vsb_group *fix = 0;
+        /* 1: the top `candidates` of the quantized column, every query from a fresh cursor, as the subquery of the composed
+         * statement; counts holds each query's candidate count until step 2 */
         offsets = (int64_t *)sqlite3_malloc64((sqlite3_uint64)(nq + 1) * sizeof(int64_t));
         qids = (int64_t *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)(cand > 0 ? cand : 1) * sizeof(int64_t));
         qdist = (double *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)(cand > 0 ? cand : 1) * sizeof(double));
-        if (!qcounts || !offsets || !qids || !qdist) { rc = SQLITE_NOMEM; goto out; }
-        memset(qcounts, 0, (size_t)nq * sizeof(int));
-        if (cand > 0) {
-            int mi = 0;
-            if (vsb_group_scan_topk(qix, v->metric, qq, nq, cand, qids, qdist, qcounts, &mi) != VSB_OK) {
-                rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
-                goto out;
-            }
-        }
-        /* each query's candidate rowids, back to back */
-        offsets[0] = 0;
+        if (!offsets || !qids || !qdist) { rc = SQLITE_NOMEM; goto out; }
+        memset(counts, 0, (size_t)nq * sizeof(int));
+        int fresh = 0;
+        if (cand > 0 && (src = vsb_group_scan_topk(q.ix, metric, q.query, nq, cand, qids, qdist, counts, &fresh)) != VSB_OK) break;
+        offsets[0] = 0;                                                  /* each query's candidate rowids, back to back */
         for (int b = 0; b < nq; ++b) {
-            memmove(qids + offsets[b], qids + (size_t)b * (size_t)cand, (size_t)qcounts[b] * sizeof(int64_t));
-            offsets[b + 1] = offsets[b] + qcounts[b];
+            memmove(qids + offsets[b], qids + (size_t)b * (size_t)cand, (size_t)counts[b] * sizeof(int64_t));
+            offsets[b + 1] = offsets[b] + counts[b];
         }
         /* 2: the rerank on the raw column, reading only the candidate rows */
-        rc = resident_index(vt, v, tbl, col, fname, 0, &fix);
-        if (rc != SQLITE_OK) goto out;
-        int src;
-        if (batch) {
-            sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->bcounts);
-            c->k_alloc = 0;
-            c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)k * sizeof(sqlite3_int64));
-            c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)nq * (sqlite3_uint64)k * sizeof(double));
-            c->bcounts = (int *)sqlite3_malloc64((sqlite3_uint64)nq * sizeof(int));
-            if (!c->ids || !c->dist || !c->bcounts) { rc = SQLITE_NOMEM; goto out; }
-            src = vsb_group_scan_topk_rows(fix, v->metric, queries, nq, k, qids, offsets, (int64_t *)c->ids, c->dist, c->bcounts, 0);
-        } else {
-            if (c->k_alloc != k) {                                          /* :1798-1806 */
-                sqlite3_free(c->ids); sqlite3_free(c->dist);
-                c->ids = (sqlite3_int64 *)sqlite3_malloc64((sqlite3_uint64)k * sizeof(sqlite3_int64));
-                c->dist = (double *)sqlite3_malloc64((sqlite3_uint64)k * sizeof(double));
-                if (!c->ids || !c->dist) { c->k_alloc = 0; rc = SQLITE_NOMEM; goto out; }
-                c->k_alloc = k;
-            }
-            int count = 0;
-            src = vsb_group_scan_topk_rows(fix, v->metric, queries, 1, k, qids, offsets, (int64_t *)c->ids, c->dist, &count, &c->max_index);
-            if (src == VSB_OK) c->row_count = count;
-        }
-        if (src != VSB_OK) {
-            rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error());
+        if ((rc = resident_index(vt, q.v, (const char *)sqlite3_value_text(argv[0]), (const char *)sqlite3_value_text(argv[1]), fname, 0, &fix)) != SQLITE_OK)
             goto out;
-        }
-        if (batch) {
-            c->bnq = nq;
-            c->bk = k;
-            batch_skip_empty(c);
-        }
+        src = vsb_group_scan_topk_rows(fix, metric, q.raw, nq, k, qids, offsets, c->ids, c->dist, counts, max_index);
+        break;
     }
+    }
+    if (src != VSB_OK) { rc = vtab_error(&vt->base, "%s: %s", fname, vsb_last_error()); goto out; }
+    if (counts) for (int b = 0; b < nq; ++b) c->count[b] = counts[b];
+    c->ngroups = ngroups;
+    skip_empty(c);
 out:
-    sqlite3_free(owned);
-    sqlite3_free(qq);
-    sqlite3_free(qids);
-    sqlite3_free(qdist);
-    sqlite3_free(qcounts);
-    sqlite3_free(offsets);
+    sqlite3_free(q.owned); sqlite3_free(q.qq);
+    sqlite3_free(allow); sqlite3_free(setbits); sqlite3_free(soq); sqlite3_free(counts);
+    sqlite3_free(qids); sqlite3_free(qdist); sqlite3_free(offsets);
+    pair_runs_free(&runs);
+    vsb_range_free(range);
+    vsb_grouped_free(res);
     return rc;
 }
-static int vt_filter_rerank(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_rerank(c, argc, argv, "vector_quantize_scan_rerank", 0); }
-static int vt_filter_rerank_batch(sqlite3_vtab_cursor *c, int n, const char *s, int argc, sqlite3_value **argv) { (void)n; (void)s; return filter_rerank(c, argc, argv, "vector_quantize_scan_rerank_batch", 1); }
-SCAN_MODULE(mod_quant_rerank, vt_connect_rerank, vt_best_index, vt_filter_rerank);
-static sqlite3_module mod_quant_rerank_batch = {0, 0, vt_connect_rerank_batch, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter_rerank_batch,
-                                                vt_next_batch, vt_eof_batch, vt_column_batch, vt_rowid_batch, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+
+static const sqlite3_module scan_module = {0, 0, vt_connect, vt_best_index, vt_disconnect, 0, vt_open, vt_close, vt_filter, vt_next,
+                                           vt_eof, vt_column, vt_rowid, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 
 /* vector_rowid_set(x): aggregate of the non-NULL x as the rowids BLOB of the *_filtered modules (int64, host byte order =
  * little-endian), e.g. (SELECT vector_rowid_set(rowid) FROM docs WHERE lang = 'en'); no rows give an empty BLOB */
@@ -1988,30 +1737,12 @@ __attribute__((visibility("default"))) int sqlite3_vector_init(sqlite3 *db, char
         rc = sqlite3_create_function(db, fns[i].name, fns[i].nargs, SQLITE_UTF8, ctx, fns[i].fn, 0, 0);
         if (rc != SQLITE_OK) return rc;
     }
-    if ((rc = sqlite3_create_module(db, "vector_full_scan", &mod_full, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan", &mod_quant, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_stream", &mod_full_stream, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_stream", &mod_quant_stream, ctx)) != SQLITE_OK) return rc;
-    /* additions (not in the reference): batched scans */
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_batch", &mod_full_batch, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch", &mod_quant_batch, ctx)) != SQLITE_OK) return rc;
-    /* additions: filtered scans and the aggregate that builds their rowid set */
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_filtered", &mod_full_filtered, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_filtered", &mod_quant_filtered, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_batch_filtered", &mod_full_batch_filtered, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch_filtered", &mod_quant_batch_filtered, ctx)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_function(db, "vector_rowid_set", 1, SQLITE_UTF8, ctx, 0, rowid_set_step, rowid_set_final)) != SQLITE_OK) return rc;
     if ((rc = sqlite3_create_function(db, "vector_rowid_sets", 2, SQLITE_UTF8, ctx, 0, rowid_sets_step, rowid_sets_final)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_batch_sets", &mod_full_batch_sets, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_batch_sets", &mod_quant_batch_sets, ctx)) != SQLITE_OK) return rc;
-    /* additions: range scans */
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_grouped", &mod_full_grouped, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_grouped", &mod_quant_grouped, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_range", &mod_full_range, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range", &mod_quant_range, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_full_scan_range_filtered", &mod_full_range_filtered, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_range_filtered", &mod_quant_range_filtered, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_rerank", &mod_quant_rerank, ctx)) != SQLITE_OK) return rc;
-    if ((rc = sqlite3_create_module(db, "vector_quantize_scan_rerank_batch", &mod_quant_rerank_batch, ctx)) != SQLITE_OK) return rc;
+    for (int i = 0; i < N_MODULES; ++i) {
+        ctx->mods[i].def = &modules[i];
+        ctx->mods[i].ctx = ctx;
+        if ((rc = sqlite3_create_module(db, modules[i].name, &scan_module, &ctx->mods[i])) != SQLITE_OK) return rc;
+    }
     return SQLITE_OK;
 }

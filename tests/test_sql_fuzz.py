@@ -180,7 +180,14 @@ ARG_VALUES = ["NULL", "1", "-1", "0", "2.5", "'t'", "'e'", "'nope'", "''", "x''"
 ARG_SCALARS = [("vector_version", [0]), ("vector_backend", [0]), ("vector_init", [3]), ("vector_quantize", [2, 3]), ("vector_quantize_memory", [2]),
                ("vector_quantize_preload", [2]), ("vector_quantize_cleanup", [2])]
 ARG_TVFS = [("vector_full_scan", 4), ("vector_quantize_scan", 4), ("vector_full_scan_stream", 3), ("vector_quantize_scan_stream", 3),
-            ("vector_full_scan_batch", 4), ("vector_quantize_scan_batch", 4)]
+            ("vector_full_scan_batch", 4), ("vector_quantize_scan_batch", 4),
+            ("vector_full_scan_filtered", 5), ("vector_quantize_scan_filtered", 5),
+            ("vector_full_scan_batch_filtered", 5), ("vector_quantize_scan_batch_filtered", 5),
+            ("vector_full_scan_batch_sets", 6), ("vector_quantize_scan_batch_sets", 6),
+            ("vector_full_scan_grouped", 6), ("vector_quantize_scan_grouped", 6),
+            ("vector_full_scan_range", 4), ("vector_quantize_scan_range", 4),
+            ("vector_full_scan_range_filtered", 5), ("vector_quantize_scan_range_filtered", 5),
+            ("vector_quantize_scan_rerank", 5), ("vector_quantize_scan_rerank_batch", 5)]
 
 
 def _arg_stmt(rng):

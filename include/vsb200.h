@@ -163,12 +163,14 @@ VSB_API int vsb_scan_topk_rows(vsb_index *ix, int metric, const void *queries, i
  * Keys with at least one row are ranked by their first row's distance (ascending, -INF first), then that row's scan position,
  * then the key index; limit > 0 keeps the first limit keys, limit 0 every key with a row.  0 <= k <= 256 (k = 0: no keys; larger
  * k is VSB_EINVAL); nkeys >= 0; limit >= 0.  Queries are answered one after another, each from a fresh cursor.  Each shard lays
- * out its rows of every key once per call (more than 2^32 - 1 (key, row) pairs on one shard: VSB_ERANGE), then per query scans
+ * out its rows of every key once per call on the device (more than 2^32 - 1 (key, row) pairs on one shard: VSB_ERANGE); this is
+ * the one-call case of a grouping (vsb_grouping_create, which keeps the layout across calls).  Then per query each shard scans
  * every distance, walks every key in pieces of 1024 rows on the device, and copies to the host only the candidates of the keys
  * whose smallest distance over all shards is at or below the limit-th smallest (DESIGN §3.15).  A streamed index keeps the
  * distances of all its windows on the device (4 bytes per row, in vsb_index_device_bytes).  Counters: "grouped_queries",
  * "grouped_pairs" (the (key, row) pairs of the last layout), "grouped_cands" (candidates replayed), "grouped_keys_replayed" (on a
- * group's first shard), "grouped_regrows", "grouped_layout_us", and the device times "grouped_scan_us" (scans) and
+ * group's first shard), "grouped_regrows", "grouped_layout_us" (layouts built), "grouped_layout_reuses" (calls that ran on a
+ * grouping's kept layout), and the device times "grouped_scan_us" (scans) and
  * "grouped_walk_us" (walk, bounds and compaction) and the host time "grouped_replay_us" (on a group's first shard).  *out receives
  * a result owned by the caller (vsb_grouped_free); vsb_grouped_get borrows query q's arrays from it: nkeys_out keys in rank
  * order, key i's rows at [row_offsets[i], row_offsets[i + 1]) of rowids and dist. */
@@ -178,6 +180,19 @@ VSB_API int vsb_scan_topk_grouped(vsb_index *ix, int metric, const void *queries
 VSB_API int vsb_grouped_get(const vsb_grouped *r, int q, int *nkeys_out, const int32_t **keys, const int64_t **row_offsets /* nkeys_out + 1 */,
                             const int64_t **rowids, const double **dist); /* borrowed until free */
 VSB_API void vsb_grouped_free(vsb_grouped *r);
+
+/* ---- groupings: a layout of keys kept across grouped calls ------------------------------------------------------------------
+ * vsb_grouping_create lays out the keys (rowids, offsets, nkeys as for vsb_scan_topk_grouped, same checks and codes) on every
+ * shard of the column once; vsb_scan_topk_grouping then answers (metric, queries, nq, k, limit) on that layout and returns bit for
+ * bit what vsb_scan_topk_grouped returns with the same keys, arguments checked as there.  The layout does not depend on k; the
+ * per-call arrays are sized by the call's k and grown, never shrunk.  A call on a grouping whose column gained rows since it was
+ * made is VSB_EINVAL ("the column changed since the grouping was made").  Freeing the index or group detaches its groupings: every
+ * later call on one is VSB_EINVAL, and vsb_grouping_free still frees it.  A grouping is an owned handle (vsb_debug_live_handles);
+ * the planted "grouped_dist" and vsb_debug_read "grouped" apply to its calls as to vsb_scan_topk_grouped. */
+typedef struct vsb_grouping vsb_grouping;
+VSB_API int vsb_grouping_create(vsb_index *ix, const int64_t *rowids, const int64_t *offsets, int nkeys, vsb_grouping **out);
+VSB_API int vsb_scan_topk_grouping(vsb_grouping *gr, int metric, const void *queries, int nq, int k, int limit, vsb_grouped **out);
+VSB_API void vsb_grouping_free(vsb_grouping *gr);
 
 /* ---- range search: every row closer than a radius (no counterpart in the reference, whose stream modules answer it as
  * SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < r ORDER BY distance) --------------------------------------
@@ -338,6 +353,8 @@ VSB_API int vsb_group_scan_topk_rows(vsb_group *g, int metric, const void *queri
  * bound is taken from each key's minimum over all shards, and each key replays the shards' candidates in shard order */
 VSB_API int vsb_group_scan_topk_grouped(vsb_group *g, int metric, const void *queries, int nq, int k, const int64_t *rowids,
                                         const int64_t *offsets, int nkeys, int limit, vsb_grouped **out);
+/* vsb_grouping_create over the group's shards: one layout per shard (vsb_scan_topk_grouping answers on all of them) */
+VSB_API int vsb_group_grouping_create(vsb_group *g, const int64_t *rowids, const int64_t *offsets, int nkeys, vsb_grouping **out);
 /* vsb_scan_range over the group's global scan order (nbits = vsb_group_rows): every shard scans its rows, the shards' lists are
  * merged by (distance, global scan row) */
 VSB_API int vsb_group_scan_range(vsb_group *g, int metric, const void *queries, int nq, const double *radius, const uint32_t *allow,
@@ -400,7 +417,7 @@ VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches,
  * level, float [P][Q] the bound each piece was refined against, +INF for level 0), "large_k_batch_cands" (the same batch's
  * candidates: int64 query count Q, int64 [Q] each query's count (-1: answered alone), then the queries' (uint32 distance bits,
  * uint32 shard row) pairs in scan order, query after query), "grouped" (this shard's state after the most recent
- * vsb_scan_topk_grouped or group call with k > 0, keys and queries, for its last query (DESIGN §3.15): int64 [7] {P positions,
+ * vsb_scan_topk_grouped, vsb_scan_topk_grouping or group call with k > 0, keys and queries, for its last query (DESIGN §3.15): int64 [7] {P positions,
  * N pieces, G keys, k, D distances (the shard's rows; 0 without positions), S (1: the limit selected keys), C survivor pairs},
  * then uint32 rows [P] (shard row of each position), koff [G + 1], pstart [N + 1], pkey [N], kpiece [G + 1], float dist [D] (the
  * query's distances), pd [P] (d where the walk logged, NaN otherwise), lists [N][k], bound [N], kmin [G], uint32 [C][2]

@@ -7,6 +7,6 @@ This package is the thin host-side mirror used by tests and bench.py: ctypes bin
 torch.distributed row-shard driver (shard.py: one process per GPU; the heads travel over NVLink peer memory).
 There is no CPU fallback anywhere in this package.
 """
-from .api import Engine, Group, Index, VsbError, load_engine  # noqa: F401
+from .api import Engine, Group, Grouping, Index, VsbError, load_engine  # noqa: F401
 
 __all__ = ["Engine", "Group", "Index", "VsbError", "load_engine"]

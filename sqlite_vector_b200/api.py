@@ -3,6 +3,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import weakref
 
 import numpy as np
 
@@ -55,6 +56,9 @@ _SIGNATURES = {
     "vsb_scan_topk_grouped": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, C.POINTER(_vp)]),
     "vsb_grouped_get": (_i, [_vp, _i, C.POINTER(_i), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp)]),
     "vsb_grouped_free": (None, [_vp]),
+    "vsb_grouping_create": (_i, [_vp, _vp, _vp, _i, C.POINTER(_vp)]),
+    "vsb_scan_topk_grouping": (_i, [_vp, _i, _vp, _i, _i, _i, C.POINTER(_vp)]),
+    "vsb_grouping_free": (None, [_vp]),
     "vsb_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_range_get": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_i64)]),
     "vsb_range_free": (None, [_vp]),
@@ -89,6 +93,7 @@ _SIGNATURES = {
     "vsb_group_scan_topk_rows": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vsb_group_scan_topk_sets": (_i, [_vp, _i, _vp, _i, _i, _vp, _i, _i64, _vp, _vp, _vp, _vp, _vp]),
     "vsb_group_scan_topk_grouped": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _i, C.POINTER(_vp)]),
+    "vsb_group_grouping_create": (_i, [_vp, _vp, _vp, _i, C.POINTER(_vp)]),
     "vsb_group_scan_range": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i64, C.POINTER(_vp)]),
     "vsb_group_gpus": (_i, [_vp]),
     "vsb_group_rows": (_i64, [_vp]),
@@ -279,18 +284,29 @@ def _range(eng: "Engine", fn, h, rows: int, metric: int, queries: np.ndarray, ra
     return out
 
 
-def _grouped(eng: "Engine", fn, h, metric: int, queries: np.ndarray, k: int, key_lists, limit: int):
-    """the grouped entry points: fn(handle, metric, queries, nq, k, rowids, offsets, nkeys, limit, &result) -> rc; per query a list
-    of (key index, rowids, distances), keys in rank order"""
-    q = np.ascontiguousarray(queries)
-    q2 = q.reshape(-1, q.shape[-1]) if q.ndim > 1 else q.reshape(1, -1)
-    nq = q2.shape[0]
+def _key_csr(key_lists):
+    """one sequence of rowids per key -> (rowids, offsets) of the grouped entry points"""
     lists = [np.asarray(r, dtype=np.int64).reshape(-1) for r in key_lists]
     offsets = np.zeros(len(lists) + 1, dtype=np.int64)
     offsets[1:] = np.cumsum([len(r) for r in lists])
-    flat = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.int64))
+    return np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.int64)), offsets
+
+
+def _grouped(eng: "Engine", fn, h, metric: int, queries: np.ndarray, k: int, key_lists, limit: int):
+    """the grouped entry points: fn(handle, metric, queries, nq, k, rowids, offsets, nkeys, limit, &result) -> rc; per query a list
+    of (key index, rowids, distances), keys in rank order"""
+    flat, offsets = _key_csr(key_lists)
+    return _grouped_call(eng, lambda qp, nq, res: fn(h, metric, qp, nq, k, _ptr(flat), _ptr(offsets), len(offsets) - 1, limit, res),
+                         queries)
+
+
+def _grouped_call(eng: "Engine", call, queries: np.ndarray):
+    """call(queries, nq, &result) -> rc, and the result as _grouped returns it"""
+    q = np.ascontiguousarray(queries)
+    q2 = q.reshape(-1, q.shape[-1]) if q.ndim > 1 else q.reshape(1, -1)
+    nq = q2.shape[0]
     res = _vp()
-    eng.check(fn(h, metric, _ptr(q2), nq, k, _ptr(flat), _ptr(offsets), len(lists), limit, C.byref(res)))
+    eng.check(call(_ptr(q2), nq, C.byref(res)))
     out = []
     try:
         for b in range(nq):
@@ -370,6 +386,15 @@ class _Column:
         the key index) and cut to `limit` (0: every key with a row); each key's rows equal scan_topk_filtered with its rowids"""
         return _grouped(self.eng, self._fn("scan_topk_grouped"), self.h, metric, queries, k, key_lists, limit)
 
+    def grouping(self, key_lists) -> "Grouping":
+        """the keys laid out once for many grouped calls (vsb_grouping_create): Grouping.scan_topk answers as scan_topk_grouped
+        with these key_lists.  The column's close() closes its groupings first"""
+        return Grouping(self, key_lists)
+
+    def _close_groupings(self):
+        for g in list(getattr(self, "_groupings", ())):
+            g.close()
+
     def scan_range(self, metric: int, queries: np.ndarray, radius, allow=None):
         """every row with distance < radius (vsb_scan_range), for one query or a batch; radius: one value or one per query, allow:
         None, a boolean mask over the scan-order rows or a uint32 row bitmap.  Returns one (rowids, distances) pair per query"""
@@ -407,6 +432,7 @@ class Index(_Column):
 
     def close(self):
         if getattr(self, "h", None):
+            self._close_groupings()
             self.eng.lib.vsb_index_free(self.h)
             self.h = None
 
@@ -698,6 +724,7 @@ class Group(_Column):
 
     def close(self):
         if getattr(self, "h", None):
+            self._close_groupings()
             self.eng.lib.vsb_group_free(self.h)
             self.h = None
 
@@ -720,6 +747,39 @@ class Group(_Column):
 
     def finalize(self):
         self.eng.check(self.eng.lib.vsb_group_finalize(self.h))
+
+
+class Grouping:
+    """A layout of keys on every shard of a column, kept across grouped calls (vsb_grouping_create): Index.grouping or
+    Group.grouping make one.  It holds its column; a call after the column gained rows or was closed raises VsbError (EINVAL)."""
+
+    def __init__(self, column: _Column, key_lists):
+        self.eng, self.column = column.eng, column
+        flat, offsets = _key_csr(key_lists)
+        h = _vp()
+        self.eng.check(column._fn("grouping_create")(column.h, _ptr(flat), _ptr(offsets), len(offsets) - 1, C.byref(h)))
+        self.h = h
+        if not hasattr(column, "_groupings"):
+            column._groupings = weakref.WeakSet()
+        column._groupings.add(self)
+
+    def scan_topk(self, metric: int, queries: np.ndarray, k: int, limit: int = 0):
+        """the column's scan_topk_grouped(metric, queries, k, key_lists, limit) on the kept layout (vsb_scan_topk_grouping)"""
+        return _grouped_call(self.eng, lambda qp, nq, res: self.eng.lib.vsb_scan_topk_grouping(self.h, metric, qp, nq, k, limit, res),
+                             queries)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.eng.lib.vsb_grouping_free(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class Quantizer:

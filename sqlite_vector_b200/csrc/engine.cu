@@ -180,6 +180,7 @@ struct HeldPass {
 struct BatchWs;   // batch_host.inc
 struct SetsState;   // batch_host.inc
 struct GroupedShard;   // batch_host.inc
+void groupings_detach(std::vector<vsb_grouping *> &list);   // column.inc
 
 }  // namespace
 
@@ -274,17 +275,29 @@ struct vsb_index {
     // null outside such a call
     const SetsState *sets = nullptr;
     long long st_sets_batches = 0, st_sets_fallbacks = 0, st_sets_levels = 0, st_sets_plan_us = 0;
-    // grouped top-k (vsb_scan_topk_grouped, DESIGN §3.15): one device area for the layout and the per-query arrays of a call, and
-    // a streamed index's distances of every window (4 bytes per row), both grown never shrunk
+    // grouped top-k (vsb_scan_topk_grouped, DESIGN §3.15): one device area for the per-query arrays of a call, and a streamed
+    // index's distances of every window (4 bytes per row), both grown never shrunk
     DeviceBuf<uint8_t> d_grouped;
     DeviceBuf<float> d_grouped_dist;
     long long grouped_cap = 0, grouped_dist_cap = 0;
-    // this shard's layout and last query's host state of the most recent grouped call (vsb_debug_read "grouped"), kept until the
-    // next one; and the distances planted by vsb_debug_write "grouped_dist" for the next call (empty: scan them)
+    // the device's (rowid ^ 2^63, row) table of explicit rowids sorted by rowid, which the layout builder searches; built for
+    // rowid_tab_rows rows on first need, so an append rebuilds it
+    DeviceBuf<unsigned long long> d_rowid_tab;
+    DeviceBuf<uint32_t> d_rowid_tab_row;
+    long long rowid_tab_cap = 0, rowid_tab_row_cap = 0, rowid_tab_rows = -1;
+    // the layout builder's pinned staging of the caller's keys (two buffers, allocated on first need)
+    HostBuf<uint8_t> lay_stage[2];
+    Event lay_stage_ev[2];
+    int lay_next = 0;
+    // this shard's state of the most recent grouped call (vsb_debug_read "grouped"), kept until the next one; and the distances
+    // planted by vsb_debug_write "grouped_dist" for the next call (empty: scan them)
     std::unique_ptr<GroupedShard> grouped;
     std::vector<float> grouped_plant;
+    // the groupings made on this index (vsb_grouping_create), detached when it is freed
+    std::vector<vsb_grouping *> groupings;
     long long st_grouped_queries = 0, st_grouped_pairs = 0, st_grouped_cands = 0, st_grouped_keys_replayed = 0;
     long long st_grouped_regrows = 0, st_grouped_layout_us = 0, st_grouped_scan_us = 0, st_grouped_walk_us = 0, st_grouped_replay_us = 0;
+    long long st_grouped_layout_reuses = 0;
 };
 
 // result of a range call (vsb_scan_range): per query, rowids and distances in result order
@@ -1670,6 +1683,7 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "grouped_keys_replayed")) return ix->st_grouped_keys_replayed;
     if (!strcmp(name, "grouped_regrows")) return ix->st_grouped_regrows;
     if (!strcmp(name, "grouped_layout_us")) return ix->st_grouped_layout_us;
+    if (!strcmp(name, "grouped_layout_reuses")) return ix->st_grouped_layout_reuses;
     if (!strcmp(name, "grouped_scan_us")) return ix->st_grouped_scan_us;
     if (!strcmp(name, "grouped_walk_us")) return ix->st_grouped_walk_us;
     if (!strcmp(name, "grouped_replay_us")) return ix->st_grouped_replay_us;
@@ -1686,6 +1700,7 @@ void vsb_index_free(vsb_index *ix) {
     cudaSetDevice(ix->device);
     drain(ix);
     cudaStreamSynchronize(ix->xstream);
+    groupings_detach(ix->groupings);
     delete ix;
 }
 
@@ -1770,10 +1785,11 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
         return (int)n;
     }
     else if (!strcmp(name, "grouped")) {                                // the layout and last query of the last grouped call
-        if (!ix->grouped) return fail(VSB_EINVAL, "no grouped call has run yet");
+        if (!ix->grouped || !ix->grouped->lay) return fail(VSB_EINVAL, "no grouped call has run yet");
         const GroupedShard &gs = *ix->grouped;
+        const GroupedLayout &L = *gs.lay;
         const GroupedParams &p = gs.p;
-        const size_t npos = gs.rows.size(), np = gs.pkey.size(), nk = gs.kmin.size(), kk = (size_t)p.k;
+        const size_t npos = (size_t)L.npos, np = (size_t)L.npieces, nk = gs.kmin.size(), kk = (size_t)p.k;
         const size_t ndist = npos ? (size_t)ix->n : 0;
         const long long head[7] = {(long long)npos, (long long)np, (long long)nk, (long long)kk, (long long)ndist, gs.ksel_used ? 1 : 0,
                                    (long long)gs.pairs.size()};
@@ -1788,12 +1804,12 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
             if (n) CU(cudaMemcpy(d.data() + at, src, n, cudaMemcpyDeviceToHost));
             return (int)VSB_OK;
         };
-        host(gs.rows.data(), 4 * npos);
-        host(gs.koff.data(), 4 * (nk + 1));
-        host(gs.pstart.data(), 4 * (np + 1));
-        host(gs.pkey.data(), 4 * np);
-        host(gs.kpiece.data(), 4 * (nk + 1));
-        int rc2 = dev(gs.d_dist, 4 * ndist);
+        host(L.h_rows.data(), 4 * npos);
+        host(L.koff.data(), 4 * (nk + 1));
+        int rc2 = dev(L.pstart, 4 * (np + 1));
+        if (rc2 == VSB_OK) rc2 = dev(L.pkey, 4 * np);
+        if (rc2 == VSB_OK) rc2 = dev(L.kpiece, 4 * (nk + 1));
+        if (rc2 == VSB_OK) rc2 = dev(gs.d_dist, 4 * ndist);
         if (rc2 == VSB_OK) rc2 = dev(p.pd, 4 * npos);
         if (rc2 == VSB_OK) rc2 = dev(p.lists, 4 * np * kk);
         if (rc2 == VSB_OK) rc2 = dev(p.bound, 4 * np);

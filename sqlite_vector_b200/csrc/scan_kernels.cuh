@@ -1249,6 +1249,363 @@ __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_write_kernel(const
     }
 }
 
+// ------------------------------------------------------------------ grouped layout (DESIGN §3.15)
+// One shard's layout of a set of keys, built on the device from the caller's CSR keys (rowids, offsets):
+//   grouped_map_count_kernel, grouped_scan64_kernel, grouped_map_write_kernel: every (key, rowid) pair becomes the shard rows that
+//   hold the rowid (implicit rowids by arithmetic, explicit ones by a binary search of the index's (rowid, row) table sorted by
+//   rowid; a rowid held by several rows yields each of them), counted, placed and written as the composite key << rbits | row;
+//   grouped_sort_hist_kernel, grouped_sort_scan_kernel, grouped_sort_scatter_kernel: one pass of a stable LSD radix sort of 64-bit
+//   keys (and optional 32-bit values) by an 8-bit digit; a sort runs only the passes its keys' bits need;
+//   grouped_uniq_count_kernel, lk_offsets_kernel, grouped_uniq_write_kernel: the sorted composites without adjacent repeats;
+//   grouped_koff_kernel: each key's first position (a binary search of its smallest composite);
+//   grouped_piece_count_kernel, lk_offsets_kernel, grouped_piece_write_kernel, grouped_rows_kernel: each key cut into pieces of at
+//   most kGroupedPiece positions (kpiece, pstart, pkey) and the shard row of every position.
+constexpr int kLayoutThreads = 256;
+constexpr int kLayoutItems = 8;                                  // entries per thread of the map, unique and piece kernels
+constexpr int kLayoutTile = kLayoutThreads * kLayoutItems;       // entries per block of those kernels
+constexpr int kSortTile = kLayoutThreads * 16;                   // keys per block of a sort pass
+
+struct LayoutParams {
+    const int64_t *rowids;           // [m] the keys' rowids, back to back
+    const int64_t *offsets;          // [nkeys + 1] key g's rowids are [offsets[g], offsets[g + 1])
+    long long m0, m;                 // map kernels: the pairs [m0, m) (m0 a multiple of kLayoutTile)
+    int nkeys, rbits;                // rbits: bits of a shard row in a composite
+    int implicit;                    // rowid = first_seq + row + 1
+    long long first_seq, n;          // n: shard rows
+    const unsigned long long *tab;   // explicit rowids: [n] rowid ^ 2^63, ascending
+    const uint32_t *tab_row;         // [n] the row of each
+    unsigned long long *bcount;      // [map blocks] rows of each block's pairs, then where they start
+    unsigned long long *comp;        // composites (map: written; unique: read, sorted)
+    unsigned long long *uniq;        // the unique composites
+    const unsigned *npos;            // device: the unique composites' count
+    unsigned *boff;                  // [blocks] per-block counts, then offsets (lk_offsets_kernel)
+    uint32_t *koff;                  // [nkeys + 1]
+    uint32_t *rows, *pstart, *pkey, *kpiece;
+};
+
+struct SortParams {
+    const unsigned long long *kin;
+    unsigned long long *kout;
+    const uint32_t *vin;             // values (nullptr: keys only)
+    uint32_t *vout;
+    long long m;
+    int shift, nblocks;
+    unsigned *hist;                  // [256][nblocks]: the digit counts of each block, then where they start within the digit
+    unsigned *dtot;                  // [256] keys of each digit
+};
+
+// exclusive prefix of v over the kLayoutThreads threads of a block (in thread order) and the block's total; wsum: shared [8],
+// free again after the next __syncthreads
+template <class T>
+__device__ __forceinline__ T layout_block_scan(T v, T *wsum, T &total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    T incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const T t = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) wsum[warp] = incl;
+    __syncthreads();
+    T before = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < kLayoutThreads / 32; ++w) {
+        before += w < warp ? wsum[w] : T(0);
+        tot += wsum[w];
+    }
+    total = tot;
+    return before + incl - v;
+}
+
+// the shard rows of rowid r: rows lo .. hi - 1 (implicit), or tab_row[lo .. hi) (explicit)
+__device__ __forceinline__ void layout_rows_of(const LayoutParams &p, int64_t r, long long &lo, long long &hi) {
+    if (p.implicit) {
+        const bool in = r > p.first_seq && r - p.first_seq <= p.n;
+        lo = in ? r - p.first_seq - 1 : 0;
+        hi = in ? lo + 1 : 0;
+        return;
+    }
+    const unsigned long long key = (unsigned long long)r ^ (1ull << 63);
+    long long a = 0, b = p.n;
+    while (a < b) {
+        const long long mid = (a + b) >> 1;
+        if (p.tab[mid] < key) a = mid + 1; else b = mid;
+    }
+    lo = a;
+    b = p.n;
+    while (a < b) {
+        const long long mid = (a + b) >> 1;
+        if (p.tab[mid] <= key) a = mid + 1; else b = mid;
+    }
+    hi = a;
+}
+
+// rows of each block's pairs
+__global__ void __launch_bounds__(kLayoutThreads) grouped_map_count_kernel(const LayoutParams p) {
+    __shared__ unsigned long long wsum[kLayoutThreads / 32];
+    const long long i0 = p.m0 + (long long)blockIdx.x * kLayoutTile;
+    unsigned long long c = 0;
+#pragma unroll
+    for (int j = 0; j < kLayoutItems; ++j) {
+        const long long i = i0 + j * kLayoutThreads + threadIdx.x;
+        if (i < p.m) {
+            long long lo, hi;
+            layout_rows_of(p, p.rowids[i], lo, hi);
+            c += (unsigned long long)(hi - lo);
+        }
+    }
+    unsigned long long total;
+    layout_block_scan(c, wsum, total);
+    if (threadIdx.x == 0) p.bcount[i0 / kLayoutTile] = total;
+}
+
+// one block: the block counts v[0, n) become where each block's entries start; *total = their sum
+__global__ void __launch_bounds__(1024, 1) grouped_scan64_kernel(unsigned long long *v, long long n, unsigned long long *total) {
+    __shared__ unsigned long long wsum[32];
+    __shared__ unsigned long long carry;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (long long b0 = 0; b0 < n; b0 += 1024) {
+        const long long i = b0 + threadIdx.x;
+        const unsigned long long x = i < n ? v[i] : 0ull;
+        unsigned long long incl = x;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long t = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= o) incl += t;
+        }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            unsigned long long w = wsum[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned long long t = __shfl_up_sync(0xFFFFFFFFu, w, o);
+                if (lane >= o) w += t;
+            }
+            wsum[lane] = w;
+        }
+        __syncthreads();
+        const unsigned long long base = carry;
+        if (i < n) v[i] = base + (warp ? wsum[warp - 1] : 0ull) + incl - x;
+        __syncthreads();
+        if (threadIdx.x == 0) carry = base + wsum[31];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *total = carry;
+}
+
+// each pair's rows as composites from its block's offset on (the order inside a block is free: the sort follows)
+__global__ void __launch_bounds__(kLayoutThreads) grouped_map_write_kernel(const LayoutParams p) {
+    __shared__ unsigned long long wsum[kLayoutThreads / 32];
+    const long long i0 = (long long)blockIdx.x * kLayoutTile;
+    long long lo[kLayoutItems], hi[kLayoutItems];
+    unsigned long long c = 0;
+#pragma unroll
+    for (int j = 0; j < kLayoutItems; ++j) {
+        const long long i = i0 + j * kLayoutThreads + threadIdx.x;
+        lo[j] = hi[j] = 0;
+        if (i < p.m) layout_rows_of(p, p.rowids[i], lo[j], hi[j]);
+        c += (unsigned long long)(hi[j] - lo[j]);
+    }
+    unsigned long long total;
+    unsigned long long at = p.bcount[blockIdx.x] + layout_block_scan(c, wsum, total);
+#pragma unroll
+    for (int j = 0; j < kLayoutItems; ++j) {
+        if (hi[j] == lo[j]) continue;
+        const long long i = i0 + j * kLayoutThreads + threadIdx.x;
+        int a = 0, b = p.nkeys + 1;                                  // the key: the last g with offsets[g] <= i
+        while (a < b) {
+            const int mid = (a + b) >> 1;
+            if (p.offsets[mid] <= i) a = mid + 1; else b = mid;
+        }
+        const unsigned long long key = (unsigned long long)(a - 1) << p.rbits;
+        for (long long r = lo[j]; r < hi[j]; ++r) p.comp[at++] = key | (p.implicit ? (unsigned long long)r : (unsigned long long)p.tab_row[r]);
+    }
+}
+
+__device__ __forceinline__ unsigned sort_digit(unsigned long long key, int shift) { return (unsigned)(key >> shift) & 255u; }
+
+// the digit counts of each block's keys
+__global__ void __launch_bounds__(kLayoutThreads) grouped_sort_hist_kernel(const SortParams p) {
+    __shared__ unsigned h[256];
+    h[threadIdx.x] = 0u;
+    __syncthreads();
+    const long long i0 = (long long)blockIdx.x * kSortTile, i1 = min(i0 + (long long)kSortTile, p.m);
+    for (long long i = i0 + threadIdx.x; i < i1; i += kLayoutThreads) atomicAdd(&h[sort_digit(p.kin[i], p.shift)], 1u);
+    __syncthreads();
+    p.hist[(size_t)threadIdx.x * p.nblocks + blockIdx.x] = h[threadIdx.x];
+}
+
+// block d: digit d's block counts become where each block's keys of digit d start inside the digit; dtot[d] = the digit's keys
+__global__ void __launch_bounds__(kLayoutThreads) grouped_sort_scan_kernel(const SortParams p) {
+    __shared__ unsigned wsum[kLayoutThreads / 32];
+    unsigned *h = p.hist + (size_t)blockIdx.x * p.nblocks;
+    unsigned carry = 0;
+    for (int b0 = 0; b0 < p.nblocks; b0 += kLayoutThreads) {
+        const int i = b0 + (int)threadIdx.x;
+        const unsigned v = i < p.nblocks ? h[i] : 0u;
+        unsigned total;
+        const unsigned ex = layout_block_scan(v, wsum, total);
+        if (i < p.nblocks) h[i] = carry + ex;
+        carry += total;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) p.dtot[blockIdx.x] = carry;
+}
+
+// each block's keys to their places, stably: in index order inside the block (warp by warp through __match_any_sync), after the
+// same digit's keys of earlier blocks, after the keys of smaller digits
+__global__ void __launch_bounds__(kLayoutThreads) grouped_sort_scatter_kernel(const SortParams p) {
+    __shared__ unsigned base[256];
+    __shared__ unsigned wc[kLayoutThreads / 32][256];
+    __shared__ unsigned wsum[kLayoutThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, t = threadIdx.x;
+    unsigned total;
+    const unsigned ex = layout_block_scan(p.dtot[t], wsum, total);
+    base[t] = ex + p.hist[(size_t)t * p.nblocks + blockIdx.x];
+#pragma unroll
+    for (int w = 0; w < kLayoutThreads / 32; ++w) wc[w][t] = 0u;
+    __syncthreads();
+    const long long i0 = (long long)blockIdx.x * kSortTile;
+    for (int it = 0; it < kSortTile / kLayoutThreads; ++it) {
+        const long long i = i0 + (long long)it * kLayoutThreads + t;
+        if (i0 + (long long)it * kLayoutThreads >= p.m) break;              // uniform across the block
+        const bool valid = i < p.m;
+        const unsigned long long key = valid ? p.kin[i] : 0ull;
+        const unsigned d = valid ? sort_digit(key, p.shift) : 256u;
+        const unsigned peers = __match_any_sync(0xFFFFFFFFu, d);
+        const unsigned rank = (unsigned)__popc(peers & ((1u << lane) - 1u));
+        if (valid && rank == 0) wc[warp][d] = (unsigned)__popc(peers);
+        __syncthreads();
+        unsigned run = base[t];
+#pragma unroll
+        for (int w = 0; w < kLayoutThreads / 32; ++w) {
+            const unsigned c = wc[w][t];
+            wc[w][t] = run;
+            run += c;
+        }
+        base[t] = run;
+        __syncthreads();
+        if (valid) {
+            const unsigned at = wc[warp][d] + rank;
+            p.kout[at] = key;
+            if (p.vin) p.vout[at] = p.vin[i];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int w = 0; w < kLayoutThreads / 32; ++w) wc[w][t] = 0u;
+        __syncthreads();
+    }
+}
+
+// explicit rowids: the table's keys (rowid ^ 2^63, so that unsigned order is signed order) and rows before the sort
+__global__ void __launch_bounds__(kLayoutThreads) grouped_table_keys_kernel(const int64_t *rowids, long long n, unsigned long long *keys,
+                                                                            uint32_t *rows) {
+    for (long long i = (long long)blockIdx.x * kLayoutThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kLayoutThreads) {
+        keys[i] = (unsigned long long)rowids[i] ^ (1ull << 63);
+        rows[i] = (uint32_t)i;
+    }
+}
+
+// the sorted composites' first occurrences, thread by thread in index order
+__device__ __forceinline__ unsigned layout_firsts(const LayoutParams &p, long long i0, bool *first) {
+    unsigned c = 0;
+#pragma unroll
+    for (int j = 0; j < kLayoutItems; ++j) {
+        const long long i = i0 + j;
+        first[j] = i < p.m && (i == 0 || p.comp[i] != p.comp[i - 1]);
+        c += first[j] ? 1u : 0u;
+    }
+    return c;
+}
+
+__global__ void __launch_bounds__(kLayoutThreads) grouped_uniq_count_kernel(const LayoutParams p) {
+    __shared__ unsigned wsum[kLayoutThreads / 32];
+    bool first[kLayoutItems];
+    const unsigned c = layout_firsts(p, (long long)blockIdx.x * kLayoutTile + (long long)threadIdx.x * kLayoutItems, first);
+    unsigned total;
+    layout_block_scan(c, wsum, total);
+    if (threadIdx.x == 0) p.boff[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(kLayoutThreads) grouped_uniq_write_kernel(const LayoutParams p) {
+    __shared__ unsigned wsum[kLayoutThreads / 32];
+    bool first[kLayoutItems];
+    const long long i0 = (long long)blockIdx.x * kLayoutTile + (long long)threadIdx.x * kLayoutItems;
+    const unsigned c = layout_firsts(p, i0, first);
+    unsigned total;
+    unsigned at = p.boff[blockIdx.x] + layout_block_scan(c, wsum, total);
+#pragma unroll
+    for (int j = 0; j < kLayoutItems; ++j)
+        if (first[j]) p.uniq[at++] = p.comp[i0 + j];
+}
+
+// koff[g] for g in [0, nkeys]: the first unique composite of key g or later
+__global__ void __launch_bounds__(kLayoutThreads) grouped_koff_kernel(const LayoutParams p) {
+    const long long g = (long long)blockIdx.x * kLayoutThreads + threadIdx.x;
+    if (g > p.nkeys) return;
+    const unsigned long long key = (unsigned long long)g << p.rbits;
+    unsigned a = 0, b = *p.npos;
+    while (a < b) {
+        const unsigned mid = a + ((b - a) >> 1);
+        if (p.uniq[mid] < key) a = mid + 1; else b = mid;
+    }
+    p.koff[g] = a;
+}
+
+// the pieces of keys [g0, g0 + kLayoutItems), thread by thread in key order
+__device__ __forceinline__ unsigned layout_pieces(const LayoutParams &p, long long g0, unsigned *np) {
+    unsigned c = 0;
+#pragma unroll
+    for (int j = 0; j < kLayoutItems; ++j) {
+        const long long g = g0 + j;
+        np[j] = g < p.nkeys ? (p.koff[g + 1] - p.koff[g] + (unsigned)kGroupedPiece - 1u) / (unsigned)kGroupedPiece : 0u;
+        c += np[j];
+    }
+    return c;
+}
+
+__global__ void __launch_bounds__(kLayoutThreads) grouped_piece_count_kernel(const LayoutParams p) {
+    __shared__ unsigned wsum[kLayoutThreads / 32];
+    unsigned np[kLayoutItems];
+    const unsigned c = layout_pieces(p, (long long)blockIdx.x * kLayoutTile + (long long)threadIdx.x * kLayoutItems, np);
+    unsigned total;
+    layout_block_scan(c, wsum, total);
+    if (threadIdx.x == 0) p.boff[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(kLayoutThreads) grouped_piece_write_kernel(const LayoutParams p) {
+    __shared__ unsigned wsum[kLayoutThreads / 32];
+    unsigned np[kLayoutItems];
+    const long long g0 = (long long)blockIdx.x * kLayoutTile + (long long)threadIdx.x * kLayoutItems;
+    const unsigned c = layout_pieces(p, g0, np);
+    unsigned total;
+    unsigned at = p.boff[blockIdx.x] + layout_block_scan(c, wsum, total);
+#pragma unroll
+    for (int j = 0; j < kLayoutItems; ++j) {
+        const long long g = g0 + j;
+        if (g >= p.nkeys) break;
+        p.kpiece[g] = at;
+        for (unsigned q = 0; q < np[j]; ++q, ++at) {
+            p.pstart[at] = p.koff[g] + q * (unsigned)kGroupedPiece;
+            p.pkey[at] = (uint32_t)g;
+        }
+        if (g == p.nkeys - 1) {
+            p.kpiece[p.nkeys] = at;
+            p.pstart[at] = p.koff[p.nkeys];
+        }
+    }
+}
+
+// the shard row of every position
+__global__ void __launch_bounds__(kLayoutThreads) grouped_rows_kernel(const LayoutParams p) {
+    const unsigned long long mask = (1ull << p.rbits) - 1ull;
+    for (long long i = (long long)blockIdx.x * kLayoutThreads + threadIdx.x; i < (long long)*p.npos; i += (long long)gridDim.x * kLayoutThreads)
+        p.rows[i] = (uint32_t)(p.uniq[i] & mask);
+}
+
 // ------------------------------------------------------------------ candidate filter
 // One warp per stream.  thresholds: a row of stream s can only enter the reference's slots if its distance
 // is below the k-th smallest distance among ALL earlier rows; any subset of earlier rows gives a valid upper

@@ -47,6 +47,15 @@ enum { COL_TBL = 0, COL_VECTOR = 1, COL_K = 2, COL_MEMIDX = 3 };
 #define N_MODULES 20                           /* rows of `modules`, the table-valued functions */
 
 /* ------------------------------------------------------------------------------------------------ state */
+/* the grouping of the most recent vector_*_scan_grouped statement on one staged column, with that statement's groups BLOB and its
+ * dense key index -> user key mapping (DESIGN §3.15) */
+typedef struct {
+    vsb_grouping *gr;
+    unsigned char *blob;
+    sqlite3_int64 bytes;
+    int64_t *keys;
+} kept_grouping;
+
 typedef struct {
     char *tbl, *col, *pk;          /* pk: "rowid" or the INTEGER PRIMARY KEY of a WITHOUT ROWID table */
     int vtype, dim, normalized, metric, qtype;
@@ -62,6 +71,7 @@ typedef struct {
     sqlite3_int64 fix_dataver;
     int fix_changes;
     int fix_tainted;               /* staged inside an open transaction: never reused */
+    kept_grouping q_kept, fix_kept; /* the grouped modules' kept grouping on qix / fix, freed before its column */
 } vcolumn;
 
 typedef struct module_def module_def;         /* one table-valued function: a row of `modules` */
@@ -414,9 +424,26 @@ static vcolumn *ctx_find(vcontext *c, const char *tbl, const char *col) { /* vec
     }
     return 0;
 }
+static void kept_free(kept_grouping *k) {
+    vsb_grouping_free(k->gr);
+    sqlite3_free(k->blob);
+    sqlite3_free(k->keys);
+    memset(k, 0, sizeof *k);
+}
+/* a staged column goes with the grouping kept on it */
+static void drop_qix(vcolumn *v) {
+    kept_free(&v->q_kept);
+    vsb_group_free(v->qix);
+    v->qix = 0;
+}
+static void drop_fix(vcolumn *v) {
+    kept_free(&v->fix_kept);
+    vsb_group_free(v->fix);
+    v->fix = 0;
+}
 static void column_drop_device(vcolumn *v) {
-    if (v->qix) { vsb_group_free(v->qix); v->qix = 0; }
-    if (v->fix) { vsb_group_free(v->fix); v->fix = 0; }
+    drop_qix(v);
+    drop_fix(v);
     v->q_user_preloaded = 0;
 }
 static void ctx_free(void *p) { /* vector_context_free, :1038-1049 */
@@ -907,7 +934,7 @@ static int rebuild_quantization(sqlite3_context *ctx, vcolumn *v, int qtype, uin
 
 /* stage every shadow-table chunk into HBM (the GPU counterpart of the loop at :1382-1394) */
 static int stage_quantized(sqlite3 *db, vcolumn *v, char **errmsg) {
-    if (v->qix) { vsb_group_free(v->qix); v->qix = 0; }
+    drop_qix(v);
     v->q_tainted = !sqlite3_get_autocommit(db);
     v->q_dataver = query_int64(db, "PRAGMA data_version;");
     quant_fingerprint(db, v, v->q_fp);
@@ -934,8 +961,7 @@ static int stage_quantized(sqlite3 *db, vcolumn *v, char **errmsg) {
     if (src == SQLITE_OK && vsb_group_finalize(v->qix) != VSB_OK) { src = SQLITE_ERROR; *errmsg = sqlite3_mprintf("%s", vsb_last_error()); }
     if (src != SQLITE_OK) {
         if (!*errmsg) *errmsg = sqlite3_mprintf("%s", sqlite3_errmsg(db));
-        vsb_group_free(v->qix);
-        v->qix = 0;
+        drop_qix(v);
     }
     return src;
 }
@@ -1009,12 +1035,12 @@ static int do_quantize(sqlite3_context *ctx, const char *tbl, const char *col, c
     if (rc == SQLITE_OK) rc = meta_store(ctx, tbl, col, "qoffset", 0, 0, (double)v->offset);
     if (rc != SQLITE_OK) goto fail;
     *was_preloaded = v->q_user_preloaded;
-    if (v->qix) { vsb_group_free(v->qix); v->qix = 0; } /* the device copy is a cache of the shadow table */
+    drop_qix(v);                                      /* the device copy is a cache of the shadow table */
     sqlite3_result_int64(ctx, (sqlite3_int64)counter);
     return SQLITE_OK;
 fail:
     sqlite3_exec(db, "ROLLBACK TO vsb_quantize; RELEASE vsb_quantize;", 0, 0, 0);
-    if (v->qix && !v->q_user_preloaded) { vsb_group_free(v->qix); v->qix = 0; }
+    if (v->qix && !v->q_user_preloaded) drop_qix(v);
     sqlite3_result_error_code(ctx, rc);
     return rc;
 }
@@ -1059,7 +1085,7 @@ static void fn_quantize_cleanup(sqlite3_context *ctx, int argc, sqlite3_value **
     const char *col = (const char *)sqlite3_value_text(argv[1]);
     vcolumn *v = ctx_find((vcontext *)sqlite3_user_data(ctx), tbl, col);
     if (!v) return;
-    if (v->qix) { vsb_group_free(v->qix); v->qix = 0; }
+    drop_qix(v);
     v->q_user_preloaded = 0;
     char *sql = sqlite3_mprintf("DROP TABLE IF EXISTS vector0_%q_%q;", tbl, col);
     if (sql) sqlite3_exec(sqlite3_context_db_handle(ctx), sql, 0, 0, 0);
@@ -1078,7 +1104,7 @@ static int stage_full_column(scan_vtab *vt, vcolumn *v) {
      * autocommit mode holds committed rows only; it stays valid until a counter moves. */
     const int in_txn = !sqlite3_get_autocommit(db);
     if (v->fix && !v->fix_tainted && v->fix_dataver == dataver && v->fix_changes == changes) return SQLITE_OK;
-    if (v->fix) { vsb_group_free(v->fix); v->fix = 0; }
+    drop_fix(v);
     char *sql = sqlite3_mprintf("SELECT COUNT(*) FROM %q;", v->tbl);
     sqlite3_int64 total = sql ? query_int64(db, sql) : 0;
     sqlite3_free(sql);
@@ -1117,7 +1143,7 @@ static int stage_full_column(scan_vtab *vt, vcolumn *v) {
     sqlite3_free(rows);
     sqlite3_free(ids);
     if (rc != SQLITE_OK) {
-        if (v->fix) { vsb_group_free(v->fix); v->fix = 0; }
+        drop_fix(v);
         if (!vt->base.zErrMsg) vtab_error(&vt->base, "vector_full_scan: %s", sqlite3_errmsg(db));
         return SQLITE_ERROR;
     }
@@ -1149,7 +1175,11 @@ static int stage_full_column(scan_vtab *vt, vcolumn *v) {
  *   little-endian (int64 key, int64 rowid) pairs (vector_rowid_sets builds it); keys may be sparse.  Rows are (key, id, distance),
  *   keys in rank order and each key's rows exactly those of vector_*_scan_filtered with that key's rowids
  *   (vsb_group_scan_topk_grouped, DESIGN §3.15).  The reference answers it with row_number() OVER (PARTITION BY key ORDER BY
- *   distance) over vector_*_scan_stream.
+ *   distance) over vector_*_scan_stream.  Each of the two modules keeps the grouping (vsb_grouping_create) of its most recent
+ *   statement beside the staged column it scanned, with a copy of that statement's groups BLOB and its key mapping: a statement
+ *   whose groups BLOB is byte for byte the kept one, on the same staged column, skips the decoding of the BLOB and the layout.
+ *   Anything else lays the keys out anew and replaces the kept grouping; re-staging the column (a changed table, data_version,
+ *   or a copy staged inside a transaction) and closing the connection free it.  The rows returned are the same either way.
  * vector_*_scan_range(tbl, col, vector, radius) and the *_range_filtered twins (+ rowids): every row with distance < radius,
  *   ordered by distance, equal distances in scan order (vsb_group_scan_range).  The reference answers this only as
  *   SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < radius ORDER BY distance: the same rows, here without a
@@ -1327,7 +1357,7 @@ static int resident_index(scan_vtab *vt, vcolumn *v, const char *tbl, const char
                     v->q_dataver = dv;
                 }
             }
-            if (stale) { vsb_group_free(v->qix); v->qix = 0; column_load_meta(vt->db, v); }
+            if (stale) { drop_qix(v); column_load_meta(vt->db, v); }
         }
         if (!v->qix) { /* not preloaded: the reference streams the chunks from disk per query (:2186-2227); we stage them once */
             char *err = 0;
@@ -1605,8 +1635,24 @@ static int vt_filter(sqlite3_vtab_cursor *cur, int idxnum, const char *idxstr, i
     case OP_GROUPED: {
         const sqlite3_int64 lim64 = sqlite3_value_type(argv[5]) == SQLITE_NULL ? 0 : sqlite3_value_int64(argv[5]);
         const int limit = lim64 > 0x7FFFFFFF ? 0 : (int)lim64;         /* a limit above every possible key count keeps every key */
-        if ((rc = pairs_by_key(argv[4], &runs)) != SQLITE_OK) goto out;
-        src = vsb_group_scan_topk_grouped(q.ix, metric, q.query, 1, k, runs.rowids, runs.offsets, (int)runs.nkeys, limit, &res);
+        kept_grouping *kept = q.ix == q.v->qix ? &q.v->q_kept : &q.v->fix_kept;
+        const void *blob = sqlite3_value_blob(argv[4]);
+        const sqlite3_int64 bytes = sqlite3_value_bytes(argv[4]);
+        if (!kept->gr || kept->bytes != bytes || (bytes > 0 && memcmp(kept->blob, blob, (size_t)bytes) != 0)) {
+            /* not the kept statement's groups: lay them out anew, in place of the kept grouping */
+            kept_free(kept);
+            if ((rc = pairs_by_key(argv[4], &runs)) != SQLITE_OK) goto out;
+            vsb_grouping *gr = 0;
+            if ((src = vsb_group_grouping_create(q.ix, runs.rowids, runs.offsets, (int)runs.nkeys, &gr)) != VSB_OK) break;
+            kept->blob = (unsigned char *)sqlite3_malloc64((sqlite3_uint64)(bytes > 0 ? bytes : 1));
+            if (!kept->blob) { vsb_grouping_free(gr); rc = SQLITE_NOMEM; goto out; }
+            if (bytes > 0) memcpy(kept->blob, blob, (size_t)bytes);
+            kept->bytes = bytes;
+            kept->gr = gr;
+            kept->keys = runs.keys;                                     /* dense key index -> user key */
+            runs.keys = 0;
+        }
+        src = vsb_scan_topk_grouping(kept->gr, metric, q.query, 1, k, limit, &res);
         if (src != VSB_OK) break;
         int nk = 0;
         const int32_t *gk = 0;
@@ -1617,7 +1663,7 @@ static int vt_filter(sqlite3_vtab_cursor *cur, int idxnum, const char *idxstr, i
         for (int i = 0; i < nk; ++i) {
             const sqlite3_int64 n = go[i + 1] - go[i];
             c->count[i] = n;
-            c->key[i] = runs.keys[gk[i]];
+            c->key[i] = kept->keys[gk[i]];
             memcpy(c->ids + (size_t)i * k, gi + go[i], (size_t)n * sizeof(int64_t));
             memcpy(c->dist + (size_t)i * k, gd + go[i], (size_t)n * sizeof(double));
         }

@@ -170,8 +170,11 @@ VSB_API int vsb_scan_topk_rows(vsb_index *ix, int metric, const void *queries, i
  * distances of all its windows on the device (4 bytes per row, in vsb_index_device_bytes).  Counters: "grouped_queries",
  * "grouped_pairs" (the (key, row) pairs of the last layout), "grouped_cands" (candidates replayed), "grouped_keys_replayed" (on a
  * group's first shard), "grouped_regrows", "grouped_layout_us" (layouts built), "grouped_layout_reuses" (calls that ran on a
- * grouping's kept layout), and the device times "grouped_scan_us" (scans) and
- * "grouped_walk_us" (walk, bounds and compaction) and the host time "grouped_replay_us" (on a group's first shard).  *out receives
+ * grouping's kept layout), "grouped_passes" and "grouped_pass_queries" (passes of the column and the queries they scored), and
+ * the device times "grouped_scan_us" (scans) and "grouped_walk_us" (walk, bounds and compaction), timed per pass, and the host
+ * time "grouped_replay_us" (on a group's first shard).  Several queries share each pass of the column (at most the scan's
+ * pass_max width, and as many per-query areas of distances and device arrays as fit option "grouped_mem_mb", default 1/8 of the
+ * free device memory); each query's answer is bit for bit what a call of that query alone returns.  *out receives
  * a result owned by the caller (vsb_grouped_free); vsb_grouped_get borrows query q's arrays from it: nkeys_out keys in rank
  * order, key i's rows at [row_offsets[i], row_offsets[i + 1]) of rowids and dist. */
 typedef struct vsb_grouped vsb_grouped;
@@ -421,15 +424,18 @@ VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches,
  * N pieces, G keys, k, D distances (the shard's rows; 0 without positions), S (1: the limit selected keys), C survivor pairs},
  * then uint32 rows [P] (shard row of each position), koff [G + 1], pstart [N + 1], pkey [N], kpiece [G + 1], float dist [D] (the
  * query's distances), pd [P] (d where the walk logged, NaN otherwise), lists [N][k], bound [N], kmin [G], uint32 [C][2]
- * survivors (distance bits, position) in position order, and with S = 1 uint8 ksel [G] (1: the key was compacted))}.  Returns
- * the bytes copied or < 0. */
+ * survivors (distance bits, position) in position order, and with S = 1 uint8 ksel [G] (1: the key was compacted))},
+ * "grouped_pass" (the same shard's state for every query of the last pass of that call: int64 [6] {P, N, G, k, D, W queries},
+ * the layout arrays rows, koff, pstart, pkey, kpiece as for "grouped", then per query int64 [2] {S, C} and dist [D], pd [P],
+ * lists [N][k], bound [N], kmin [G], the C survivor pairs and with S = 1 ksel [G]).  Returns the bytes copied or < 0. */
 VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes);
 /* diagnostics: the counterpart of vsb_debug_read for name "bounds": plants a row partition (int64 tile boundaries, one per scan
  * CTA plus one, non-decreasing from 0 to the tile count of the k <= 32 plan; vsb_index_stat "sms" CTAs) into every scan
  * workspace of a resident index, so that the next single-query scans with k <= 32 use it instead of equal shares (the filter
  * then rewrites it as usual).  Rejects an index too small for the adaptive partition.  Name "grouped_dist": float32 [shard
  * rows], the distances every query of the next grouped call on this index (resident or streamed, or a shard of a group through
- * vsb_group_shard) uses instead of its scans; everything after the scans runs as usual, and the call drops the plant when it
+ * vsb_group_shard) uses instead of its scans, or float32 [nq][shard rows], row j for query j of a call of nq queries (a size
+ * that is not whole rows is rejected here, a row count other than 1 or the call's nq by the call); everything after the scans runs as usual, and the call drops the plant when it
  * ends, however it ends.  Returns 0 or < 0. */
 VSB_API int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t bytes);
 /* diagnostics: the survivors of a result slot (fetch != 0) exactly as vsb_collect replays them: (uint32 distance bits, uint32
@@ -466,7 +472,7 @@ VSB_API int vsb_debug_refine(vsb_index *ix, int metric, const void *queries, int
 VSB_API int vsb_debug_replay(vsb_index *ix, int metric, const void *queries, int nq, int k, int level0, const uint32_t *bucket,
                              const uint32_t *bcount, float *slot_d, uint32_t *slot_row, int *slot_mi, int acc_cap, uint32_t *acc_log,
                              int *acc_count, int final_sort, float *out_U, uint32_t *out_qc, uint32_t *out_bcount, uint32_t *out_stats);
-/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","scan_streams","xwait_ms","epi_chunk","f32_batch","sets_mem_mb"};
+/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","scan_streams","xwait_ms","epi_chunk","f32_batch","sets_mem_mb","grouped_mem_mb"};
  * "f32_batch" = 1: f32 columns batch L2 / cosine / dot queries on the tensor cores in TF32 (default 0, or VSB_F32_BATCH=1 in the
  * environment when the library loads; per process).  Values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);

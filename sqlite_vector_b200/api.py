@@ -579,7 +579,7 @@ class Index(_Column):
 
     def debug_write(self, name: str, data: np.ndarray):
         """plant an internal buffer (vsb_debug_write); "bounds": int64 [stat("sms") + 1] tile boundaries; "grouped_dist":
-        float32 [rows], the distances of the next grouped call instead of its scans"""
+        float32 [rows] (every query) or [nq * rows] (query j: row j), the distances of the next grouped call instead of its scans"""
         a = np.ascontiguousarray(data, dtype=np.float32 if name == "grouped_dist" else np.int64)
         self.eng.check(self.eng.lib.vsb_debug_write(self.h, name.encode(), _ptr(a), a.nbytes))
 
@@ -602,6 +602,38 @@ class Index(_Column):
         out["pairs"] = out["pairs"].reshape(Cn, 2)
         if not S:
             out["ksel"] = None
+        return out
+
+    def debug_grouped_pass(self) -> dict:
+        """this shard's state after the last grouped call, for every query of its last pass (vsb_debug_read "grouped_pass"): the
+        layout arrays of debug_grouped, "k", and "queries", one dict per query of the pass with "dist", "pd", "lists", "bound",
+        "kmin", "pairs" and "ksel" as debug_grouped returns them"""
+        head = self.debug_read("grouped_pass", np.int64, 6)
+        P, N, G, k, D, W = (int(v) for v in head)
+        lay = [("rows", "<u4", P), ("koff", "<u4", G + 1), ("pstart", "<u4", N + 1), ("pkey", "<u4", N), ("kpiece", "<u4", G + 1)]
+        fixed = 48 + sum(np.dtype(t).itemsize * c for _, t, c in lay)
+        per = 16 + 4 * (D + P + N * k + N + G)
+        raw = self.debug_read("grouped_pass", np.uint8, fixed + W * (per + 8 * P + G))   # at most every position survives
+        out, at = {"k": k}, 48
+        for name, t, c in lay:
+            nb = np.dtype(t).itemsize * c
+            out[name] = raw[at:at + nb].view(t).copy()
+            at += nb
+        out["queries"] = []
+        for _ in range(W):
+            S, Cn = (int(v) for v in raw[at:at + 16].view("<i8"))
+            at += 16
+            q = {}
+            for name, t, c in (("dist", "<f4", D), ("pd", "<f4", P), ("lists", "<f4", N * k), ("bound", "<f4", N), ("kmin", "<f4", G),
+                               ("pairs", "<u4", 2 * Cn), ("ksel", "u1", G if S else 0)):
+                nb = np.dtype(t).itemsize * c
+                q[name] = raw[at:at + nb].view(t).copy()
+                at += nb
+            q["lists"] = q["lists"].reshape(N, k)
+            q["pairs"] = q["pairs"].reshape(Cn, 2)
+            if not S:
+                q["ksel"] = None
+            out["queries"].append(q)
         return out
 
     def debug_survivors(self, slot: int, cap: int = 1 << 16):

@@ -57,6 +57,7 @@ int g_opt_f32_batch = [] {
     return (e && atoi(e) > 0) ? 1 : 0;
 }();
 int g_opt_sets_mem_mb = 0;     // vsb_scan_topk_sets: device memory its one-pass buffers may take, in MB (0: 1/8 of the free memory)
+int g_opt_grouped_mem_mb = 0;  // grouped top-k: device memory the per-query areas of a pass may take, in MB (0: 1/8 of the free memory)
 int g_opt_xwait_ms = 10000;    // exchange: how long the receiving side waits for a peer's head before it reports an error (a dead
                                // peer, not a slow one: ranks sharing one GPU or a busy host can start a batch seconds apart)
 
@@ -297,7 +298,7 @@ struct vsb_index {
     std::vector<vsb_grouping *> groupings;
     long long st_grouped_queries = 0, st_grouped_pairs = 0, st_grouped_cands = 0, st_grouped_keys_replayed = 0;
     long long st_grouped_regrows = 0, st_grouped_layout_us = 0, st_grouped_scan_us = 0, st_grouped_walk_us = 0, st_grouped_replay_us = 0;
-    long long st_grouped_layout_reuses = 0;
+    long long st_grouped_layout_reuses = 0, st_grouped_passes = 0, st_grouped_pass_queries = 0;
 };
 
 // result of a range call (vsb_scan_range): per query, rowids and distances in result order
@@ -535,7 +536,9 @@ int merge_blocks_strided(const uint8_t *blocks, int world, size_t stride, const 
 int exchange_fill_push(vsb_index *ix, PushParams *pp);
 
 // launches one pass of the scan kernel for nq <= pass_max queries (device pointers queries[j], pitch bytes each) on ss and, when
-// k > 0, one filter per query on ix->fstream; slots[j] receives query j's result.  nq > 1 needs k > 0.
+// k > 0, one filter per query on ix->fstream; slots[j] receives query j's result.  nq > 1 needs k > 0, or k == 0 with
+// plan_kcap >= 0 and nq <= pass_max(ix, plan_kcap): an all-distances pass, query j's distances at d_dist_all + j * dist_stride
+// (no workspace, filter or slot state; slots may hold nullptr)
 // fetch: copy each slot's head to pinned host memory afterwards (false when the heads are all-gathered on the device)
 // ss: the scan stream of this launch (next_scan_stream); push: the heads are labelled for the exchange (shard index and
 // exchange sequence number); push_heads_kernel moves them (exchange_push)
@@ -545,7 +548,7 @@ int exchange_fill_push(vsb_index *ix, PushParams *pp);
 // the bits of a top-k scan at that k (grouped top-k)
 int launch_scan(vsb_index *ix, int metric, const uint8_t *const *queries, Slot *const *slots, int nq, int k, float *d_dist_all, bool fetch,
                 cudaStream_t ss, bool push = false, const uint8_t *view_vec = nullptr, long long view_n = -1, long long view_r0 = 0,
-                int plan_kcap = -1) {
+                int plan_kcap = -1, long long dist_stride = 0) {
     const uint8_t *scan_vec = view_vec ? view_vec : ix->d_vec;
     const long long scan_n = view_vec ? view_n : ix->n;
     if (!scan_vec) return fail(VSB_EINVAL, "this entry point needs a resident (not streamed) index");
@@ -556,7 +559,8 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *const *queries, Slot *
     // the scan's list layout, the filter's FAST/generic choice and its shared-memory layout all follow THIS query's k
     const int kcap = k > 0 ? ((k + 31) & ~31) : 0;
     if (kcap > ix->ws_kcap) return fail(VSB_EINVAL, "scan workspace too small for k = %d", k);
-    if (nq < 1 || (nq > 1 && (k <= 0 || nq > ix->ws_width || nq > pass_max(ix, kcap))))
+    const bool all_pass = k == 0 && plan_kcap >= 0 && d_dist_all != nullptr && nq <= pass_max(ix, plan_kcap);
+    if (nq < 1 || (nq > 1 && !all_pass && (k <= 0 || nq > ix->ws_width || nq > pass_max(ix, kcap))))
         return fail(VSB_EINVAL, "bad pass of %d queries", nq);
     const Plan pl = make_plan(ix, k == 0 && plan_kcap >= 0 ? plan_kcap : kcap, nq);
     ScanFn fn = pick_kernel(ix->vtype, mc, pl.direct, false, nq);
@@ -599,6 +603,7 @@ int launch_scan(vsb_index *ix, int metric, const uint8_t *const *queries, Slot *
     p.logs = wk ? wk->d_logs.get() : nullptr;
     p.counts = wk ? wk->d_counts.get() : nullptr;
     p.dist_all = d_dist_all;
+    p.dist_stride = dist_stride;
     p.bounds = balance ? wk->d_bounds.get() : nullptr;
     p.cta_time = balance ? wk->d_cta_time.get() : nullptr;
     Event *pev = nullptr;
@@ -1434,6 +1439,7 @@ int vsb_set_option(const char *name, int value) {
     else if (!strcmp(name, "xwait_ms")) p = &g_opt_xwait_ms;
     else if (!strcmp(name, "f32_batch")) p = &g_opt_f32_batch;
     else if (!strcmp(name, "sets_mem_mb")) p = &g_opt_sets_mem_mb;
+    else if (!strcmp(name, "grouped_mem_mb")) p = &g_opt_grouped_mem_mb;
     if (!p) return fail(VSB_EINVAL, "unknown option %s", name);
     if (value < 0) return fail(VSB_EINVAL, "option %s: values are non-negative", name);   // so that a negative return is always an error
     int old = *p;
@@ -1684,6 +1690,8 @@ int64_t vsb_index_stat(const vsb_index *ix, const char *name) {
     if (!strcmp(name, "grouped_regrows")) return ix->st_grouped_regrows;
     if (!strcmp(name, "grouped_layout_us")) return ix->st_grouped_layout_us;
     if (!strcmp(name, "grouped_layout_reuses")) return ix->st_grouped_layout_reuses;
+    if (!strcmp(name, "grouped_passes")) return ix->st_grouped_passes;
+    if (!strcmp(name, "grouped_pass_queries")) return ix->st_grouped_pass_queries;
     if (!strcmp(name, "grouped_scan_us")) return ix->st_grouped_scan_us;
     if (!strcmp(name, "grouped_walk_us")) return ix->st_grouped_walk_us;
     if (!strcmp(name, "grouped_replay_us")) return ix->st_grouped_replay_us;
@@ -1784,17 +1792,20 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
         memcpy(out, d.data(), n);
         return (int)n;
     }
-    else if (!strcmp(name, "grouped")) {                                // the layout and last query of the last grouped call
+    else if (!strcmp(name, "grouped") || !strcmp(name, "grouped_pass")) {
+        // "grouped": the layout and the last query of the last grouped call; "grouped_pass": the layout once, then every query of
+        // the call's last pass
         if (!ix->grouped || !ix->grouped->lay) return fail(VSB_EINVAL, "no grouped call has run yet");
         const GroupedShard &gs = *ix->grouped;
         const GroupedLayout &L = *gs.lay;
         const GroupedParams &p = gs.p;
-        const size_t npos = (size_t)L.npos, np = (size_t)L.npieces, nk = gs.kmin.size(), kk = (size_t)p.k;
+        const size_t npos = (size_t)L.npos, np = (size_t)L.npieces, nk = (size_t)L.nkeys, kk = (size_t)p.k;
         const size_t ndist = npos ? (size_t)ix->n : 0;
-        const long long head[7] = {(long long)npos, (long long)np, (long long)nk, (long long)kk, (long long)ndist, gs.ksel_used ? 1 : 0,
-                                   (long long)gs.pairs.size()};
-        std::vector<uint8_t> d(sizeof head);
-        memcpy(d.data(), head, sizeof head);
+        const bool pass = !strcmp(name, "grouped_pass");
+        const int q1 = std::max(gs.nq, 1), q0 = pass ? 0 : q1 - 1;
+        const auto cut = [&](int q) { return q < gs.nq && gs.cut.size() > (size_t)q && gs.cut[(size_t)q]; };
+        const auto npairs = [&](int q) { return q < gs.nq && gs.qoff.size() > (size_t)q + 1 ? gs.qoff[(size_t)q + 1] - gs.qoff[(size_t)q] : 0; };
+        std::vector<uint8_t> d;
         const auto host = [&](const void *src, size_t n) {
             d.insert(d.end(), (const uint8_t *)src, (const uint8_t *)src + n);
         };
@@ -1804,19 +1815,42 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
             if (n) CU(cudaMemcpy(d.data() + at, src, n, cudaMemcpyDeviceToHost));
             return (int)VSB_OK;
         };
-        host(L.h_rows.data(), 4 * npos);
-        host(L.koff.data(), 4 * (nk + 1));
-        int rc2 = dev(L.pstart, 4 * (np + 1));
-        if (rc2 == VSB_OK) rc2 = dev(L.pkey, 4 * np);
-        if (rc2 == VSB_OK) rc2 = dev(L.kpiece, 4 * (nk + 1));
-        if (rc2 == VSB_OK) rc2 = dev(gs.d_dist, 4 * ndist);
-        if (rc2 == VSB_OK) rc2 = dev(p.pd, 4 * npos);
-        if (rc2 == VSB_OK) rc2 = dev(p.lists, 4 * np * kk);
-        if (rc2 == VSB_OK) rc2 = dev(p.bound, 4 * np);
-        if (rc2) return rc2;
-        host(gs.kmin.data(), 4 * nk);
-        host(gs.pairs.data(), sizeof(uint2) * gs.pairs.size());
-        if (gs.ksel_used && (rc2 = dev(gs.d_ksel, nk))) return rc2;
+        if (pass) {
+            const long long head[6] = {(long long)npos, (long long)np, (long long)nk, (long long)kk, (long long)ndist, (long long)gs.nq};
+            host(head, sizeof head);
+        }
+        for (int q = q0; q < q1; ++q) {
+            if (!pass || q == 0) {
+                if (!pass) {
+                    const long long head[7] = {(long long)npos, (long long)np, (long long)nk, (long long)kk, (long long)ndist, cut(q) ? 1 : 0,
+                                               (long long)npairs(q)};
+                    host(head, sizeof head);
+                }
+                host(L.h_rows.data(), 4 * npos);
+                host(L.koff.data(), 4 * (nk + 1));
+                int rc2 = dev(L.pstart, 4 * (np + 1));
+                if (rc2 == VSB_OK) rc2 = dev(L.pkey, 4 * np);
+                if (rc2 == VSB_OK) rc2 = dev(L.kpiece, 4 * (nk + 1));
+                if (rc2) return rc2;
+            }
+            if (pass) {
+                const long long qhead[2] = {cut(q) ? 1 : 0, (long long)npairs(q)};
+                host(qhead, sizeof qhead);
+            }
+            const size_t qq = (size_t)q;
+            int rc2 = VSB_OK;
+            if (npos) {
+                rc2 = dev(gs.d_dist + qq * (size_t)p.sdist, 4 * ndist);
+                if (rc2 == VSB_OK) rc2 = dev(p.pd + qq * (size_t)p.spd, 4 * npos);
+                if (rc2 == VSB_OK) rc2 = dev(p.lists + qq * (size_t)p.slists, 4 * np * kk);
+                if (rc2 == VSB_OK) rc2 = dev(p.bound + qq * (size_t)p.sbound, 4 * np);
+                if (rc2) return rc2;
+            }
+            if (gs.kmin.size() >= (qq + 1) * nk) host(gs.kmin.data() + qq * nk, 4 * nk);
+            else d.resize(d.size() + 4 * nk, 0);
+            if (npairs(q)) host(gs.pairs.data() + gs.qoff[qq], sizeof(uint2) * npairs(q));
+            if (cut(q) && (rc2 = dev(gs.d_ksel + qq * (size_t)p.sksel, nk))) return rc2;
+        }
         const size_t n = std::min<size_t>({d.size(), (size_t)bytes, (size_t)INT32_MAX});
         memcpy(out, d.data(), n);
         return (int)n;
@@ -1831,9 +1865,11 @@ int vsb_debug_write(vsb_index *ix, const char *name, const void *data, int64_t b
     if (check_index(ix)) return VSB_EINVAL;
     if (!name || !data) return fail(VSB_EINVAL, "bad debug write arguments");
     if (!strcmp(name, "grouped_dist")) {       // the distances of every shard row for the next grouped call, instead of its scans
-        if (bytes != (int64_t)sizeof(float) * ix->n || ix->n == 0)
-            return fail(VSB_EINVAL, "grouped_dist: %lld bytes expected (float32 x %lld)", (long long)sizeof(float) * ix->n, ix->n);
-        ix->grouped_plant.assign((const float *)data, (const float *)data + ix->n);
+        // one row for every query of the call, or one row per query (query j: row j; the call checks the count)
+        const int64_t row = (int64_t)sizeof(float) * ix->n;
+        if (ix->n == 0 || bytes <= 0 || bytes % row != 0)
+            return fail(VSB_EINVAL, "grouped_dist: a multiple of %lld bytes expected (float32 x %lld per query)", (long long)row, ix->n);
+        ix->grouped_plant.assign((const float *)data, (const float *)data + bytes / (int64_t)sizeof(float));
         return VSB_OK;
     }
     if (strcmp(name, "bounds") != 0) return fail(VSB_EINVAL, "unknown debug buffer %s", name);

@@ -78,6 +78,8 @@ struct ScanParams {
     unsigned *range_count;
     long long range_cap;
     unsigned range_row_base;   // shard row of vec's first row, added to the rows written (the windows of a streamed index)
+    // a pass of M > 1 queries writes query m's distances at dist_all + m * dist_stride (an all-distances pass, k == 0)
+    long long dist_stride;
 };
 
 // query j's part of the pass workspaces (streams = scan CTAs x kWarps; the filter of query j gets the same offsets)
@@ -655,7 +657,13 @@ __device__ __forceinline__ void scan_body(const ScanParams &prm) {
             }
             continue;
         }
-        if (prm.dist_all != nullptr && valid && p == 0) prm.dist_all[row0 + r] = d[0];
+        if constexpr (M == 1) {
+            if (prm.dist_all != nullptr && valid && p == 0) prm.dist_all[row0 + r] = d[0];
+        } else if (prm.dist_all != nullptr && valid && p == 0) {
+#pragma unroll
+            for (int m = 0; m < M; ++m)
+                if (m < nq) prm.dist_all[(size_t)m * prm.dist_stride + row0 + r] = d[m];
+        }
         if (topk) {
 #pragma unroll
             for (int m = 0; m < M; ++m) {
@@ -989,17 +997,13 @@ __global__ void __launch_bounds__(kLkThreads) lk_count_kernel(const LkParams p) 
     }
 }
 
-// one block: the block counts become the positions their candidates start at, after the pairs of the earlier views (*total);
-// *total grows by this view's candidates
-__global__ void __launch_bounds__(kLkScanThreads, 1) lk_offsets_kernel(const LkParams p) {
-    __shared__ unsigned wsum[kLkScanThreads / 32];
-    __shared__ unsigned carry;
+// one block of kLkScanThreads: counts [0, n) become the positions their items start at, from carry (shared, set and synchronised
+// by the caller) on; carry ends as carry plus their sum
+__device__ __forceinline__ void block_offsets(unsigned *counts, int n, unsigned *wsum, unsigned &carry) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = *p.total;
-    __syncthreads();
-    for (int b0 = 0; b0 < p.nblocks; b0 += kLkScanThreads) {
+    for (int b0 = 0; b0 < n; b0 += kLkScanThreads) {
         const int i = b0 + (int)threadIdx.x;
-        const unsigned v = i < p.nblocks ? p.boff[i] : 0u;
+        const unsigned v = i < n ? counts[i] : 0u;
         unsigned incl = v;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
@@ -1019,11 +1023,21 @@ __global__ void __launch_bounds__(kLkScanThreads, 1) lk_offsets_kernel(const LkP
         }
         __syncthreads();
         const unsigned base = carry;
-        if (i < p.nblocks) p.boff[i] = base + (warp ? wsum[warp - 1] : 0u) + incl - v;
+        if (i < n) counts[i] = base + (warp ? wsum[warp - 1] : 0u) + incl - v;
         __syncthreads();
         if (threadIdx.x == 0) carry = base + wsum[kLkScanThreads / 32 - 1];
         __syncthreads();
     }
+}
+
+// one block: the block counts become the positions their candidates start at, after the pairs of the earlier views (*total);
+// *total grows by this view's candidates
+__global__ void __launch_bounds__(kLkScanThreads, 1) lk_offsets_kernel(const LkParams p) {
+    __shared__ unsigned wsum[kLkScanThreads / 32];
+    __shared__ unsigned carry;
+    if (threadIdx.x == 0) carry = *p.total;
+    __syncthreads();
+    block_offsets(p.boff, p.nblocks, wsum, carry);
     if (threadIdx.x == 0) *p.total = carry;
 }
 
@@ -1075,6 +1089,10 @@ __global__ void __launch_bounds__(kLkThreads) lk_write_kernel(const LkParams p) 
 //   earlier pieces of its key (+INF for the first), the key's minimum the smallest value of all of them (+INF: empty key).
 //   grouped_count_kernel, lk_offsets_kernel, grouped_write_kernel: the ordered compaction of the positions with pd < their
 //   piece's bound, of the selected keys only, into the pair list as (distance bits, position).
+// A pass of several queries runs each kernel once with blockIdx.y the query: query q's arrays start q strides in (the strides
+// below), and its pairs follow those of queries 0 .. q-1 in the one pair list.  Its offsets come from grouped_offsets_kernel,
+// one block per query, which also leaves each query's pair count in qcount; the write adds the counts of the earlier queries.
+// With one query (gridDim.y == 1) every offset is 0 and the kernels compute what the single-query sequence computes.
 constexpr int kGroupedPiece = 1024;  // positions of a piece
 constexpr int kGroupedWarps = 8;     // warps of a block: one piece or key each
 
@@ -1094,6 +1112,9 @@ struct GroupedParams {
     long long cap;
     long long npieces;
     int nkeys, k;
+    unsigned *qcount;                // a pass: [queries] pairs of each query (grouped_offsets_kernel); nullptr: one query
+    unsigned *total;                 // a pass: the pair list's counter (grouped_offsets_kernel adds every query's pairs)
+    long long sdist, spd, slists, sbound, skmin, sksel, spcount;   // per-query strides (elements) of the arrays above
 };
 
 // the k smallest values (k <= kcap, entries >= k of list hold -INF) of a warp's shared list, ascending, into out[0, k)
@@ -1114,10 +1135,12 @@ template <bool SMALL>
 __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_walk_kernel(const GroupedParams p) {
     __shared__ float sl[SMALL ? 1 : kGroupedWarps * 256];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp;
+    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp, q = blockIdx.y;
     if (pc >= p.npieces) return;
     const uint32_t a = p.pstart[pc], b = p.pstart[pc + 1];
     const int k = p.k, kcap = (k + 31) & ~31;
+    const float *dist = p.dist + q * p.sdist;
+    float *pd = p.pd + q * p.spd;
     SortedList L;
     float *list = sl + (SMALL ? 0 : warp * 256);
     float thr = INFINITY;
@@ -1132,7 +1155,7 @@ __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_walk_kernel(const 
     for (uint32_t c0 = a; c0 < b; c0 += 32) {
         const uint32_t at = c0 + (uint32_t)lane;
         const bool valid = at < b;
-        const float d = valid ? p.dist[p.rows[at]] : __int_as_float(0x7FC00000);
+        const float d = valid ? dist[p.rows[at]] : __int_as_float(0x7FC00000);
         unsigned msk = __ballot_sync(0xFFFFFFFFu, valid && d < (SMALL ? L.thr : thr));
         unsigned logged = 0u;
         while (msk) {
@@ -1151,9 +1174,9 @@ __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_walk_kernel(const 
                 logged |= 1u << src;
             }
         }
-        if (valid) p.pd[at] = ((logged >> lane) & 1u) ? d : __int_as_float(0x7FC00000);
+        if (valid) pd[at] = ((logged >> lane) & 1u) ? d : __int_as_float(0x7FC00000);
     }
-    float *out = p.lists + (size_t)pc * k;
+    float *out = p.lists + q * p.slists + (size_t)pc * k;
     if constexpr (SMALL) {
         if (lane < k) out[lane] = L.v;
     } else {
@@ -1171,6 +1194,8 @@ __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_bounds_kernel(cons
     if (g >= p.nkeys) return;
     const int k = p.k, kcap = (k + 31) & ~31;
     const uint32_t q0 = p.kpiece[g], q1 = p.kpiece[g + 1];
+    const float *lists = p.lists + blockIdx.y * p.slists;
+    float *bound = p.bound + blockIdx.y * p.sbound;
     SortedList L;
     float *list = sl + (SMALL ? 0 : warp * 256);
     float thr = INFINITY, mn = INFINITY;
@@ -1183,8 +1208,8 @@ __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_bounds_kernel(cons
         list_argmax(list, kcap, lane, thr, pos);
     }
     for (uint32_t pc = q0; pc < q1; ++pc) {
-        const float *src = p.lists + (size_t)pc * k;
-        if (lane == 0) p.bound[pc] = SMALL ? L.thr : thr;
+        const float *src = lists + (size_t)pc * k;
+        if (lane == 0) bound[pc] = SMALL ? L.thr : thr;
         mn = fminf(mn, src[0]);
         if constexpr (SMALL) {
             L.offer_sorted(lane, lane < k ? src[lane] : INFINITY);
@@ -1207,40 +1232,58 @@ __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_bounds_kernel(cons
             }
         }
     }
-    if (lane == 0) p.kmin[g] = mn;
+    if (lane == 0) p.kmin[blockIdx.y * p.skmin + g] = mn;
 }
 
-__device__ __forceinline__ bool grouped_selected(const GroupedParams &p, long long pc) {
-    return p.ksel == nullptr || p.ksel[p.pkey[pc]] != 0;
+// query q's selection of the piece's key
+__device__ __forceinline__ bool grouped_selected(const GroupedParams &p, long long q, long long pc) {
+    return p.ksel == nullptr || p.ksel[q * p.sksel + p.pkey[pc]] != 0;
 }
 
 // one warp per piece: its survivors
 __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_count_kernel(const GroupedParams p) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp;
+    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp, q = blockIdx.y;
     if (pc >= p.npieces) return;
     unsigned c = 0;
-    if (grouped_selected(p, pc)) {
+    if (grouped_selected(p, q, pc)) {
         const uint32_t a = p.pstart[pc], b = p.pstart[pc + 1];
-        const float bd = p.bound[pc];
-        for (uint32_t at = a + (uint32_t)lane; at < b; at += 32) c += p.pd[at] < bd ? 1u : 0u;
+        const float bd = p.bound[q * p.sbound + pc];
+        const float *pd = p.pd + q * p.spd;
+        for (uint32_t at = a + (uint32_t)lane; at < b; at += 32) c += pd[at] < bd ? 1u : 0u;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, o);
     }
-    if (lane == 0) p.pcount[pc] = c;
+    if (lane == 0) p.pcount[q * p.spcount + pc] = c;
+}
+
+// a pass: one block per query places its pieces' survivors from 0 on (the write adds the earlier queries' pairs), leaves the
+// query's count in qcount and adds it to the pair list's counter
+__global__ void __launch_bounds__(kLkScanThreads, 1) grouped_offsets_kernel(const GroupedParams p) {
+    __shared__ unsigned wsum[kLkScanThreads / 32];
+    __shared__ unsigned carry;
+    if (threadIdx.x == 0) carry = 0u;
+    __syncthreads();
+    block_offsets(p.pcount + blockIdx.x * p.spcount, (int)p.npieces, wsum, carry);
+    if (threadIdx.x == 0) {
+        p.qcount[blockIdx.x] = carry;
+        atomicAdd(p.total, carry);
+    }
 }
 
 // one warp per piece: its survivors in position order from the piece's offset on
 __global__ void __launch_bounds__(kGroupedWarps * 32) grouped_write_kernel(const GroupedParams p) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp;
-    if (pc >= p.npieces || !grouped_selected(p, pc)) return;
+    const long long pc = (long long)blockIdx.x * kGroupedWarps + warp, q = blockIdx.y;
+    if (pc >= p.npieces || !grouped_selected(p, q, pc)) return;
     const uint32_t a = p.pstart[pc], b = p.pstart[pc + 1];
-    const float bd = p.bound[pc];
-    unsigned w = p.pcount[pc];
+    const float bd = p.bound[q * p.sbound + pc];
+    const float *pd = p.pd + q * p.spd;
+    unsigned w = p.pcount[q * p.spcount + pc];
+    for (long long j = 0; j < q; ++j) w += p.qcount[j];
     for (uint32_t c0 = a; c0 < b; c0 += 32) {
         const uint32_t at = c0 + (uint32_t)lane;
-        const float d = at < b ? p.pd[at] : __int_as_float(0x7FC00000);
+        const float d = at < b ? pd[at] : __int_as_float(0x7FC00000);
         const bool hit = d < bd;
         const unsigned m = __ballot_sync(0xFFFFFFFFu, hit);
         const unsigned o = w + (unsigned)__popc(m & ((1u << lane) - 1u));

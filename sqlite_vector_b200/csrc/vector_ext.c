@@ -44,7 +44,7 @@ const sqlite3_api_routines *vsq_api = 0;
 
 /* the hidden columns every table-valued function starts with (src/sqlite-vector.c:98-103, :1830) */
 enum { COL_TBL = 0, COL_VECTOR = 1, COL_K = 2, COL_MEMIDX = 3 };
-#define N_MODULES 20                           /* rows of `modules`, the table-valued functions */
+#define N_MODULES 22                           /* rows of `modules`, the table-valued functions */
 
 /* ------------------------------------------------------------------------------------------------ state */
 /* the grouping of the most recent vector_*_scan_grouped statement on one staged column, with that statement's groups BLOB and its
@@ -94,13 +94,14 @@ typedef struct {
 } scan_vtab;
 
 /* a result is ngroups groups of rows: group g has count[g] rows at ids / dist + g * stride and, for grouped scans, the key
- * key[g].  One group for the one-query modules, one per query for the many-query modules, one per returned key for grouped. */
+ * key[g] of query query[g].  One group for the one-query modules, one per query for the many-query modules, one per returned key
+ * (of every query) for grouped. */
 typedef struct {
     sqlite3_vtab_cursor base;
     int64_t *ids;
     double *dist;
     float *fdist;                  /* a stream's distances, in place of dist: every row of the column is one result row */
-    sqlite3_int64 *count, *key;
+    sqlite3_int64 *count, *key, *query;
     sqlite3_int64 ngroups, stride;
     sqlite3_int64 g, j;            /* the current row: row j of group g; a stream starts at j = -1, the reference's (0, 0.0) row */
     int max_index;                 /* carried from one xFilter to the next, as the reference's cursor does (:1808-1813) */
@@ -1180,6 +1181,13 @@ static int stage_full_column(scan_vtab *vt, vcolumn *v) {
  *   whose groups BLOB is byte for byte the kept one, on the same staged column, skips the decoding of the BLOB and the layout.
  *   Anything else lays the keys out anew and replaces the kept grouping; re-staging the column (a changed table, data_version,
  *   or a copy staged inside a transaction) and closing the connection free it.  The rows returned are the same either way.
+ * vector_*_scan_grouped_batch(tbl, col, vectors, k, groups, limit): B queries of vector_*_scan_grouped in one call, `vectors` as
+ *   for vector_*_scan_batch.  Rows are (query, key, id, distance): query b's rows are exactly those vector_*_scan_grouped returns
+ *   for vector b, queries in order.  The queries share each pass of the column (DESIGN §3.15); k = 0 returns no rows.  The two
+ *   batch modules share the kept grouping of the column with the single ones: a repeated groups BLOB skips the layout whichever
+ *   of them ran last.  Arguments are checked as for every module (test_sql_modules_host.py): the count, each argument in
+ *   position order (k >= 0, the groups BLOB a whole number of pairs, limit >= 0), the context, the vectors, the quantization
+ *   table and staging.
  * vector_*_scan_range(tbl, col, vector, radius) and the *_range_filtered twins (+ rowids): every row with distance < radius,
  *   ordered by distance, equal distances in scan order (vsb_group_scan_range).  The reference answers this only as
  *   SELECT id, distance FROM vector_*_scan_stream(...) WHERE distance < radius ORDER BY distance: the same rows, here without a
@@ -1220,6 +1228,8 @@ static const module_def modules[] = {
     {"vector_quantize_scan_batch_sets", SCHEMA("sets hidden, query_sets hidden, query, id, distance"), 1, 1, {ARG_SETS, ARG_QUERY_SETS}, OP_SETS},
     {"vector_full_scan_grouped", SCHEMA("groups hidden, \"limit\" hidden, key, id, distance"), 0, 0, {ARG_GROUPS, ARG_LIMIT}, OP_GROUPED},
     {"vector_quantize_scan_grouped", SCHEMA("groups hidden, \"limit\" hidden, key, id, distance"), 1, 0, {ARG_GROUPS, ARG_LIMIT}, OP_GROUPED},
+    {"vector_full_scan_grouped_batch", SCHEMA("groups hidden, \"limit\" hidden, query, key, id, distance"), 0, 1, {ARG_GROUPS, ARG_LIMIT}, OP_GROUPED},
+    {"vector_quantize_scan_grouped_batch", SCHEMA("groups hidden, \"limit\" hidden, query, key, id, distance"), 1, 1, {ARG_GROUPS, ARG_LIMIT}, OP_GROUPED},
     {"vector_full_scan_range", SCHEMA("id, distance"), 0, 0, {ARG_NONE}, OP_RANGE},
     {"vector_quantize_scan_range", SCHEMA("id, distance"), 1, 0, {ARG_NONE}, OP_RANGE},
     {"vector_full_scan_range_filtered", SCHEMA("rowids hidden, id, distance"), 0, 0, {ARG_ROWIDS}, OP_RANGE},
@@ -1233,6 +1243,8 @@ _Static_assert(sizeof modules / sizeof modules[0] == N_MODULES, "N_MODULES count
 static int nhidden(const module_def *m) { return (m->hidden[0] != ARG_NONE) + (m->hidden[1] != ARG_NONE); }
 /* many-query and grouped results lead each row with its query or key, and number the rows by their position in the result */
 static int leads_group(const module_def *m) { return m->many || m->op == OP_GROUPED; }
+/* the columns before id: query and / or key (the batch grouped modules lead with both) */
+static int lead_columns(const module_def *m) { return leads_group(m) + (m->many && m->op == OP_GROUPED); }
 
 static int vt_connect(sqlite3 *db, void *aux, int argc, const char *const *argv, sqlite3_vtab **out, char **err) { /* :1828-1842 */
     (void)argc; (void)argv; (void)err;
@@ -1287,14 +1299,16 @@ static int vt_open(sqlite3_vtab *t, sqlite3_vtab_cursor **out) {
 }
 static void cursor_free_result(scan_cursor *c) {
     sqlite3_free(c->ids); sqlite3_free(c->dist); sqlite3_free(c->fdist); sqlite3_free(c->count); sqlite3_free(c->key);
-    c->ids = 0; c->dist = 0; c->fdist = 0; c->count = 0; c->key = 0;
+    sqlite3_free(c->query);
+    c->ids = 0; c->dist = 0; c->fdist = 0; c->count = 0; c->key = 0; c->query = 0;
 }
 static int vt_close(sqlite3_vtab_cursor *cur) {
     cursor_free_result((scan_cursor *)cur);
     sqlite3_free(cur);
     return SQLITE_OK;
 }
-/* the cursor's result arrays for `groups` groups of up to `stride` rows: float distances for a stream, a key per group for grouped */
+/* the cursor's result arrays for `groups` groups of up to `stride` rows: float distances for a stream, a key and a query per group
+ * for grouped */
 static int cursor_alloc(scan_cursor *c, sqlite3_int64 groups, sqlite3_int64 stride, int op) {
     const sqlite3_uint64 ng = (sqlite3_uint64)(groups > 0 ? groups : 1), nr = ng * (sqlite3_uint64)(stride > 0 ? stride : 1);
     cursor_free_result(c);
@@ -1302,9 +1316,12 @@ static int cursor_alloc(scan_cursor *c, sqlite3_int64 groups, sqlite3_int64 stri
     if (op == OP_STREAM) c->fdist = (float *)sqlite3_malloc64(nr * sizeof(float));
     else c->dist = (double *)sqlite3_malloc64(nr * sizeof(double));
     c->count = (sqlite3_int64 *)sqlite3_malloc64(ng * sizeof(sqlite3_int64));
-    if (op == OP_GROUPED) c->key = (sqlite3_int64 *)sqlite3_malloc64(ng * sizeof(sqlite3_int64));
+    if (op == OP_GROUPED) {
+        c->key = (sqlite3_int64 *)sqlite3_malloc64(ng * sizeof(sqlite3_int64));
+        c->query = (sqlite3_int64 *)sqlite3_malloc64(ng * sizeof(sqlite3_int64));
+    }
     c->stride = stride;
-    return c->ids && (c->dist || c->fdist) && c->count && (c->key || op != OP_GROUPED) ? SQLITE_OK : SQLITE_NOMEM;
+    return c->ids && (c->dist || c->fdist) && c->count && ((c->key && c->query) || op != OP_GROUPED) ? SQLITE_OK : SQLITE_NOMEM;
 }
 static void skip_empty(scan_cursor *c) {
     while (c->g < c->ngroups && c->j >= c->count[c->g]) { ++c->g; c->j = 0; }
@@ -1324,8 +1341,9 @@ static int vt_column(sqlite3_vtab_cursor *cur, sqlite3_context *ctx, int col) { 
     const scan_cursor *c = (const scan_cursor *)cur;
     const module_def *m = ((scan_vtab *)cur->pVtab)->def;
     const sqlite3_int64 at = c->g * c->stride + c->j;
-    const int first = COL_MEMIDX + 1 + nhidden(m), lead = leads_group(m);     /* the visible columns: [query | key,] id, distance */
-    if (lead && col == first) sqlite3_result_int64(ctx, c->key ? c->key[c->g] : c->g);
+    const int first = COL_MEMIDX + 1 + nhidden(m), lead = lead_columns(m);   /* the visible columns: [query,] [key,] id, distance */
+    if (lead == 2 && col == first) sqlite3_result_int64(ctx, c->query[c->g]);
+    else if (lead && col == first + lead - 1) sqlite3_result_int64(ctx, c->key ? c->key[c->g] : c->g);
     else if (col == first + lead) sqlite3_result_int64(ctx, cur_id(c));
     else if (col == first + lead + 1) sqlite3_result_double(ctx, c->j < 0 ? 0.0 : c->fdist ? (double)c->fdist[at] : c->dist[at]);
     return SQLITE_OK;
@@ -1652,22 +1670,35 @@ static int vt_filter(sqlite3_vtab_cursor *cur, int idxnum, const char *idxstr, i
             kept->keys = runs.keys;                                     /* dense key index -> user key */
             runs.keys = 0;
         }
-        src = vsb_scan_topk_grouping(kept->gr, metric, q.query, 1, k, limit, &res);
+        src = vsb_scan_topk_grouping(kept->gr, metric, q.query, nq, k, limit, &res);
         if (src != VSB_OK) break;
-        int nk = 0;
-        const int32_t *gk = 0;
-        const int64_t *go = 0, *gi = 0;
-        const double *gd = 0;
-        vsb_grouped_get(res, 0, &nk, &gk, &go, &gi, &gd);
-        if ((rc = cursor_alloc(c, nk, k, m->op)) != SQLITE_OK) goto out;
-        for (int i = 0; i < nk; ++i) {
-            const sqlite3_int64 n = go[i + 1] - go[i];
-            c->count[i] = n;
-            c->key[i] = kept->keys[gk[i]];
-            memcpy(c->ids + (size_t)i * k, gi + go[i], (size_t)n * sizeof(int64_t));
-            memcpy(c->dist + (size_t)i * k, gd + go[i], (size_t)n * sizeof(double));
+        sqlite3_int64 total = 0;                                        /* every query's keys, one group each */
+        for (int b = 0; b < nq; ++b) {
+            int nk = 0;
+            const int32_t *gk = 0;
+            const int64_t *go = 0, *gi = 0;
+            const double *gd = 0;
+            vsb_grouped_get(res, b, &nk, &gk, &go, &gi, &gd);
+            total += nk;
         }
-        ngroups = nk;
+        if ((rc = cursor_alloc(c, total, k, m->op)) != SQLITE_OK) goto out;
+        sqlite3_int64 i = 0;
+        for (int b = 0; b < nq; ++b) {
+            int nk = 0;
+            const int32_t *gk = 0;
+            const int64_t *go = 0, *gi = 0;
+            const double *gd = 0;
+            vsb_grouped_get(res, b, &nk, &gk, &go, &gi, &gd);
+            for (int t = 0; t < nk; ++t, ++i) {
+                const sqlite3_int64 n = go[t + 1] - go[t];
+                c->count[i] = n;
+                c->key[i] = kept->keys[gk[t]];
+                c->query[i] = b;
+                memcpy(c->ids + (size_t)i * k, gi + go[t], (size_t)n * sizeof(int64_t));
+                memcpy(c->dist + (size_t)i * k, gd + go[t], (size_t)n * sizeof(double));
+            }
+        }
+        ngroups = total;
         break;
     }
     case OP_RERANK: {

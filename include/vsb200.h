@@ -427,7 +427,14 @@ VSB_API int vsb_profile_read(vsb_index *ix, double *scan_ms, int *scan_launches,
  * survivors (distance bits, position) in position order, and with S = 1 uint8 ksel [G] (1: the key was compacted))},
  * "grouped_pass" (the same shard's state for every query of the last pass of that call: int64 [6] {P, N, G, k, D, W queries},
  * the layout arrays rows, koff, pstart, pkey, kpiece as for "grouped", then per query int64 [2] {S, C} and dist [D], pd [P],
- * lists [N][k], bound [N], kmin [G], the C survivor pairs and with S = 1 ksel [G]).  Returns the bytes copied or < 0. */
+ * lists [N][k], bound [N], kmin [G], the C survivor pairs and with S = 1 ksel [G]), "sets_plan" (the level plan of the most
+ * recent vsb_scan_topk_sets or group sets call on this shard that reached its plan, kept also when the call then answered set by
+ * set (DESIGN §3.14): int64 [10] {T tiles, V views, m0, growth, over (1: a view needed more than 256 levels; no levels and
+ * pairs0 0 then), pairs0, S sets (the distinct sets the queries name, in order of first use), W words per set, L levels in
+ * all, D (1: the bitmaps follow)}, then int64 tb [T + 1] (tile bounds in shard rows), vt [V + 1] (view v: tiles [vt[v],
+ * vt[v + 1])), nlev [V], ends [L] (each level's end tile, view after view), and with D = 1 (option "sets_debug" was 1 during
+ * the call) uint32 sets [S][W] (the shard's cut of each set), union [W], prefix [S][T + 1] (each set's rows before each
+ * tile)).  Returns the bytes copied or < 0. */
 VSB_API int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes);
 /* diagnostics: the counterpart of vsb_debug_read for name "bounds": plants a row partition (int64 tile boundaries, one per scan
  * CTA plus one, non-decreasing from 0 to the tile count of the k <= 32 plan; vsb_index_stat "sms" CTAs) into every scan
@@ -455,6 +462,17 @@ VSB_API int64_t vsb_debug_survivors(vsb_index *ix, int slot, uint32_t *out_pairs
  * int; left untouched for L1) may be NULL.  Synchronous. */
 VSB_API int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1,
                                int N, int mode, void *out, int64_t out_cap, void *out_qc, void *out_norms, int64_t *out_count);
+/* diagnostics: vsb_debug_tc_level (mode 0) under a row filter or per-query sets, as a level of a filtered or sets batch runs:
+ * row r of the index is bit allow_base + r of bitmaps of nbits bits (allow_base >= 0, allow_base + r1 <= nbits).  allow: one
+ * row bitmap (the filter of vsb_scan_topk_filtered), or NULL; sets (with allow NULL): nsets bitmaps of words_of(nbits) words
+ * back to back and set_of_query[nq], query q seeing only the rows of set set_of_query[q], their union the row filter (as
+ * vsb_scan_topk_sets).  level0 != 0: level 0 instead of a scorer level, rows [0, r1) with r0 = 0: every (row, query) pair of
+ * the eligible rows (all_pairs_kernel), or with sets each row's pairs with the queries whose set holds it (sets_pairs_kernel);
+ * U is then unused, and a level of more than 16 Mi pairs returns VSB_ERANGE.  Synchronous. */
+VSB_API int vsb_debug_tc_level_filtered(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1,
+                                        int N, int level0, const uint32_t *allow, int64_t allow_base, int64_t nbits, const uint32_t *sets,
+                                        int nsets, const int32_t *set_of_query, void *out, int64_t out_cap, void *out_qc, void *out_norms,
+                                        int64_t *out_count);
 /* diagnostics: ONE launch of the batch path's exact refinement (refine_kernel, production grid) over npairs (row, query) uint32
  * pairs given by the caller (at most 16 Mi; only the first cand_cap are refined, like a truncated candidate log), with the
  * per-query bounds U[nq] (kept when distance < U).  out_bucket: nq x 2048 (row, distance bits) uint32 pairs, each query's
@@ -472,7 +490,8 @@ VSB_API int vsb_debug_refine(vsb_index *ix, int metric, const void *queries, int
 VSB_API int vsb_debug_replay(vsb_index *ix, int metric, const void *queries, int nq, int k, int level0, const uint32_t *bucket,
                              const uint32_t *bcount, float *slot_d, uint32_t *slot_row, int *slot_mi, int acc_cap, uint32_t *acc_log,
                              int *acc_count, int final_sort, float *out_U, uint32_t *out_qc, uint32_t *out_bcount, uint32_t *out_stats);
-/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","scan_streams","xwait_ms","epi_chunk","f32_batch","sets_mem_mb","grouped_mem_mb"};
+/* tuning knobs for experiments: name in {"stage_bytes","direct","ring_bytes","time_kernels","no_batch","batch_debug","batch_m0","batch_growth","balance","scan_streams","xwait_ms","epi_chunk","f32_batch","sets_mem_mb","grouped_mem_mb","sets_debug"};
+ * "sets_debug" = 1: sets calls also keep their bitmaps, union and prefix counts for vsb_debug_read "sets_plan" (default 0);
  * "f32_batch" = 1: f32 columns batch L2 / cosine / dot queries on the tensor cores in TF32 (default 0, or VSB_F32_BATCH=1 in the
  * environment when the library loads; per process).  Values are non-negative; returns the previous value, or a negative VSB_E* code (unknown name, negative value) */
 VSB_API int vsb_set_option(const char *name, int value);

@@ -116,6 +116,8 @@ _SIGNATURES = {
     "vsb_debug_write": (_i, [_vp, C.c_char_p, _vp, _i64]),
     "vsb_debug_survivors": (_i64, [_vp, _i, _vp, _i64, C.POINTER(_i)]),
     "vsb_debug_tc_level": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i64, _i, _i, _vp, _i64, _vp, _vp, C.POINTER(_i64)]),
+    "vsb_debug_tc_level_filtered": (_i, [_vp, _i, _vp, _i, _vp, _i64, _i64, _i, _i, _vp, _i64, _i64, _vp, _i, _vp, _vp, _i64, _vp, _vp,
+                                         C.POINTER(_i64)]),
     "vsb_debug_refine": (_i, [_vp, _i, _vp, _i, _vp, _i64, _vp, _i64, _vp, _vp, _vp]),
     "vsb_debug_replay": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
 }
@@ -649,16 +651,23 @@ class Index(_Column):
         return pairs[:n].copy(), flags.value
 
     def debug_tc_level(self, metric: int, queries: np.ndarray, U: np.ndarray, r0: int, r1: int, N: int = 0, scores: bool = False,
-                       cap: int = 1 << 22):
+                       cap: int = 1 << 22, allow=None, allow_base: int = 0, sets=None, set_of_query=None, level0: bool = False):
         """one tensor-core level of the batch path over rows [r0, r1) with the per-query bounds U (vsb_debug_tc_level; metric
         L1: one level of the CUDA-core L1 batch kernel, any column type).
         scores=False: {"log": (row, query) uint32 pairs, "count": hits counted (> len(log) when truncated at cap),
         "qc": uint32 bits [nq], "norms": row sums of squares [r1 - r0] (zeros for L1)}; scores=True: the same with "scores"
-        [r1 - r0, nq] (int32 for int8 / uint8, float32 for f32 / f16 / bf16) instead of the log"""
+        [r1 - r0, nq] (int32 for int8 / uint8, float32 for f32 / f16 / bf16) instead of the log.
+        allow / sets / level0 (vsb_debug_tc_level_filtered, the log only): the level as a filtered or sets batch runs it, row r
+        being bit allow_base + r.  allow: a boolean mask or uint32 bitmap; sets: boolean masks of one length or a uint32 array
+        [nsets, words], set_of_query[q] query q's set (their union is the row filter); level0: level 0 over rows [0, r1) (r0 = 0,
+        U unused) instead of a scorer level"""
         q2 = np.ascontiguousarray(queries).reshape(-1, queries.shape[-1])
         nq = q2.shape[0]
         u = np.ascontiguousarray(U, dtype=np.float32)
         assert u.shape == (nq,)
+        if allow is not None or sets is not None or level0:
+            assert not scores, "a filtered level returns its log"
+            return self._debug_tc_level_filtered(metric, q2, u, r0, r1, N, cap, allow, allow_base, sets, set_of_query, level0)
         integer = self.vtype in (U8, I8)
         qc = np.zeros(nq, dtype=np.uint32)
         norms = np.zeros(r1 - r0, dtype=np.int32 if integer else np.float32)
@@ -676,6 +685,57 @@ class Index(_Column):
         else:
             res["log"] = out[: min(int(count.value), cap)].copy()
         return res
+
+    def _debug_tc_level_filtered(self, metric, q2, u, r0, r1, N, cap, allow, allow_base, sets, set_of_query, level0):
+        nq = q2.shape[0]
+        bits, nbits, flat, nsets, soq = None, 0, None, 0, None
+        if allow is not None:
+            a = np.asarray(allow)
+            bits = row_bitmap(a) if a.dtype == bool else np.ascontiguousarray(a, dtype=np.uint32)
+            nbits = len(a) if a.dtype == bool else 32 * bits.size
+        if sets is not None:
+            if isinstance(sets, np.ndarray) and sets.dtype == np.uint32 and sets.ndim == 2:
+                flat, nbits = np.ascontiguousarray(sets), 32 * sets.shape[1]
+            else:
+                nbits = len(sets[0])
+                flat = np.stack([row_bitmap(np.asarray(m, bool)) for m in sets])
+            nsets = flat.shape[0]
+            soq = np.ascontiguousarray(set_of_query, dtype=np.int32)
+            assert soq.shape == (nq,)
+        if allow is None and sets is None:
+            nbits = allow_base + r1
+        integer = self.vtype in (U8, I8)
+        qc = np.zeros(nq, dtype=np.uint32)
+        norms = np.zeros(r1 - r0, dtype=np.int32 if integer else np.float32)
+        count = _i64()
+        out = np.zeros((cap, 2), dtype=np.uint32)
+        self.eng.check(self.eng.lib.vsb_debug_tc_level_filtered(self.h, metric, _ptr(q2), nq, _ptr(u), r0, r1, N, int(level0), _ptr(bits),
+                                                                allow_base, nbits, _ptr(flat), nsets, _ptr(soq), _ptr(out), cap, _ptr(qc),
+                                                                _ptr(norms), C.byref(count)))
+        return {"count": int(count.value), "qc": qc, "norms": norms, "log": out[: min(int(count.value), cap)].copy()}
+
+    def debug_sets_plan(self) -> dict:
+        """the level plan of this shard's most recent sets call (vsb_debug_read "sets_plan"): "tb", "vt", "nlev" and "ends" (one
+        int64 array of level end tiles per view), "m0", "growth", "over", "pairs0", "nsets", "words"; with option sets_debug on
+        during the call also "sets" (uint32 [nsets, words], this shard's cut of each set the queries name, in order of first use),
+        "union" [words] and "prefix" (uint32 [nsets, T + 1]), else None"""
+        head = self.debug_read("sets_plan", np.int64, 10)
+        T, V, m0, growth, over, pairs0, S, W, L, D = (int(v) for v in head)
+        n64 = 10 + (T + 1) + (V + 1) + V + L
+        raw = self.debug_read("sets_plan", np.uint8, 8 * n64 + (4 * (S * W + W + S * (T + 1)) if D else 0))
+        i64 = raw[: 8 * n64].view("<i8")
+        at = 10
+        tb, vt, nlev = i64[at:at + T + 1].copy(), i64[at + T + 1:at + T + V + 2].copy(), i64[at + T + V + 2:at + T + 2 * V + 2].copy()
+        flat = i64[at + T + 2 * V + 2:].copy()
+        cut = np.concatenate([[0], np.cumsum(nlev)]).astype(np.int64)
+        out = {"tb": tb, "vt": vt, "nlev": nlev, "ends": [flat[cut[v]:cut[v + 1]] for v in range(V)], "m0": m0, "growth": growth,
+               "over": bool(over), "pairs0": pairs0, "nsets": S, "words": W, "sets": None, "union": None, "prefix": None}
+        if D:
+            u4 = raw[8 * n64:].view("<u4")
+            out["sets"] = u4[:S * W].reshape(S, W).copy()
+            out["union"] = u4[S * W:S * W + W].copy()
+            out["prefix"] = u4[S * W + W:].reshape(S, T + 1).copy()
+        return out
 
     def debug_refine(self, metric: int, queries: np.ndarray, pairs: np.ndarray, U: np.ndarray, cand_cap: int | None = None):
         """one launch of the batch path's exact refinement over (row, query) pairs [npairs, 2] with the bounds U

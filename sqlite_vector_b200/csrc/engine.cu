@@ -57,6 +57,7 @@ int g_opt_f32_batch = [] {
     return (e && atoi(e) > 0) ? 1 : 0;
 }();
 int g_opt_sets_mem_mb = 0;     // vsb_scan_topk_sets: device memory its one-pass buffers may take, in MB (0: 1/8 of the free memory)
+int g_opt_sets_debug = 0;      // 1: sets calls also keep their bitmaps, union and prefix counts for vsb_debug_read "sets_plan"
 int g_opt_grouped_mem_mb = 0;  // grouped top-k: device memory the per-query areas of a pass may take, in MB (0: 1/8 of the free memory)
 int g_opt_xwait_ms = 10000;    // exchange: how long the receiving side waits for a peer's head before it reports an error (a dead
                                // peer, not a slow one: ranks sharing one GPU or a busy host can start a batch seconds apart)
@@ -180,6 +181,7 @@ struct HeldPass {
 
 struct BatchWs;   // batch_host.inc
 struct SetsState;   // batch_host.inc
+struct SetsPlan;    // batch_host.inc
 struct GroupedShard;   // batch_host.inc
 void groupings_detach(std::vector<vsb_grouping *> &list);   // column.inc
 
@@ -276,6 +278,8 @@ struct vsb_index {
     // null outside such a call
     const SetsState *sets = nullptr;
     long long st_sets_batches = 0, st_sets_fallbacks = 0, st_sets_levels = 0, st_sets_plan_us = 0;
+    // the plan of the most recent sets call that reached it (vsb_debug_read "sets_plan"), kept until the next one
+    std::unique_ptr<SetsPlan> sets_plan;
     // grouped top-k (vsb_scan_topk_grouped, DESIGN §3.15): one device area for the per-query arrays of a call, and a streamed
     // index's distances of every window (4 bytes per row), both grown never shrunk
     DeviceBuf<uint8_t> d_grouped;
@@ -1440,6 +1444,7 @@ int vsb_set_option(const char *name, int value) {
     else if (!strcmp(name, "f32_batch")) p = &g_opt_f32_batch;
     else if (!strcmp(name, "sets_mem_mb")) p = &g_opt_sets_mem_mb;
     else if (!strcmp(name, "grouped_mem_mb")) p = &g_opt_grouped_mem_mb;
+    else if (!strcmp(name, "sets_debug")) p = &g_opt_sets_debug;
     if (!p) return fail(VSB_EINVAL, "unknown option %s", name);
     if (value < 0) return fail(VSB_EINVAL, "option %s: values are non-negative", name);   // so that a negative return is always an error
     int old = *p;
@@ -1855,6 +1860,13 @@ int vsb_debug_read(vsb_index *ix, const char *name, void *out, int64_t bytes) {
         memcpy(out, d.data(), n);
         return (int)n;
     }
+    else if (!strcmp(name, "sets_plan")) {
+        if (!ix->sets_plan) return fail(VSB_EINVAL, "no sets call has planned its levels yet");
+        const std::vector<uint8_t> d = sets_plan_bytes(*ix->sets_plan);
+        const size_t n = std::min<size_t>({d.size(), (size_t)bytes, (size_t)INT32_MAX});
+        memcpy(out, d.data(), n);
+        return (int)n;
+    }
     else return fail(VSB_EINVAL, "unknown debug buffer %s", name);
     if (!src) return fail(VSB_EINVAL, "no %s has run yet", strcmp(name, "topk_bounds") ? "scan" : "large-k query");
     CU(cudaMemcpy(out, src, std::min<size_t>(have, (size_t)bytes), cudaMemcpyDeviceToHost));
@@ -1924,6 +1936,18 @@ int vsb_debug_tc_level(vsb_index *ix, int metric, const void *queries, int nq, c
     if (check_index(ix)) return VSB_EINVAL;
     long long cnt = 0;
     const int rc = batch_tc_level(ix, metric, queries, nq, U, r0, r1, N, mode, out, out_cap, out_qc, out_norms, &cnt);
+    if (rc == VSB_OK && out_count) *out_count = cnt;
+    return rc;
+}
+
+int vsb_debug_tc_level_filtered(vsb_index *ix, int metric, const void *queries, int nq, const float *U, int64_t r0, int64_t r1,
+                                int N, int level0, const uint32_t *allow, int64_t allow_base, int64_t nbits, const uint32_t *sets,
+                                int nsets, const int32_t *set_of_query, void *out, int64_t out_cap, void *out_qc, void *out_norms,
+                                int64_t *out_count) {
+    if (check_index(ix)) return VSB_EINVAL;
+    const LevelFilter f{allow, sets, nsets, set_of_query, nbits, allow_base, level0 != 0};
+    long long cnt = 0;
+    const int rc = batch_tc_level(ix, metric, queries, nq, U, r0, r1, N, 0, out, out_cap, out_qc, out_norms, &cnt, &f);
     if (rc == VSB_OK && out_count) *out_count = cnt;
     return rc;
 }
